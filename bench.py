@@ -1,7 +1,7 @@
 #!/usr/bin/env python
 """bench.py — MD steps/s of the non-bonded + VelocityVerlet hot path (BASELINE.json metric).
 
-    python bench.py [--gpus N] [--steps K] [--warmup W] [--impl ours|reference] [--workload c2|c3]
+    python bench.py [--gpus N] [--steps K] [--warmup W] [--impl ours|reference] [--workload c2|c3] [--dump-outputs DIR]
 
 A "step" is one VelocityVerlet MD step (kick, drift, neighbour policy, pairwise forces, kick, CM removal)
 of the workload; at N=1 the workload is BASELINE config[1]: the 256 000-atom argon LJ fluid, cubic PBC,
@@ -80,7 +80,7 @@ def workload(name: str, dtype):
 
 # ----------------------------------------------------------------------------------------------------
 class ClockSampler:
-    """nvidia-smi clocks / throttle reasons sampled during the timed region (B200_PROFILING.md)."""
+    """nvidia-smi clocks / throttle reasons sampled during the timed region."""
     Q = ("clocks.sm,clocks.max.sm,power.draw,clocks_event_reasons.hw_slowdown,clocks_event_reasons.hw_thermal_slowdown,"
          "clocks_event_reasons.sw_thermal_slowdown,clocks_event_reasons.sw_power_cap")
 
@@ -131,8 +131,9 @@ class ClockSampler:
 
 
 def default_r_list(wl, rc):
-    """List radius = cutoff + skin. The skins are tuned on B200 (profiles/r02_experiments.md section 8): 0.08 nm for C2 (a rebuild every
-    ~36 steps), 0.10 nm for C4 (its rebuild costs 4x as much), 0.12 nm for 6mrr at 300 K / 0.5 fs. Both arms use the same radius."""
+    """List radius = cutoff + skin: 0.08 nm for C2 (a rebuild every ~36 steps), 0.10 nm for C4 (its rebuild costs 4x as much),
+    0.12 nm for 6mrr at 300 K / 0.5 fs. On an H100, C2 runs fastest at 1.28 nm of 1.26 / 1.28 / 1.30 / 1.32 nm. Both arms use
+    the same radius."""
     return rc + {"c2": 0.08, "c3": 0.12, "c4": 0.10}.get(wl, 0.10)
 
 
@@ -141,18 +142,14 @@ def measured_peaks():
     if os.path.exists(p):
         d = json.load(open(p))
         return float(d["hbm_gbs"]), "measured (MEASURED_PEAKS.json)"
-    return 6650.0, "fallback (B200_PROFILING.md)"
+    return 3350.0, "data sheet (H100 SXM, HBM3)"
 
 
-def ncu_traffic(workload_name: str):
-    """DRAM bytes per launch of the force kernel from the committed ncu capture, if any."""
-    p = os.path.join(ROOT, "profiles", f"force_kernel_{workload_name}.json")
-    if os.path.exists(p):
-        try:
-            return json.load(open(p)).get("dram_bytes_per_launch")
-        except Exception:
-            return None
-    return None
+def dump_outputs(out_dir, sysm):
+    """What the timed path hands its caller after its last step: the (n, 3) coordinates and velocities, float32."""
+    os.makedirs(out_dir, exist_ok=True)
+    for name, a in (("coords", sysm.coords), ("velocities", sysm.velocities)):
+        np.save(os.path.join(out_dir, f"{name}.npy"), a.detach().cpu().numpy().astype(np.float32))
 
 
 # ----------------------------------------------------------------------------------------------------
@@ -215,6 +212,8 @@ def main():
     ap.add_argument("--no-cm", action="store_true", help="diagnostic: remove_CM_motion=false")
     ap.add_argument("--replicas", action="store_true", help="N>1: independent replicas instead of the spatial decomposition")
     ap.add_argument("--no-extra", action="store_true", help="only the primary workload (no `workloads` object)")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="write the primary workload's coordinates and velocities after the last timed step as DIR/<name>.npy")
     args = ap.parse_args()
 
     rank = int(os.environ.get("RANK", "0"))
@@ -339,6 +338,8 @@ def run_ours(wl, args, ctx, steps, warmup, with_cpu, with_e2e, brief=False):
     t_ms = max_over_ranks(ev0.elapsed_time(ev1))
     clocks = sampler.stop() if rank == 0 else None
     st1 = sysm.stats()
+    if args.dump_outputs and rank == 0 and not brief:
+        dump_outputs(args.dump_outputs, sysm)
     # decomposed: all ranks advance ONE system; replicas: every rank advances its own copy
     mult = 1 if decomposed or world == 1 else world
     value = mult * steps / (t_ms * 1e-3)
@@ -355,7 +356,7 @@ def run_ours(wl, args, ctx, steps, warmup, with_cpu, with_e2e, brief=False):
     vv_us = max_over_ranks(1e3 * stp["vv_ms"] / max(stp["vv_launches"], 1))
     rebuilds_prof = stp["n_rebuilds"] - st1["n_rebuilds"]
     # stream mode enqueues the gated rebuild pipeline every step (2-3 us no-op kernels unless the flag is set), so this
-    # total is an upper bound of the real rebuild cost; profiles/r02_launches_*.md has the per-kernel numbers
+    # total is an upper bound of the real rebuild cost
     rebuild_total_ms = stp["rebuild_ms"]
 
     # ---- e2e through the C ABI with host (pinned) buffers
@@ -409,7 +410,8 @@ def run_ours(wl, args, ctx, steps, warmup, with_cpu, with_e2e, brief=False):
         step_gbs = step_bytes / (t_ms / steps * 1e-3) / 1e9
         pairs_in_cut = {"c2": 1.955e7, "c4": 7.64e7, "c3": 2.63e6}[wl]
         flop_per_pair = 42.0 if wl != "c3" else 50.0
-        fp32_peak = 148 * 128 * 2 * (clocks["sm_mhz"] or 1965.0) * 1e6 / 1e12 if clocks else None
+        props = torch.cuda.get_device_properties(dev)
+        fp32_peak = props.multi_processor_count * 128 * 2 * (clocks["sm_mhz"] or 1980.0) * 1e6 / 1e12 if clocks else None
         fp32_ach = (pairs_in_cut / share) * flop_per_pair / (force_us * 1e-6) / 1e12 if force_us > 0 else None
         par = ("single GPU" if world == 1 else (
             f"spatial decomposition: {world} z-slabs; per step: "
@@ -429,7 +431,8 @@ def run_ours(wl, args, ctx, steps, warmup, with_cpu, with_e2e, brief=False):
                        "parallelism": par,
                        "brick_dims": st1["brick_dims"], "list_stride": st1["list_stride"], "n_bricks": st1["n_bricks"],
                        "l2": "not flushed between steps: step k+1 consumes the state step k wrote; per-step working set = "
-                             f"{(st1['n_list_entries'] * 2 + n * 100) / 1e6:.0f} MB (neighbour list + state) vs 126 MB L2"},
+                             f"{(st1['n_list_entries'] * 2 + n * 100) / 1e6:.0f} MB (neighbour list + state) vs "
+                             f"{props.L2_cache_size / 2**20:.0f} MB L2"},
             "ns_per_day": value * dt * 1e3 * 0.0864,
             "gpu_launches": int(launches),
             "rebuilds_in_timed_region": int(st1["n_rebuilds"] - st0["n_rebuilds"]),
@@ -437,7 +440,7 @@ def run_ours(wl, args, ctx, steps, warmup, with_cpu, with_e2e, brief=False):
             "clocks": clocks,
             "e2e": e2e,
             "roofline": {"bound": "hbm", "kernel": "brick_force_kernel", "achieved": achieved, "peak": peak, "unit": "GB/s",
-                         "frac": (achieved / peak) if achieved else None, "traffic": ncu_traffic(wl), "peak_source": peak_src,
+                         "frac": (achieved / peak) if achieved else None, "peak_source": peak_src,
                          "algorithmic_bytes_per_launch": alg_bytes, "launch_us": force_us,
                          "per_rank_share": f"1/{share} of the atoms per launch (slowest rank's kernel time)",
                          "whole_step": {"algorithmic_bytes": step_bytes, "achieved": step_gbs, "frac": step_gbs / peak}},

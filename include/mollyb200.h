@@ -1,5 +1,5 @@
 /*
- * mollyb200.h — C ABI of libmollyb200.so, the B200-native (sm_100a) engine for
+ * mollyb200.h — C ABI of libmollyb200.so, the H100-native (sm_90a) engine for
  * Molly.jl's pairwise non-bonded + VelocityVerlet hot path.
  *
  * Every entry point is what a Julia `ccall` (or Python ctypes) binds; no C++ or

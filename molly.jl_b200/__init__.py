@@ -1,4 +1,4 @@
-"""mollyb200 — B200-native engine for Molly.jl's pairwise non-bonded + VelocityVerlet hot path.
+"""mollyb200 — H100-native engine for Molly.jl's pairwise non-bonded + VelocityVerlet hot path.
 
 The directory is named after the reference (`molly.jl_b200`); import it through the top-level
 `mollyb200` module. Only what the path needs lives here: csrc/ (CUDA kernels + the C ABI), the ctypes

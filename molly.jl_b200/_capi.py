@@ -68,7 +68,7 @@ def load():
         return _lib
     if not os.path.exists(LIB_PATH):
         raise ImportError(
-            f"{LIB_PATH} is missing: build it with `python __graft_entry__.py` (nvcc, sm_100a). "
+            f"{LIB_PATH} is missing: build it with `python __graft_entry__.py` (nvcc, sm_90a). "
             "mollyb200 has no CPU or PyTorch fallback.")
     L = C.CDLL(LIB_PATH)
     vp, i32, i64, dbl = C.c_void_p, C.c_int32, C.c_int64, C.c_double

@@ -1,4 +1,4 @@
-"""Build libmollyb200.so in-tree with nvcc for sm_100a (the only target)."""
+"""Build libmollyb200.so in-tree with nvcc for sm_90a (H100, the only target)."""
 from __future__ import annotations
 
 import os
@@ -38,7 +38,7 @@ def build(force: bool = False, verbose: bool = False, defines=(), out: str = Non
     host_cxx = "/usr/bin/g++" if os.path.exists("/usr/bin/g++") else "g++"
     cmd = [
         _nvcc(), "-std=c++17", "-O3", "-lineinfo",
-        "-gencode", "arch=compute_100a,code=sm_100a",
+        "-gencode", "arch=compute_90a,code=sm_90a",
         "-ccbin", host_cxx,
         "-Xcompiler", "-fPIC,-O2,-Wall,-Wno-unused-function",
         "--expt-relaxed-constexpr",

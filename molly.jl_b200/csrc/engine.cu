@@ -1238,8 +1238,7 @@ class Engine : public EngineBase {
     // L2 keeps under plain LRU streaming). Pin a fraction of it in L2 with an access-policy window: lines of the window
     // are kept "persisting" with probability hitRatio, the rest stream through.
     int set_l2_persistence() {
-        // opt-in (MOLLYB200_L2PERSIST=1): measured on B200 at C2 it changes nothing (83.8 us without, 84.3-86.2 us with), the
-        // kernel is not bound by the list stream
+        // opt-in (MOLLYB200_L2PERSIST=1): by default the L2 policy of the stream is left alone
         const char* on = getenv("MOLLYB200_L2PERSIST");
         if (!(on && on[0] == '1')) return MB_OK;
         int max_persist = 0, max_window = 0;
@@ -2129,7 +2128,7 @@ class Engine : public EngineBase {
    private:
     int device_;
     cudaStream_t stream_;
-    int sm_count_ = 148;
+    int sm_count_ = 132;
     size_t smem_optin_ = 232448;
     int64_t n_ = 0;
     std::vector<T> h_mass_, h_charge_, h_sigma_, h_eps_, h_eps_raw_;
@@ -2243,8 +2242,8 @@ int mb_ctx_create(int device, int dtype, void* cuda_stream, mb_ctx** out) {
     if (cudaSetDevice(device) != cudaSuccess) return mb::set_error(MB_ERR_CUDA, "cudaSetDevice failed");
     cudaDeviceProp prop;
     if (cudaGetDeviceProperties(&prop, device) != cudaSuccess) return mb::set_error(MB_ERR_CUDA, "cudaGetDeviceProperties failed");
-    if (prop.major < 10)
-        return mb::set_error(MB_ERR_NOGPU, std::string("device ") + prop.name + " is not sm_100-class; this library is built for sm_100a only");
+    if (prop.major != 9 || prop.minor != 0)  // sm_90a code runs on compute capability 9.0 only
+        return mb::set_error(MB_ERR_NOGPU, std::string("device ") + prop.name + " is not sm_90 (H100-class); this library is built for sm_90a only");
     mb_ctx* c = new mb_ctx();
     c->device = device;
     c->dtype = dtype;

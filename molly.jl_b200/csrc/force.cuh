@@ -36,8 +36,14 @@ constexpr int FORCE_MAX_STAGES = 3;
 #define MB_LIST_BATCH 8
 #endif
 #ifndef MB_USE_F32X2
-#define MB_USE_F32X2 1  // Blackwell packed-f32 (FFMA2/FMUL2) pair loop for the uniform-LJ f32 force path
+#define MB_USE_F32X2 1  // two-neighbour (even/odd) pair loop for the uniform-LJ f32 force path
 #endif
+
+// element-wise float2 helpers of that loop: two independent FMA chains, rounded like the scalar intrinsics
+__device__ __forceinline__ float2 ffma2_rn(float2 a, float2 b, float2 c) {
+    return make_float2(__fmaf_rn(a.x, b.x, c.x), __fmaf_rn(a.y, b.y, c.y));
+}
+__device__ __forceinline__ float2 fmul2_rn(float2 a, float2 b) { return make_float2(__fmul_rn(a.x, b.x), __fmul_rn(a.y, b.y)); }
 
 template <typename T>
 struct ForceOut {
@@ -209,7 +215,7 @@ __global__ void __launch_bounds__(FORCE_THREADS, (sizeof(T) == 8) ? 1 : FORCE_CT
         T lj_s_i = (T)0, lj_e_i = (T)0, kq_i = (T)0;
         T fx = (T)0, fy = (T)0, fz = (T)0;
 #if MB_USE_F32X2
-        float2 axx = make_float2(0.f, 0.f), ayy = axx, azz = axx;  // packed-f32 accumulators (two neighbours per lane)
+        float2 axx = make_float2(0.f, 0.f), ayy = axx, azz = axx;  // even/odd-neighbour accumulators of the uniform-LJ f32 loop
         (void)axx; (void)ayy; (void)azz;
 #endif
         auto eval = [&](int j, auto special_tag) {
@@ -254,25 +260,23 @@ __global__ void __launch_bounds__(FORCE_THREADS, (sizeof(T) == 8) ? 1 : FORCE_CT
             }
 #if MB_USE_F32X2
             if constexpr (std::is_same<T, float>::value && UNIFORM && CUTM == CUTM_PLAIN && !ENERGY && COUL == COUL_NONE) {
-                // Blackwell packed-f32 path (FADD2 / FMUL2 / FFMA2): two neighbours per instruction
+                // neighbours 0/2 and 1/3 accumulate into separate partial sums: two independent FMA chains per lane
 #pragma unroll
                 for (int h2 = 0; h2 < 2; h2++) {
                     const float4 a = pj[2 * h2], b = pj[2 * h2 + 1];
-                    // scalar subtractions write straight into register pairs; packing (a.x, b.x) first costs two moves
-                    // per component because the gathered float4s arrive as x,y,z,w quads
                     const float2 dx = make_float2(pi.x - a.x, pi.x - b.x);
                     const float2 dy = make_float2(pi.y - a.y, pi.y - b.y);
                     const float2 dz = make_float2(pi.z - a.z, pi.z - b.z);
-                    const float2 r2 = __ffma2_rn(dz, dz, __ffma2_rn(dy, dy, __fmul2_rn(dx, dx)));
+                    const float2 r2 = ffma2_rn(dz, dz, ffma2_rn(dy, dy, fmul2_rn(dx, dx)));
                     const float2 iv = make_float2(frcp(r2.x), frcp(r2.y));
-                    const float2 i3 = __fmul2_rn(__fmul2_rn(iv, iv), iv);
-                    const float2 tt = __ffma2_rn(make_float2(P.uni_A, P.uni_A), i3, make_float2(-P.uni_B, -P.uni_B));
-                    float2 fr = __fmul2_rn(tt, __fmul2_rn(i3, iv));
+                    const float2 i3 = fmul2_rn(fmul2_rn(iv, iv), iv);
+                    const float2 tt = ffma2_rn(make_float2(P.uni_A, P.uni_A), i3, make_float2(-P.uni_B, -P.uni_B));
+                    float2 fr = fmul2_rn(tt, fmul2_rn(i3, iv));
                     fr.x = (r2.x <= P.lj_rc2) ? fr.x : 0.f;
                     fr.y = (r2.y <= P.lj_rc2) ? fr.y : 0.f;
-                    axx = __ffma2_rn(fr, dx, axx);
-                    ayy = __ffma2_rn(fr, dy, ayy);
-                    azz = __ffma2_rn(fr, dz, azz);
+                    axx = ffma2_rn(fr, dx, axx);
+                    ayy = ffma2_rn(fr, dy, ayy);
+                    azz = ffma2_rn(fr, dz, azz);
                 }
                 return;
             }

@@ -539,7 +539,7 @@ def test_c2_energy_conservation_f32():
 # full-size parity against the oracle's neighbour-list path (the configs that carry the bench numbers)
 # ---------------------------------------------------------------------------------------------------
 def _full_size_vs_oracle(cells, label):
-    """Forces + energy of the packed-f32 fast path at full size vs the f64 oracle on the same f32-rounded coordinates.
+    """Forces + energy of the uniform-LJ f32 fast path at full size vs the f64 oracle on the same f32-rounded coordinates.
     Bar: the repo's f32 tolerance (5e-5 max|F| + 2e-3 kJ/mol/nm per component; pairs within f32 rounding of the cutoff
     may land on either side and are allowed one F(rc) jump each), energy rel 2e-6."""
     sd = H.lj_fluid(cells, seed=42, dtype=np.float32)

@@ -86,7 +86,7 @@ def test_c5_pme_total_energy_f64(golden_6mrr):
     """BASELINE config 5 on the system the reference ships goldens for (SURVEY.md section 8d: 6mrr with :pme, Float64): total energy
     over 0.2 ps of VelocityVerlet at two step sizes. The reference's energy-conservation protocol (test/energy_conservation.jl) is
     the soft LJ system of tests/test_gpu_parity.py::test_energy_conservation_reference_protocol, which passes at its 5e-4 kJ/mol
-    bar; for a solvated protein it states no bar. Measured here (B200): E - E0 = -984 kJ/mol (1.5 % of KE) at dt 0.5 fs and
+    bar; for a solvated protein it states no bar. Measured on an H100: E - E0 = -984 kJ/mol (1.5 % of KE) at dt 0.5 fs and
     -527 kJ/mol at dt 0.25 fs: an O(dt^2) part (this start - flexible TIP3P with velocities_300K - is off the integrator's shadow
     Hamiltonian while the O-H stretches thermalise) plus a step-size-independent part of about -380 kJ/mol that the truncated
     (not shifted) LJ / Ewald real-space energies at 1.0 nm allow. The same run with the reaction-field cutoff instead of PME, with
