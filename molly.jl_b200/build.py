@@ -31,8 +31,8 @@ def needs_build() -> bool:
     return False
 
 
-def build(force: bool = False, verbose: bool = False, defines=(), out: str = None) -> str:
-    """defines/out: build a tuning variant (e.g. defines=("MB_LIST_BATCH=4",), out="libmollyb200_b4.so")."""
+def build(force: bool = False, verbose: bool = False, out: str = None) -> str:
+    """out: build under another file name next to the default library (e.g. to A/B two versions via MOLLYB200_LIB)."""
     if out is None and not force and not needs_build():
         return LIB
     host_cxx = "/usr/bin/g++" if os.path.exists("/usr/bin/g++") else "g++"
@@ -44,7 +44,6 @@ def build(force: bool = False, verbose: bool = False, defines=(), out: str = Non
         "--expt-relaxed-constexpr",
         "-shared", "-o", os.path.join(HERE, out) if out else LIB,
     ]
-    cmd += [f"-D{d}" for d in defines]
     if verbose:
         cmd += ["-Xptxas", "-v"]
     cmd += [os.path.join(CSRC, s) for s in SOURCES]
@@ -55,6 +54,5 @@ def build(force: bool = False, verbose: bool = False, defines=(), out: str = Non
 
 
 if __name__ == "__main__":
-    defs = tuple(a[2:] for a in sys.argv[1:] if a.startswith("-D"))
     outs = [a[6:] for a in sys.argv[1:] if a.startswith("--out=")]
-    build(force="--force" in sys.argv, verbose="-v" in sys.argv, defines=defs, out=outs[0] if outs else None)
+    build(force="--force" in sys.argv, verbose="-v" in sys.argv, out=outs[0] if outs else None)

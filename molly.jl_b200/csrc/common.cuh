@@ -153,22 +153,9 @@ __device__ __forceinline__ dbl2 lds_pair(uint32_t addr, double) {
 // streaming (read-once) global loads that do not pollute L1
 __device__ __forceinline__ uint2 ldg_stream_u2(const uint2* p) {
     uint2 r;
-#if defined(MB_ABL_NOLIST)  // ablation: no neighbour-list loads (indices derived from the address: wrong results, timing only)
-    const unsigned int a = (unsigned int)((unsigned long long)p >> 3);
-    r.x = ((a * 2654435761u) >> 19 & 0x1ff0u) | (((a * 40503u) & 0x1ff0u) << 16);
-    r.y = ((a * 97u) & 0x1ff0u) | (((a * 31u) & 0x1ff0u) << 16);
-    return r;
-#endif
-#if defined(MB_LDG_PLAIN)
-    asm volatile("ld.global.v2.u32 {%0, %1}, [%2];" : "=r"(r.x), "=r"(r.y) : "l"(p));
-#elif defined(MB_LDG_NC)
-    asm volatile("ld.global.nc.v2.u32 {%0, %1}, [%2];" : "=r"(r.x), "=r"(r.y) : "l"(p));
-#else
     asm volatile("ld.global.nc.L1::no_allocate.v2.u32 {%0, %1}, [%2];" : "=r"(r.x), "=r"(r.y) : "l"(p));
-#endif
     return r;
 }
-__device__ __forceinline__ void prefetch_l2(const void* p) { asm volatile("prefetch.global.L2 [%0];" ::"l"(p)); }
 
 // warp helpers
 template <typename T>

@@ -320,7 +320,7 @@ class Engine : public EngineBase {
     using T2 = typename VT<T>::T2;
 
    public:
-    Engine(int device, cudaStream_t stream) : device_(device), stream_(stream) {
+    Engine(int device, cudaStream_t stream) : stream_(stream) {
         cudaDeviceProp prop;
         cudaGetDeviceProperties(&prop, device);
         sm_count_ = prop.multiProcessorCount;
@@ -335,8 +335,6 @@ class Engine : public EngineBase {
         prof_.stream = stream_;
         const char* ng = getenv("MOLLYB200_NO_GRAPH");
         graph_enabled_ = !(ng && ng[0] == '1');
-        const char* ss = getenv("MOLLYB200_STATIC_SCHED");
-        static_sched_ = ss && ss[0] == '1';
     }
     ~Engine() override {
         destroy_graph();
@@ -497,7 +495,6 @@ class Engine : public EngineBase {
         }
         if (!(lpa == 0 || lpa == 8))
             return set_error(MB_ERR_INVALID, "lanes_per_atom must be 0 (default) or 8: the 4- and 16-lane variants were measured slower and removed");
-        lpa_ = lpa ? lpa : 8;
         have_list_ = false;
         dirty_ = true;
         return MB_OK;
@@ -539,7 +536,6 @@ class Engine : public EngineBase {
         if (path_ == 1 && max_rc > r_list_)
             return set_error(MB_ERR_INVALID, "neighbour list radius is smaller than an interaction cutoff");
         skin_ = (path_ == 1) ? (any_nocut_nl ? 0.0 : r_list_ - max_rc) : 0.0;
-        max_rc_ = max_rc;
         P_.has_lj = 0;
         P_.coul_kind = COUL_NONE;
         P_.lj_rc2 = (T)0;
@@ -653,7 +649,6 @@ class Engine : public EngineBase {
         const int vvb = (int)((n_ + VV_THREADS - 1) / VV_THREADS);
         MB_CUDA(d_partial_.ensure((size_t)std::max(vvb, 2048) * 8 * sizeof(double)));
         have_list_ = false;
-        slots_init_ = false;
         dirty_ = false;
         return MB_OK;
     }
@@ -768,7 +763,6 @@ class Engine : public EngineBase {
         while (ctas_per_sm > 1 && (sm_total / ctas_per_sm - 1024 - static_bytes) / stage < 1) ctas_per_sm--;
         const size_t budget = (ctas_per_sm > 1) ? sm_total / ctas_per_sm - 1024 - static_bytes : smem_optin_ - static_bytes;
         nbuf = (int)std::min<size_t>(FORCE_MAX_STAGES, std::max<size_t>(1, budget / stage));
-        if (const char* e = getenv("MOLLYB200_NBUF")) nbuf = std::max(1, std::min(nbuf, atoi(e)));  // tuning aid: shallower ring
     }
     size_t build_smem_bytes() const {
         return (size_t)g_.halo_cap * (sizeof(T4) + sizeof(int)) + (size_t)((g_.hcells + 3) & ~3) * sizeof(ushort2) +
@@ -1234,34 +1228,6 @@ class Engine : public EngineBase {
         return MB_OK;
     }
 
-    // The neighbour list is the one large stream the force kernel re-reads every step (131 MB at C2, larger than what
-    // L2 keeps under plain LRU streaming). Pin a fraction of it in L2 with an access-policy window: lines of the window
-    // are kept "persisting" with probability hitRatio, the rest stream through.
-    int set_l2_persistence() {
-        // opt-in (MOLLYB200_L2PERSIST=1): by default the L2 policy of the stream is left alone
-        const char* on = getenv("MOLLYB200_L2PERSIST");
-        if (!(on && on[0] == '1')) return MB_OK;
-        int max_persist = 0, max_window = 0;
-        cudaDeviceGetAttribute(&max_persist, cudaDevAttrMaxPersistingL2CacheSize, device_);
-        cudaDeviceGetAttribute(&max_window, cudaDevAttrMaxAccessPolicyWindowSize, device_);
-        if (max_persist <= 0 || max_window <= 0) return MB_OK;
-        const char* fr = getenv("MOLLYB200_L2PERSIST_FRAC");
-        const double frac = fr ? atof(fr) : 0.75;
-        size_t persist = (size_t)(frac * max_persist);
-        if (cudaDeviceSetLimit(cudaLimitPersistingL2CacheSize, persist) != cudaSuccess) { cudaGetLastError(); return MB_OK; }
-        DevBuf& lst = d_list_;
-        size_t bytes = std::min((size_t)n_ * g_.stride * sizeof(unsigned short), (size_t)max_window);
-        cudaStreamAttrValue attr;
-        memset(&attr, 0, sizeof(attr));
-        attr.accessPolicyWindow.base_ptr = lst.p;
-        attr.accessPolicyWindow.num_bytes = bytes;
-        attr.accessPolicyWindow.hitRatio = (float)std::min(1.0, (double)persist / (double)bytes);
-        attr.accessPolicyWindow.hitProp = cudaAccessPropertyPersisting;
-        attr.accessPolicyWindow.missProp = cudaAccessPropertyStreaming;
-        if (cudaStreamSetAttribute(stream_, cudaStreamAttributeAccessPolicyWindow, &attr) != cudaSuccess) cudaGetLastError();
-        return MB_OK;
-    }
-
     // launch the list builder (count-only or real; with or without exclusion handling)
     int launch_build(bool count_only) {
         const size_t smem = build_smem_bytes();
@@ -1354,7 +1320,6 @@ class Engine : public EngineBase {
                                                       d_mass_in_.as<T>(), d_pos4_.as<T4>(), d_vel4_.as<T4>(), d_lj2_.as<T2>(),
                                                       d_orig_.as<int>(), d_inv_orig_.as<int>(), d_mass_.as<T>(), d_xref4_.as<T4>());
         launches_++;
-        slots_init_ = true;
         for (int attempt = 0; attempt < 8; attempt++) {
             MB_TRY(choose_geometry());
             MB_TRY(alloc_brick_tables());
@@ -1413,10 +1378,8 @@ class Engine : public EngineBase {
             MB_TRY(enqueue_rebuild(true, false));
             MB_TRY(read_ctl(c));
             if (c.overflow) return set_error(MB_ERR_CAPACITY, "neighbour capacity overflow during first build");
-            last_ctl_ = c;
             have_list_ = true;
             geom_version_++;
-            set_l2_persistence();
             if (decomposed()) {
                 MB_TRY(update_ownership());
                 since_rebuild_ = 0;
@@ -1439,8 +1402,7 @@ class Engine : public EngineBase {
         prof_.begin(Prof::FORCE);
         kern<<<grid, FORCE_THREADS, smem, stream_>>>(g_, P_, d_hdrs_.as<BrickHdr>(), d_runs_.as<Run>(), d_task_tab_.as<int2>(),
                                                      d_pos4e_.as<T4>(), d_lj2e_.as<T2>(), d_list_.as<unsigned short>(),
-                                                     d_slist_.as<unsigned short>(), out, brick0, nbr, nbuf,
-                                                     static_sched_ ? nullptr : d_sched_.as<unsigned int>());
+                                                     d_slist_.as<unsigned short>(), out, brick0, nbr, nbuf, d_sched_.as<unsigned int>());
         prof_.end(Prof::FORCE);
         launches_++;
         n_force_evals_++;
@@ -1449,12 +1411,8 @@ class Engine : public EngineBase {
     }
     template <int COUL, bool UNIFORM>
     int launch_force_c(bool energy, ForceOut<T> out, int b0, int nbr) {
-#ifdef MB_EXP_FAST  // experiment builds (scripts/): only the plain-cutoff variants are instantiated
-        if (cutm_ != CUTM_PLAIN) return set_error(MB_ERR_INVALID, "experiment build: plain cutoffs only");
-#else
         if (cutm_ == CUTM_TWO_POINT) return energy ? launch_force_t<COUL, UNIFORM, CUTM_TWO_POINT, true>(out, b0, nbr) : launch_force_t<COUL, UNIFORM, CUTM_TWO_POINT, false>(out, b0, nbr);
         if (cutm_ == CUTM_SHIFTED) return energy ? launch_force_t<COUL, UNIFORM, CUTM_SHIFTED, true>(out, b0, nbr) : launch_force_t<COUL, UNIFORM, CUTM_SHIFTED, false>(out, b0, nbr);
-#endif
         return energy ? launch_force_t<COUL, UNIFORM, CUTM_PLAIN, true>(out, b0, nbr) : launch_force_t<COUL, UNIFORM, CUTM_PLAIN, false>(out, b0, nbr);
     }
     // owned_only: in a decomposed run the step loop evaluates only this rank's slab of bricks
@@ -1470,13 +1428,9 @@ class Engine : public EngineBase {
         switch (P_.coul_kind) {
             case COUL_NONE:
                 return P_.uniform_lj ? launch_force_c<COUL_NONE, true>(energy, out, b0, nbr) : launch_force_c<COUL_NONE, false>(energy, out, b0, nbr);
-#ifndef MB_EXP_FAST
             case COUL_PLAIN: return launch_force_c<COUL_PLAIN, false>(energy, out, b0, nbr);
-            default: return launch_force_c<COUL_EWALD, false>(energy, out, b0, nbr);
-#else
-            default: return set_error(MB_ERR_INVALID, "experiment build: LJ and LJ + CoulombReactionField only");
-#endif
             case COUL_CRF: return launch_force_c<COUL_CRF, false>(energy, out, b0, nbr);
+            default: return launch_force_c<COUL_EWALD, false>(energy, out, b0, nbr);
         }
     }
 
@@ -1565,7 +1519,6 @@ class Engine : public EngineBase {
     int check_overflow_sync() {
         Control c;
         MB_TRY(read_ctl(c));
-        last_ctl_ = c;
         if (c.overflow) {
             have_list_ = false;  // next call re-derives capacities
             static const int zero = 0;
@@ -2126,7 +2079,6 @@ class Engine : public EngineBase {
     }
 
    private:
-    int device_;
     cudaStream_t stream_;
     int sm_count_ = 132;
     size_t smem_optin_ = 232448;
@@ -2141,14 +2093,12 @@ class Engine : public EngineBase {
     double r_list_ = 0, skin_ = 0, cap_scale_ = 1.0, total_mass_ = 0;
     int rebuild_every_ = 0;
     int user_b_[3] = {0, 0, 0};
-    int lpa_ = 8;
-    bool dirty_ = true, have_list_ = false, slots_init_ = false;
+    bool dirty_ = true, have_list_ = false;
     int cutm_ = CUTM_PLAIN;  // cutoff family of the kernel variant (pair.cuh)
     int path_ = 0;
     PairParams<T> P_;
     Geom<T> g_, g_ap_;
     Tric<T> tric_ = {};  // TriclinicBoundary (on = 0: cubic / rectangular box)
-    Control last_ctl_;
     int64_t launches_ = 0, n_force_evals_ = 0, n_steps_ = 0, graph_step_launches_ = 0;
     Prof prof_;
     cudaGraph_t graph_ = nullptr;
@@ -2199,8 +2149,6 @@ class Engine : public EngineBase {
     DevBuf d_ext_of_, d_gptr_, d_ghosts_, d_pos4e_, d_lj2e_, d_orig_e_;    // slot -> extended map, ghost table, extended arrays
     DevBuf d_task_tab_, d_sched_;  // per-brick task tables; brick ticket + finished-CTA counter of the force kernel
     int force_grid_ = 0;           // CTAs of the last force launch (= number of energy partials)
-    bool static_sched_ = false;    // MOLLYB200_STATIC_SCHED=1: round-robin bricks instead of tickets
-    double max_rc_ = 0;
     DevBuf d_partial_, d_pe_partial_;
 };
 
@@ -2249,11 +2197,7 @@ int mb_ctx_create(int device, int dtype, void* cuda_stream, mb_ctx** out) {
     c->dtype = dtype;
     cudaStream_t s = reinterpret_cast<cudaStream_t>(cuda_stream);
     if (dtype == 32) c->e.reset(new mb::Engine<float>(device, s));
-#ifndef MB_EXP_FAST
     else c->e.reset(new mb::Engine<double>(device, s));
-#else
-    else { delete c; return mb::set_error(MB_ERR_INVALID, "experiment build: Float32 only"); }
-#endif
     *out = c;
     return MB_OK;
 }

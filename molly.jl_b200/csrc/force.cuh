@@ -22,28 +22,10 @@ namespace mb {
 // ---- launch shape of the persistent brick kernel ---------------------------------------------------------------
 // 16 warps per CTA: 15 consumer warps evaluate pairs, 1 producer warp feeds them through a ring of up to FORCE_MAX_STAGES
 // shared-memory stages (one stage = one brick's halo + its task table), filled by the TMA engine.
-#ifndef MB_FORCE_THREADS
-#define MB_FORCE_THREADS 512
-#endif
-#ifndef MB_FORCE_CTAS
-#define MB_FORCE_CTAS 2  // resident CTAs per SM the f32 variants are compiled for (register cap = 64K / (CTAs x threads))
-#endif
-constexpr int FORCE_THREADS = MB_FORCE_THREADS;
-constexpr int FORCE_CTAS_F32 = MB_FORCE_CTAS;
+constexpr int FORCE_THREADS = 512;
+constexpr int FORCE_CTAS_F32 = 2;  // resident CTAs per SM the f32 variants are compiled for (register cap = 64K / (CTAs x threads))
 constexpr int FORCE_CONSUMER_WARPS = FORCE_THREADS / 32 - 1;
 constexpr int FORCE_MAX_STAGES = 3;
-#ifndef MB_LIST_BATCH
-#define MB_LIST_BATCH 8
-#endif
-#ifndef MB_USE_F32X2
-#define MB_USE_F32X2 1  // two-neighbour (even/odd) pair loop for the uniform-LJ f32 force path
-#endif
-
-// element-wise float2 helpers of that loop: two independent FMA chains, rounded like the scalar intrinsics
-__device__ __forceinline__ float2 ffma2_rn(float2 a, float2 b, float2 c) {
-    return make_float2(__fmaf_rn(a.x, b.x, c.x), __fmaf_rn(a.y, b.y, c.y));
-}
-__device__ __forceinline__ float2 fmul2_rn(float2 a, float2 b) { return make_float2(__fmul_rn(a.x, b.x), __fmul_rn(a.y, b.y)); }
 
 template <typename T>
 struct ForceOut {
@@ -140,9 +122,9 @@ __global__ void __launch_bounds__(FORCE_THREADS, (sizeof(T) == 8) ? 1 : FORCE_CT
         };
         for (int seq = 0, s = 0, use = 0;; seq++, s = (s + 1 == nbuf) ? 0 : s + 1, use += (s == 0) ? 1 : 0) {
             // (1) next brick: the first one of a CTA is its block index (no ticket latency in front of the first stage), the
-            //     others are drawn from the global ticket counter; static round-robin when the launch asks for it
+            //     others are drawn from the global ticket counter; static round-robin for ENERGY launches
             int bi;
-            if (ENERGY || sched == nullptr) {
+            if (ENERGY) {
                 bi = (int)blockIdx.x + seq * (int)gridDim.x;
             } else if (seq == 0) {
                 bi = (int)blockIdx.x;
@@ -207,17 +189,13 @@ __global__ void __launch_bounds__(FORCE_THREADS, (sizeof(T) == 8) ? 1 : FORCE_CT
     } else {
         // =============================== consumer warps ===============================
         const int sub4 = lane >> 3, l = lane & 7;
-        constexpr int LIST_HALF = (MB_LIST_BATCH >= 2) ? MB_LIST_BATCH / 2 : 1;
+        constexpr int LIST_HALF = 4;  // list words (4 entries each) per lane and half batch: 8 words in flight
         const int words_in_row = g.stride >> 5;  // groups a row can hold
         // per-quad state (the stage changes from quad to quad): shared-memory addresses of the staged positions / LJ pairs
         uint32_t s_pos_u32 = 0, s_lj_u32 = 0;
         T4 pi = make4<T>(0, 0, 0, 0);
         T lj_s_i = (T)0, lj_e_i = (T)0, kq_i = (T)0;
         T fx = (T)0, fy = (T)0, fz = (T)0;
-#if MB_USE_F32X2
-        float2 axx = make_float2(0.f, 0.f), ayy = axx, azz = axx;  // even/odd-neighbour accumulators of the uniform-LJ f32 loop
-        (void)axx; (void)ayy; (void)azz;
-#endif
         auto eval = [&](int j, auto special_tag) {
             constexpr bool SPECIAL = decltype(special_tag)::value;
             const T4 pj = lds_pos(s_pos_u32 + (uint32_t)j * (uint32_t)sizeof(T4), (T)0);
@@ -245,12 +223,7 @@ __global__ void __launch_bounds__(FORCE_THREADS, (sizeof(T) == 8) ? 1 : FORCE_CT
         // chains are independent and in flight together
         auto eval4 = [&](uint2 wd) {
             // entries are byte offsets of float4 records (halo index << LIST_SHIFT)
-#ifdef MB_ABL_NOGATHER  // ablation: conflict-free gathers (every lane reads the record at its own lane index)
-            const int jj = (int)((threadIdx.x & 31u) << 4) + (int)((wd.x ^ wd.y) & 0x10u);
-            const int j[4] = {jj, jj, jj, jj};
-#else
             const int j[4] = {(int)(wd.x & 0xffffu), (int)(wd.x >> 16), (int)(wd.y & 0xffffu), (int)(wd.y >> 16)};
-#endif
             T4 pj[4];
             T2 lj[4];
 #pragma unroll
@@ -258,29 +231,6 @@ __global__ void __launch_bounds__(FORCE_THREADS, (sizeof(T) == 8) ? 1 : FORCE_CT
                 pj[u] = lds_pos(s_pos_u32 + (uint32_t)j[u] * (uint32_t)(sizeof(T4) >> LIST_SHIFT), (T)0);
                 if (!UNIFORM) lj[u] = lds_pair(s_lj_u32 + (((uint32_t)j[u] * (uint32_t)sizeof(T2)) >> LIST_SHIFT), (T)0);
             }
-#if MB_USE_F32X2
-            if constexpr (std::is_same<T, float>::value && UNIFORM && CUTM == CUTM_PLAIN && !ENERGY && COUL == COUL_NONE) {
-                // neighbours 0/2 and 1/3 accumulate into separate partial sums: two independent FMA chains per lane
-#pragma unroll
-                for (int h2 = 0; h2 < 2; h2++) {
-                    const float4 a = pj[2 * h2], b = pj[2 * h2 + 1];
-                    const float2 dx = make_float2(pi.x - a.x, pi.x - b.x);
-                    const float2 dy = make_float2(pi.y - a.y, pi.y - b.y);
-                    const float2 dz = make_float2(pi.z - a.z, pi.z - b.z);
-                    const float2 r2 = ffma2_rn(dz, dz, ffma2_rn(dy, dy, fmul2_rn(dx, dx)));
-                    const float2 iv = make_float2(frcp(r2.x), frcp(r2.y));
-                    const float2 i3 = fmul2_rn(fmul2_rn(iv, iv), iv);
-                    const float2 tt = ffma2_rn(make_float2(P.uni_A, P.uni_A), i3, make_float2(-P.uni_B, -P.uni_B));
-                    float2 fr = fmul2_rn(tt, fmul2_rn(i3, iv));
-                    fr.x = (r2.x <= P.lj_rc2) ? fr.x : 0.f;
-                    fr.y = (r2.y <= P.lj_rc2) ? fr.y : 0.f;
-                    axx = ffma2_rn(fr, dx, axx);
-                    ayy = ffma2_rn(fr, dy, ayy);
-                    azz = ffma2_rn(fr, dz, azz);
-                }
-                return;
-            }
-#endif
             T dx[4], dy[4], dz[4], r2[4], fr[4], e[4];
 #pragma unroll
             for (int u = 0; u < 4; u++) {
@@ -333,7 +283,7 @@ __global__ void __launch_bounds__(FORCE_THREADS, (sizeof(T) == 8) ? 1 : FORCE_CT
                 const int4 mt = *reinterpret_cast<const int4*>(&s_meta[look_s]);  // brick, icount, nq, next_q
                 if (mt.y < 0) return 0;
                 int q;
-                if (ENERGY || sched == nullptr) {
+                if (ENERGY) {
                     q = w + NW * k_local;
                     k_local++;
                 } else {
@@ -361,9 +311,6 @@ __global__ void __launch_bounds__(FORCE_THREADS, (sizeof(T) == 8) ? 1 : FORCE_CT
         uint2 wa[LIST_HALF];
         auto request_first = [&](const QD& qd) {
             const uint2* p2 = reinterpret_cast<const uint2*>(list + (size_t)max(qd.slot, 0) * g.stride) + l;
-#ifdef MB_L2PF  // experiment: the second half of the row towards L2 while the first half is on its way to registers
-            if (qd.slot >= 0 && l < 2) prefetch_l2(reinterpret_cast<const char*>(p2) - l * 8 + 256 + l * 128);
-#endif
 #pragma unroll
             for (int u = 0; u < LIST_HALF; u++)
                 wa[u] = (qd.slot >= 0 && u < words_in_row) ? ldg_stream_u2(p2 + (size_t)u * 8) : make_uint2(0u, 0u);
@@ -387,9 +334,6 @@ __global__ void __launch_bounds__(FORCE_THREADS, (sizeof(T) == 8) ? 1 : FORCE_CT
             }
             kq_i = P.ke * pi.w;
             fx = (T)0; fy = (T)0; fz = (T)0;
-#if MB_USE_F32X2
-            axx = make_float2(0.f, 0.f); ayy = axx; azz = axx;
-#endif
             // main list: groups of 32 entries; each of the 8 lanes owns 4 entries (one 8-byte word) per group
             const int n_groups = (cur_n_main + 31) >> 5;
             // the four atoms of the quad run the same number of group iterations (the longest row's); shorter rows feed zero
@@ -423,13 +367,6 @@ __global__ void __launch_bounds__(FORCE_THREADS, (sizeof(T) == 8) ? 1 : FORCE_CT
             }
             // special (1-4) pairs
             for (int m = l; m < cur_n_spec; m += 8) eval((int)slist[(size_t)slot * g.sstride + m], std::true_type{});
-#if MB_USE_F32X2
-            if constexpr (std::is_same<T, float>::value) {
-                fx += axx.x + axx.y;
-                fy += ayy.x + ayy.y;
-                fz += azz.x + azz.y;
-            }
-#endif
             // reduce the 8 partial forces of every atom
             __syncwarp();
 #pragma unroll
@@ -470,7 +407,7 @@ __global__ void __launch_bounds__(FORCE_THREADS, (sizeof(T) == 8) ? 1 : FORCE_CT
             else out.vir_partial[(size_t)blockIdx.x * 6 + (tid - 1)] = s;
         }
     }
-    if (!ENERGY && sched != nullptr && tid == FORCE_THREADS - 32) {
+    if (!ENERGY && tid == FORCE_THREADS - 32) {
         // the last CTA to get here re-arms the brick ticket for the next launch (every CTA has drawn its last ticket)
         __threadfence();
         const unsigned int t = atomicInc(sched + 1, gridDim.x - 1);

@@ -1,6 +1,6 @@
 #!/usr/bin/env python
-"""Tuning sweep on the GPU box: force-kernel / rebuild stage times for several brick shapes and lane counts.
-    python scripts/sweep.py --workload c2 --configs 0,0,0,8 3,3,3,8 4,4,4,8 ...   (bx,by,bz,lanes; 0,0,0 = auto)"""
+"""Tuning sweep on the GPU box: force-kernel / rebuild stage times for several brick shapes.
+    python scripts/sweep.py --workload c2 --configs 0,0,0 3,3,3 4,4,4 ...   (bx,by,bz; 0,0,0 = auto)"""
 import argparse
 import json
 import os
@@ -20,7 +20,7 @@ import mollyb200 as mb  # noqa: E402
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--workload", default="c2")
-    ap.add_argument("--configs", nargs="+", default=["0,0,0,8"])
+    ap.add_argument("--configs", nargs="+", default=["0,0,0"])
     ap.add_argument("--r-list", type=float, nargs="+", default=[None])
     ap.add_argument("--steps", type=int, default=100)
     args = ap.parse_args()
@@ -29,7 +29,7 @@ def main():
     for rl in args.r_list:
         r_list = rl if rl is not None else rc + 0.1
         for cfg in args.configs:
-            bx, by, bz, lanes = [int(v) for v in cfg.split(",")]
+            bx, by, bz = [int(v) for v in cfg.split(",")]
             nf = mb.GPUNeighborFinder(dist_cutoff=r_list, excluded_pairs=sd.get("excluded", np.zeros((0, 2), np.int32)) + 1,
                                       special_pairs=sd.get("special", np.zeros((0, 2), np.int32)) + 1, n_steps=0)
             specific = H.sixmrr_specific_lists(sd["golden"]) if "golden" in sd else ()
@@ -38,7 +38,7 @@ def main():
                           specific_inter_lists=specific)
             s.engine()
             try:
-                s.set_launch_config((bx, by, bz), lanes)
+                s.set_launch_config((bx, by, bz))
                 sim = mb.VelocityVerlet(dt=dt)
                 mb.simulate(s, sim, 20)
                 t0 = time.perf_counter()
