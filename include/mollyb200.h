@@ -111,7 +111,9 @@ int mb_set_box(mb_ctx* ctx, const double side[3]);
 /* TriclinicBoundary(bv1, bv2, bv3) (src/spatial.jl:151-215): three basis vectors, row-major (bv1 = basis_vectors[0..2] along
  * x; bv2 in the xy plane; bv3 with a positive z component), approx_images = true. Minimum image as vector() :528-534, wrap
  * as wrap_coords :584-600. Served by the no-list kernel (the reference's triclinic tests are small systems:
- * test/gpu_consistency.jl:287-337); specific interaction lists, PME and decomposed runs are refused for such a box. */
+ * test/gpu_consistency.jl:287-337). Specific interaction lists use the same vector; they are refused when the system would
+ * take the cell-list path in a rectangular box (every interaction on the list, n >= 64, smallest box height >= 2.5 r_list),
+ * which does not handle triclinic boxes yet. PME and decomposed runs are refused for such a box. */
 int mb_set_box_triclinic(mb_ctx* ctx, const double basis_vectors[9]);
 /* sys.pairwise_inters translated to descriptors (dispatch by type in the reference, SURVEY §8b). */
 int mb_set_inters(mb_ctx* ctx, int n_inters, const mb_inter_t* inters);

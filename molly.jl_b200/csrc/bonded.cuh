@@ -4,7 +4,7 @@
 // partials. Reference formulas: src/interactions/harmonic_bond.jl:13-54, harmonic_angle.jl:45-67,
 // periodic_torsion.jl:17-142, dihedral by atan2 (src/spatial.jl:882-894). Displacements are minimum-image.
 #pragma once
-#include "common.cuh"
+#include "cells.cuh"
 
 namespace mb {
 
@@ -38,6 +38,32 @@ __device__ __forceinline__ Vec3<T> mic_vec(const typename VT<T>::T4& c1, const t
     dz -= L[2] * frint(dz * invL[2]);
     return v3(dx, dy, dz);
 }
+struct BoxT {
+    double L[3];
+};
+// minimum-image displacement c2 - c1 for the box kind B: BoxT (rectangular) or Tric<T> (TriclinicBoundary's vector,
+// src/spatial.jl:528-534)
+template <typename T, typename B>
+struct Mic;
+template <typename T>
+struct Mic<T, BoxT> {
+    T L[3], invL[3];
+    __device__ __forceinline__ explicit Mic(const BoxT& box)
+        : L{(T)box.L[0], (T)box.L[1], (T)box.L[2]}, invL{(T)(1.0 / box.L[0]), (T)(1.0 / box.L[1]), (T)(1.0 / box.L[2])} {}
+    __device__ __forceinline__ Vec3<T> operator()(const typename VT<T>::T4& c1, const typename VT<T>::T4& c2) const {
+        return mic_vec<T>(c1, c2, L, invL);
+    }
+};
+template <typename T>
+struct Mic<T, Tric<T>> {
+    Tric<T> t;
+    __device__ __forceinline__ explicit Mic(const Tric<T>& box) : t(box) {}
+    __device__ __forceinline__ Vec3<T> operator()(const typename VT<T>::T4& c1, const typename VT<T>::T4& c2) const {
+        T dx = c2.x - c1.x, dy = c2.y - c1.y, dz = c2.z - c1.z;
+        tric_vector<T>(t, dx, dy, dz);
+        return v3(dx, dy, dz);
+    }
+};
 template <typename T>
 __device__ __forceinline__ void add_force(typename VT<T>::T4* f4, int slot, Vec3<T> f) {
     T* p = reinterpret_cast<T*>(&f4[slot]);
@@ -45,10 +71,6 @@ __device__ __forceinline__ void add_force(typename VT<T>::T4* f4, int slot, Vec3
     atomicAdd(p + 1, f.y);
     atomicAdd(p + 2, f.z);
 }
-
-struct BoxT {
-    double L[3];
-};
 
 constexpr int BONDED_THREADS = 128;
 
@@ -66,18 +88,17 @@ __device__ __forceinline__ void block_energy(double e, double* __restrict__ part
 }
 
 // slot_of: original atom index -> slot (inv_orig), or nullptr when positions are in original order
-template <typename T, bool ENERGY>
+template <typename T, bool ENERGY, typename B>
 __device__ __forceinline__ double bond_term(int t, int n, const int* __restrict__ idx, const T* __restrict__ par,
                                             const int* __restrict__ slot_of, const typename VT<T>::T4* __restrict__ pos4,
-                                            typename VT<T>::T4* __restrict__ f4, const BoxT& box) {
+                                            typename VT<T>::T4* __restrict__ f4, const B& box) {
     double e = 0;
     if (t < n) {
-        const T L[3] = {(T)box.L[0], (T)box.L[1], (T)box.L[2]};
-        const T invL[3] = {(T)(1.0 / box.L[0]), (T)(1.0 / box.L[1]), (T)(1.0 / box.L[2])};
+        const Mic<T, B> mic(box);
         int i = idx[2 * t], j = idx[2 * t + 1];
         if (slot_of) { i = slot_of[i]; j = slot_of[j]; }
         const T k = par[2 * t], r0 = par[2 * t + 1];
-        Vec3<T> ab = mic_vec<T>(pos4[i], pos4[j], L, invL);
+        Vec3<T> ab = mic(pos4[i], pos4[j]);
         const T r = fsqrt(dot(ab, ab));
         const T c = k * (r - r0);
         Vec3<T> fi = (c / r) * ab;  // f_i = +c ab/|ab|, f_j = -f_i (harmonic_bond.jl:25-33)
@@ -88,19 +109,18 @@ __device__ __forceinline__ double bond_term(int t, int n, const int* __restrict_
     return e;
 }
 
-template <typename T, bool ENERGY>
+template <typename T, bool ENERGY, typename B>
 __device__ __forceinline__ double angle_term(int t, int n, const int* __restrict__ idx, const T* __restrict__ par,
                                              const int* __restrict__ slot_of, const typename VT<T>::T4* __restrict__ pos4,
-                                             typename VT<T>::T4* __restrict__ f4, const BoxT& box) {
+                                             typename VT<T>::T4* __restrict__ f4, const B& box) {
     double e = 0;
     if (t < n) {
-        const T L[3] = {(T)box.L[0], (T)box.L[1], (T)box.L[2]};
-        const T invL[3] = {(T)(1.0 / box.L[0]), (T)(1.0 / box.L[1]), (T)(1.0 / box.L[2])};
+        const Mic<T, B> mic(box);
         int i = idx[3 * t], j = idx[3 * t + 1], kk = idx[3 * t + 2];
         if (slot_of) { i = slot_of[i]; j = slot_of[j]; kk = slot_of[kk]; }
         const T k = par[2 * t], th0 = par[2 * t + 1];
-        Vec3<T> ba = mic_vec<T>(pos4[j], pos4[i], L, invL);
-        Vec3<T> bc = mic_vec<T>(pos4[j], pos4[kk], L, invL);
+        Vec3<T> ba = mic(pos4[j], pos4[i]);
+        Vec3<T> bc = mic(pos4[j], pos4[kk]);
         Vec3<T> nrm = cross(ba, bc);
         const T n2 = dot(nrm, nrm);
         if (n2 > (T)0) {
@@ -123,20 +143,19 @@ __device__ __forceinline__ double angle_term(int t, int n, const int* __restrict
 }
 
 // one (periodicity, phase, k) term per entry; a torsion with several terms appears several times
-template <typename T, bool ENERGY>
+template <typename T, bool ENERGY, typename B>
 __device__ __forceinline__ double torsion_term(int t, int n, const int* __restrict__ idx, const T* __restrict__ par,
                                                const int* __restrict__ slot_of, const typename VT<T>::T4* __restrict__ pos4,
-                                               typename VT<T>::T4* __restrict__ f4, const BoxT& box) {
+                                               typename VT<T>::T4* __restrict__ f4, const B& box) {
     double e = 0;
     if (t < n) {
-        const T L[3] = {(T)box.L[0], (T)box.L[1], (T)box.L[2]};
-        const T invL[3] = {(T)(1.0 / box.L[0]), (T)(1.0 / box.L[1]), (T)(1.0 / box.L[2])};
+        const Mic<T, B> mic(box);
         int i = idx[4 * t], j = idx[4 * t + 1], k = idx[4 * t + 2], l = idx[4 * t + 3];
         if (slot_of) { i = slot_of[i]; j = slot_of[j]; k = slot_of[k]; l = slot_of[l]; }
         const T per = par[3 * t], phase = par[3 * t + 1], kk = par[3 * t + 2];
-        Vec3<T> ab = mic_vec<T>(pos4[i], pos4[j], L, invL);
-        Vec3<T> bc = mic_vec<T>(pos4[j], pos4[k], L, invL);
-        Vec3<T> cd = mic_vec<T>(pos4[k], pos4[l], L, invL);
+        Vec3<T> ab = mic(pos4[i], pos4[j]);
+        Vec3<T> bc = mic(pos4[j], pos4[k]);
+        Vec3<T> cd = mic(pos4[k], pos4[l]);
         Vec3<T> m = cross(ab, bc), nn = cross(bc, cd);
         const T nbc = fsqrt(dot(bc, bc));
         const T th = atan2(dot(cross(m, nn), bc) / nbc, dot(m, nn));
@@ -165,20 +184,20 @@ struct BondedLists {
     const int* idx[3];
     const void* par[3];
 };
-template <typename T, bool ENERGY>
+template <typename T, bool ENERGY, typename B>
 __global__ void __launch_bounds__(BONDED_THREADS)
     bonded_kernel(BondedLists L, const int* __restrict__ slot_of, const typename VT<T>::T4* __restrict__ pos4,
-                  typename VT<T>::T4* __restrict__ f4, BoxT box, double* __restrict__ partial) {
+                  typename VT<T>::T4* __restrict__ f4, B box, double* __restrict__ partial) {
     int blk = blockIdx.x;
     double e = 0;
     if (blk < L.nblk[0]) {
-        e = bond_term<T, ENERGY>(blk * BONDED_THREADS + threadIdx.x, L.n[0], L.idx[0], static_cast<const T*>(L.par[0]), slot_of, pos4, f4, box);
+        e = bond_term<T, ENERGY, B>(blk * BONDED_THREADS + threadIdx.x, L.n[0], L.idx[0], static_cast<const T*>(L.par[0]), slot_of, pos4, f4, box);
     } else if (blk < L.nblk[0] + L.nblk[1]) {
         blk -= L.nblk[0];
-        e = angle_term<T, ENERGY>(blk * BONDED_THREADS + threadIdx.x, L.n[1], L.idx[1], static_cast<const T*>(L.par[1]), slot_of, pos4, f4, box);
+        e = angle_term<T, ENERGY, B>(blk * BONDED_THREADS + threadIdx.x, L.n[1], L.idx[1], static_cast<const T*>(L.par[1]), slot_of, pos4, f4, box);
     } else {
         blk -= L.nblk[0] + L.nblk[1];
-        e = torsion_term<T, ENERGY>(blk * BONDED_THREADS + threadIdx.x, L.n[2], L.idx[2], static_cast<const T*>(L.par[2]), slot_of, pos4, f4, box);
+        e = torsion_term<T, ENERGY, B>(blk * BONDED_THREADS + threadIdx.x, L.n[2], L.idx[2], static_cast<const T*>(L.par[2]), slot_of, pos4, f4, box);
     }
     if (ENERGY) block_energy<T>(e, partial);
 }

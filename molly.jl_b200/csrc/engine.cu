@@ -530,8 +530,20 @@ class Engine : public EngineBase {
         }
         const double min_box = std::min(box_[0], std::min(box_[1], box_[2]));
         path_ = (all_nl && r_list_ > 0 && min_box >= 2.5 * r_list_ && n_ >= 64 && !tric_.on) ? 1 : 0;
-        if (tric_.on && (has_lists() || pme_on_))
-            return set_error(MB_ERR_INVALID, "TriclinicBoundary: specific interaction lists and PME are not supported by this engine");
+        if (tric_.on && pme_on_) return set_error(MB_ERR_INVALID, "TriclinicBoundary: PME is not supported by this engine");
+        if (tric_.on && has_lists() && all_nl && r_list_ > 0 && n_ >= 64) {
+            // A system this large would take the cell-list path in a rectangular box; the cell-list path does not handle
+            // triclinic boxes, so its pairs would run on the O(N^2) no-list kernel. Bonded terms in a triclinic box are served
+            // only where the no-list kernel is the intended path (box heights below 2.5 r_list).
+            const double ax = tric_.bv[0][0], bx = tric_.bv[1][0], by = tric_.bv[1][1];
+            const double cx = tric_.bv[2][0], cy = tric_.bv[2][1], cz = tric_.bv[2][2];
+            const double vol = ax * by * cz;
+            const double h0 = vol / std::sqrt(by * cz * by * cz + bx * cz * bx * cz + (bx * cy - by * cx) * (bx * cy - by * cx));
+            const double h1 = vol / (ax * std::sqrt(cz * cz + cy * cy));
+            if (std::min(h0, std::min(h1, cz)) >= 2.5 * r_list_)
+                return set_error(MB_ERR_INVALID, "TriclinicBoundary: specific interaction lists in a box this large need the cell-list "
+                                                 "path, which does not support triclinic boxes yet");
+        }
         if (tric_.on && decomposed()) return set_error(MB_ERR_INVALID, "TriclinicBoundary: not available in decomposed (multi-GPU) runs");
         if (path_ == 1 && max_rc > r_list_)
             return set_error(MB_ERR_INVALID, "neighbour list radius is smaller than an interaction cutoff");
@@ -852,8 +864,15 @@ class Engine : public EngineBase {
             total_blk += L.nblk[kind];
         }
         if (total_blk > 0) {
-            if (energy) bonded_kernel<T, true><<<total_blk, BONDED_THREADS, 0, stream_>>>(L, slot_of, d_pos4_.as<T4>(), d_f4_.as<T4>(), bx, part);
-            else bonded_kernel<T, false><<<total_blk, BONDED_THREADS, 0, stream_>>>(L, slot_of, d_pos4_.as<T4>(), d_f4_.as<T4>(), bx, part);
+            const T4* pos = d_pos4_.as<T4>();
+            T4* f4 = d_f4_.as<T4>();
+            if (tric_.on) {
+                if (energy) bonded_kernel<T, true, Tric<T>><<<total_blk, BONDED_THREADS, 0, stream_>>>(L, slot_of, pos, f4, tric_, part);
+                else bonded_kernel<T, false, Tric<T>><<<total_blk, BONDED_THREADS, 0, stream_>>>(L, slot_of, pos, f4, tric_, part);
+            } else {
+                if (energy) bonded_kernel<T, true, BoxT><<<total_blk, BONDED_THREADS, 0, stream_>>>(L, slot_of, pos, f4, bx, part);
+                else bonded_kernel<T, false, BoxT><<<total_blk, BONDED_THREADS, 0, stream_>>>(L, slot_of, pos, f4, bx, part);
+            }
             launches_++;
             if (energy) {
                 sum_partials_kernel<<<1, 256, 0, stream_>>>(total_blk, part, d_sp_energy_.as<double>());
