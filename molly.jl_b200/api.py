@@ -472,14 +472,27 @@ def _ptr(a):
 # ------------------------------------------------------------------------------------------------
 # functions
 # ------------------------------------------------------------------------------------------------
+def _evaluate(call, *outputs):
+    """Run one evaluation through the C ABI. MB_ERR_CAPACITY means a neighbour-structure capacity overflowed for these
+    coordinates (an atom cloud that moved into a face or gathered since the last call): the outputs are invalid, and the
+    engine re-derives its capacities on the next call. The outputs accumulate (ADD semantics), so they are cleared and the
+    evaluation runs once more, as simulate does."""
+    rc = call()
+    if rc == capi.MB_ERR_CAPACITY:
+        for a in outputs:
+            a[...] = 0
+        rc = call()
+    capi.check(rc)
+
+
 def forces(sys: System, neighbors=None, step_n: int = 0) -> np.ndarray:
     """forces(sys[, neighbors, step_n]) — src/force.jl:678-687. Returns (n,3) in kJ mol^-1 nm^-1."""
     ctx = sys.engine()
     fs = np.zeros((sys.n, 3), sys.dtype)
     if sys.specific_inter_lists or sys.general_inters:  # forces(sys) sums pairwise + specific + general interactions
-        capi.check(sys._L.mb_forces_energy_all(ctx, _ptr(sys.coords), fs.ctypes.data, None, step_n))
+        _evaluate(lambda: sys._L.mb_forces_energy_all(ctx, _ptr(sys.coords), fs.ctypes.data, None, step_n), fs)
     else:
-        capi.check(sys._L.mb_forces(ctx, _ptr(sys.coords), fs.ctypes.data, None, step_n))
+        _evaluate(lambda: sys._L.mb_forces(ctx, _ptr(sys.coords), fs.ctypes.data, None, step_n), fs)
     return fs
 
 
@@ -491,7 +504,7 @@ def forces_virial(sys: System, neighbors=None, step_n: int = 0):
     ctx = sys.engine()
     fs = np.zeros((sys.n, 3), sys.dtype)
     vir = np.zeros(9, sys.dtype)
-    capi.check(sys._L.mb_forces(ctx, _ptr(sys.coords), fs.ctypes.data, vir.ctypes.data, step_n))
+    _evaluate(lambda: sys._L.mb_forces(ctx, _ptr(sys.coords), fs.ctypes.data, vir.ctypes.data, step_n), fs, vir)
     return fs, vir.reshape(3, 3).T.copy()
 
 
@@ -500,9 +513,9 @@ def potential_energy(sys: System, neighbors=None, step_n: int = 0) -> float:
     ctx = sys.engine()
     pe = np.zeros(1, sys.dtype)
     if sys.specific_inter_lists or sys.general_inters:  # potential_energy(sys): pairwise + specific + general
-        capi.check(sys._L.mb_forces_energy_all(ctx, _ptr(sys.coords), None, pe.ctypes.data, step_n))
+        _evaluate(lambda: sys._L.mb_forces_energy_all(ctx, _ptr(sys.coords), None, pe.ctypes.data, step_n), pe)
     else:
-        capi.check(sys._L.mb_energy(ctx, _ptr(sys.coords), pe.ctypes.data, step_n))
+        _evaluate(lambda: sys._L.mb_energy(ctx, _ptr(sys.coords), pe.ctypes.data, step_n), pe)
     return float(pe[0])
 
 
@@ -512,9 +525,9 @@ def forces_energy(sys: System, step_n: int = 0):
     fs = np.zeros((sys.n, 3), sys.dtype)
     pe = np.zeros(1, sys.dtype)
     if sys.specific_inter_lists or sys.general_inters:
-        capi.check(sys._L.mb_forces_energy_all(ctx, _ptr(sys.coords), fs.ctypes.data, pe.ctypes.data, step_n))
+        _evaluate(lambda: sys._L.mb_forces_energy_all(ctx, _ptr(sys.coords), fs.ctypes.data, pe.ctypes.data, step_n), fs, pe)
     else:
-        capi.check(sys._L.mb_forces_energy(ctx, _ptr(sys.coords), fs.ctypes.data, pe.ctypes.data, None, step_n))
+        _evaluate(lambda: sys._L.mb_forces_energy(ctx, _ptr(sys.coords), fs.ctypes.data, pe.ctypes.data, None, step_n), fs, pe)
     return fs, float(pe[0])
 
 

@@ -36,7 +36,10 @@ struct Control {
     int max_halo;
     int max_special;
     int n_ext;          // atoms + ghost copies in the extended array of the last build
-    int pad2_;          // (keeps rebuild_every .. call_max_disp2_bits a 48-byte tail the host uploads in one copy)
+    // largest n_ghost / n_ext / max_halo / max_icount / max_neighbors of any rebuild since the first build. The counters
+    // keep counting past a capacity, so after an overflow these size the next first build. (Five ints: they keep
+    // rebuild_every .. call_max_disp2_bits a 48-byte tail the host uploads in one copy.)
+    int peak_ghost, peak_ext, peak_halo, peak_icount, peak_neighbors;
     unsigned int ticket;  // last-block-done counter
     int rebuild_every;    // fixed-interval policy (0 = displacement-triggered)
     long long step;       // MD step counter (simulate!'s step_n), advanced on the device
@@ -837,6 +840,11 @@ __global__ void rebuild_finish_kernel(Control* ctl) {
         ctl->disp = 0;
         ctl->rebuild = 0;
         ctl->n_rebuilds++;
+        ctl->peak_ghost = max(ctl->peak_ghost, ctl->n_ghost);
+        ctl->peak_ext = max(ctl->peak_ext, ctl->n_ext);
+        ctl->peak_halo = max(ctl->peak_halo, ctl->max_halo);
+        ctl->peak_icount = max(ctl->peak_icount, ctl->max_icount);
+        ctl->peak_neighbors = max(ctl->peak_neighbors, ctl->max_neighbors);
         if (ctl->max_disp2_bits > ctl->call_max_disp2_bits) ctl->call_max_disp2_bits = ctl->max_disp2_bits;
         ctl->max_disp2_bits = 0;
     }

@@ -660,6 +660,7 @@ class Engine : public EngineBase {
         for (size_t i = 0; i + 1 < sp_ptr_.size(); i++) max_special_host_ = std::max(max_special_host_, sp_ptr_[i + 1] - sp_ptr_[i]);
         const int vvb = (int)((n_ + VV_THREADS - 1) / VV_THREADS);
         MB_CUDA(d_partial_.ensure((size_t)std::max(vvb, 2048) * 8 * sizeof(double)));
+        floor_ = CapFloor();
         have_list_ = false;
         dirty_ = false;
         return MB_OK;
@@ -776,9 +777,16 @@ class Engine : public EngineBase {
         const size_t budget = (ctas_per_sm > 1) ? sm_total / ctas_per_sm - 1024 - static_bytes : smem_optin_ - static_bytes;
         nbuf = (int)std::min<size_t>(FORCE_MAX_STAGES, std::max<size_t>(1, budget / stage));
     }
-    size_t build_smem_bytes() const {
-        return (size_t)g_.halo_cap * (sizeof(T4) + sizeof(int)) + (size_t)((g_.hcells + 3) & ~3) * sizeof(ushort2) +
-               (size_t)g_.n_irows * sizeof(IRow);
+    static size_t build_smem_bytes(int halo_cap, int hcells, int n_irows) {
+        return (size_t)halo_cap * (sizeof(T4) + sizeof(int)) + (size_t)((hcells + 3) & ~3) * sizeof(ushort2) +
+               (size_t)n_irows * sizeof(IRow);
+    }
+    size_t build_smem_bytes() const { return build_smem_bytes(g_.halo_cap, g_.hcells, g_.n_irows); }
+    // shared memory the force kernel (one stage) and the list builder need for bricks of b cells with these capacities
+    size_t brick_smem_need(int halo_cap, int task_cap, const int b[3]) const {
+        const int hc = (b[0] + 2 * g_.h) * (b[1] + 2 * g_.h) * (b[2] + 2 * g_.h);
+        return std::max(force_stage_bytes<T>(halo_cap, task_cap, P_.uniform_lj != 0) + 2048,
+                        build_smem_bytes(halo_cap, hc, b[1] * b[2]) + 1024);
     }
 
     int alloc_brick_tables() {
@@ -1339,7 +1347,9 @@ class Engine : public EngineBase {
                                                       d_mass_in_.as<T>(), d_pos4_.as<T4>(), d_vel4_.as<T4>(), d_lj2_.as<T2>(),
                                                       d_orig_.as<int>(), d_inv_orig_.as<int>(), d_mass_.as<T>(), d_xref4_.as<T4>());
         launches_++;
-        for (int attempt = 0; attempt < 8; attempt++) {
+        static const int zeros[5] = {0, 0, 0, 0, 0};  // peak_ghost .. peak_neighbors
+        MB_CUDA(cudaMemcpyAsync(&d_ctl_.as<Control>()->peak_ghost, zeros, sizeof(zeros), cudaMemcpyHostToDevice, stream_));
+        for (;;) {  // ends: every retry makes the brick smaller, and a single cell that does not fit is refused
             MB_TRY(choose_geometry());
             MB_TRY(alloc_brick_tables());
             // pass A: sort + tables with unlimited halo capacity to measure
@@ -1353,14 +1363,41 @@ class Engine : public EngineBase {
             MB_TRY(enqueue_rebuild(false, true));
             Control c;
             MB_TRY(read_ctl(c));
-            int cap = (int)(c.max_halo * (1.0 + 0.08 * cap_scale_)) + 32;  // temporal drift of the fullest brick's halo
+            // measured sizes, but at least those of a rebuild that overflowed the previous capacities (floor_)
+            const int hvol = g_.hcells, bvol = g_.b[0] * g_.b[1] * g_.b[2];
+            const double max_halo = std::max((double)c.max_halo, std::ceil(floor_.halo_per_hcell * hvol));
+            const double max_icount = std::max((double)c.max_icount, std::ceil(floor_.icount_per_cell * bvol));
+            int cap = (int)(max_halo * (1.0 + 0.08 * cap_scale_)) + 32;  // temporal drift of the fullest brick's halo
             cap = (cap + 63) & ~63;
             g_.halo_cap = std::min(cap, LIST_MAX_HALO);
-            g_.task_cap = (((int)(c.max_icount * (1.0 + 0.08 * cap_scale_)) + 8) + 1) & ~1;  // even: 16-byte rows for the bulk copy
+            g_.task_cap = (((int)(max_icount * (1.0 + 0.08 * cap_scale_)) + 8) + 1) & ~1;  // even: 16-byte rows for the bulk copy
+            if (cap > LIST_MAX_HALO || brick_smem_need(g_.halo_cap, g_.task_cap, g_.b) > smem_optin_) {
+                // List entries are 16-bit byte offsets of float4 records, and a stage must fit in shared memory. Pick the
+                // next brick from the measurement: the fullest halo's atoms per halo cell (and the fullest brick's owned
+                // atoms per cell) times the cells of a smaller brick, shrinking its largest dimension until that fits.
+                if (g_.b[0] == 1 && g_.b[1] == 1 && g_.b[2] == 1)
+                    return set_error(MB_ERR_CAPACITY, "halo of a single cell does not fit in shared memory (density too high for r_list)");
+                const double per_hcell = (double)cap / hvol, per_cell = (double)g_.task_cap / bvol;
+                int cur[3] = {g_.b[0], g_.b[1], g_.b[2]};
+                for (;;) {
+                    int dmax = 0;
+                    for (int d = 1; d < 3; d++) if (cur[d] > cur[dmax]) dmax = d;
+                    cur[dmax]--;
+                    if (cur[0] == 1 && cur[1] == 1 && cur[2] == 1) break;
+                    const int hc = (cur[0] + 2 * g_.h) * (cur[1] + 2 * g_.h) * (cur[2] + 2 * g_.h);
+                    const int est_cap = ((int)std::ceil(per_hcell * hc) + 63) & ~63;
+                    const int est_task = ((int)std::ceil(per_cell * cur[0] * cur[1] * cur[2]) + 1) & ~1;
+                    if (est_cap <= LIST_MAX_HALO && brick_smem_need(est_cap, est_task, cur) <= smem_optin_) break;
+                }
+                for (int d = 0; d < 3; d++) user_b_[d] = cur[d];
+                continue;
+            }
             MB_CUDA(d_task_tab_.ensure((size_t)g_.nbricks * g_.task_cap * sizeof(int2)));
             // extended array / ghost table: measured sizes plus room for the boundary cells' population to drift
-            g_.ext_cap = (int)std::min<double>(2.0e9, c.n_ext + (c.n_ext - (double)n_) * 0.10 * cap_scale_ + 1024);
-            g_.ghost_cap = (int)std::min<double>(2.6e8, c.n_ghost * (1.0 + 0.10 * cap_scale_) + 1024);
+            const double n_ext = std::max((double)c.n_ext, (double)floor_.ext);
+            const double n_ghost = std::max((double)c.n_ghost, (double)floor_.ghost);
+            g_.ext_cap = (int)std::min<double>(2.0e9, n_ext + (n_ext - (double)n_) * 0.10 * cap_scale_ + 1024);
+            g_.ghost_cap = (int)std::min<double>(2.6e8, n_ghost * (1.0 + 0.10 * cap_scale_) + 1024);
             MB_CUDA(d_pos4e_.ensure(((size_t)g_.ext_cap + 64) * sizeof(T4)));
             MB_CUDA(cudaMemsetAsync(d_pos4e_.p, 0, ((size_t)g_.ext_cap + 64) * sizeof(T4), stream_));
             if (!P_.uniform_lj) {
@@ -1369,23 +1406,11 @@ class Engine : public EngineBase {
             }
             if (!(ex_ptr_.empty() && sp_ptr_.empty())) MB_CUDA(d_orig_e_.ensure(((size_t)g_.ext_cap + 64) * sizeof(int)));
             MB_CUDA(d_ghosts_.ensure(((size_t)g_.ghost_cap + 64) * sizeof(int2)));
-            size_t need = std::max(force_stage() + 2048, build_smem_bytes() + 1024);
-            if (cap > LIST_MAX_HALO || need > smem_optin_) {  // list entries are 16-bit byte offsets of float4 records
-                // shrink the brick and retry
-                int* ub = user_b_;
-                int cur[3] = {g_.b[0], g_.b[1], g_.b[2]};
-                int dmax = 0;
-                for (int d = 1; d < 3; d++) if (cur[d] > cur[dmax]) dmax = d;
-                if (cur[dmax] == 1) return set_error(MB_ERR_CAPACITY, "halo of a single cell does not fit in shared memory (density too high for r_list)");
-                cur[dmax]--;
-                for (int d = 0; d < 3; d++) ub[d] = cur[d];
-                continue;
-            }
             // pass B: the pipeline again (idempotent: the positions are sorted) now that the extended array exists, with the
             // list builder only counting neighbours (the rebuild flag is still set because finish did not run)
             MB_TRY(enqueue_rebuild(true, true));
             MB_TRY(read_ctl(c));
-            int stride = (int)(c.max_neighbors * (1.0 + 0.10 * cap_scale_)) + 16;
+            int stride = (int)(std::max(c.max_neighbors, floor_.neighbors) * (1.0 + 0.10 * cap_scale_)) + 16;
             stride = (stride + 31) & ~31;
             g_.stride = std::max(stride, 32);
             g_.sstride = std::max(8, (std::max(c.max_special, max_special_host_) + 7) & ~7);
@@ -1405,7 +1430,6 @@ class Engine : public EngineBase {
             }
             return MB_OK;
         }
-        return set_error(MB_ERR_CAPACITY, "could not find a brick size that fits in shared memory");
     }
 
     // ------------------------------------------------------------------------------------------
@@ -1539,7 +1563,15 @@ class Engine : public EngineBase {
         Control c;
         MB_TRY(read_ctl(c));
         if (c.overflow) {
-            have_list_ = false;  // next call re-derives capacities
+            have_list_ = false;  // next call re-derives capacities, with room for what overflowed
+            // The next first build measures the configuration it is given, which for a retry of mb_simulate_vv is the
+            // start of the run that overflowed. The peaks of that run become floors, the halo and owned-atom counts
+            // per cell so that they also apply when the next build picks a different brick.
+            floor_.ghost = std::max(floor_.ghost, c.peak_ghost);
+            floor_.ext = std::max(floor_.ext, c.peak_ext);
+            floor_.neighbors = std::max(floor_.neighbors, c.peak_neighbors);
+            floor_.halo_per_hcell = std::max(floor_.halo_per_hcell, (double)c.peak_halo / g_.hcells);
+            floor_.icount_per_cell = std::max(floor_.icount_per_cell, (double)c.peak_icount / (g_.b[0] * g_.b[1] * g_.b[2]));
             static const int zero = 0;
             cudaMemcpyAsync(&d_ctl_.as<Control>()->overflow, &zero, sizeof(int), cudaMemcpyHostToDevice, stream_);
             return set_error(MB_ERR_CAPACITY, "neighbour/halo capacity overflow; results of this call are invalid, retry");
@@ -2112,6 +2144,12 @@ class Engine : public EngineBase {
     double r_list_ = 0, skin_ = 0, cap_scale_ = 1.0, total_mass_ = 0;
     int rebuild_every_ = 0;
     int user_b_[3] = {0, 0, 0};
+    // lower bounds for the capacities of the next first build, from rebuilds that overflowed (check_overflow_sync);
+    // cleared when the system changes
+    struct CapFloor {
+        int ghost = 0, ext = 0, neighbors = 0;
+        double halo_per_hcell = 0, icount_per_cell = 0;
+    } floor_;
     bool dirty_ = true, have_list_ = false;
     int cutm_ = CUTM_PLAIN;  // cutoff family of the kernel variant (pair.cuh)
     int path_ = 0;

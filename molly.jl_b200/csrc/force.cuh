@@ -190,7 +190,6 @@ __global__ void __launch_bounds__(FORCE_THREADS, (sizeof(T) == 8) ? 1 : FORCE_CT
         // =============================== consumer warps ===============================
         const int sub4 = lane >> 3, l = lane & 7;
         constexpr int LIST_HALF = 4;  // list words (4 entries each) per lane and half batch: 8 words in flight
-        const int words_in_row = g.stride >> 5;  // groups a row can hold
         // per-quad state (the stage changes from quad to quad): shared-memory addresses of the staged positions / LJ pairs
         uint32_t s_pos_u32 = 0, s_lj_u32 = 0;
         T4 pi = make4<T>(0, 0, 0, 0);
@@ -310,10 +309,13 @@ __global__ void __launch_bounds__(FORCE_THREADS, (sizeof(T) == 8) ? 1 : FORCE_CT
         };
         uint2 wa[LIST_HALF];
         auto request_first = [&](const QD& qd) {
+            // only the groups this row was written with: a row shorter than the quad's longest one feeds zero words (the
+            // dummy atom) for the rest. The part of the row beyond its padded length holds entries of earlier builds.
+            const int ng = (((qd.packed >> 12) & 0xfff) + 31) >> 5;
             const uint2* p2 = reinterpret_cast<const uint2*>(list + (size_t)max(qd.slot, 0) * g.stride) + l;
 #pragma unroll
             for (int u = 0; u < LIST_HALF; u++)
-                wa[u] = (qd.slot >= 0 && u < words_in_row) ? ldg_stream_u2(p2 + (size_t)u * 8) : make_uint2(0u, 0u);
+                wa[u] = (qd.slot >= 0 && u < ng) ? ldg_stream_u2(p2 + (size_t)u * 8) : make_uint2(0u, 0u);
         };
         QD cur, nxt;
         int r = lookup(0x7fffffff, false, cur);

@@ -36,6 +36,58 @@ def lj_fluid(cells: int, seed: int = 42, jitter: float = 0.01, temp: float = 90.
                 eps=np.full(n, ARGON["eps"]))
 
 
+def _argon(x, box, seed, temp, dtype):
+    rng = np.random.default_rng(seed + 1)
+    n = len(x)
+    v = rng.normal(0.0, np.sqrt(K_B * temp / ARGON["mass"]), (n, 3))
+    v -= v.mean(0)
+    box = np.asarray(box, float)
+    x = x - np.floor(x / box) * box
+    return dict(n=n, box=box, coords=x.astype(dtype), velocities=v.astype(dtype), mass=np.full(n, ARGON["mass"]),
+                charge=np.zeros(n), sigma=np.full(n, ARGON["sigma"]), eps=np.full(n, ARGON["eps"]))
+
+
+def fluid_in_box(box, seed: int = 3, jitter: float = 0.01, temp: float = 90.0, dtype=np.float64):
+    """Argon filling a rectangular box: an FCC lattice of about the reference density, stretched per axis to tile the box."""
+    box = np.asarray(box, float)
+    a = (4.0 / ARGON_DENSITY) ** (1.0 / 3.0)
+    m = np.maximum(1, np.round(box / a)).astype(int)
+    base = np.array([[0, 0, 0], [0.5, 0.5, 0], [0.5, 0, 0.5], [0, 0.5, 0.5]])
+    g = np.stack(np.meshgrid(*[np.arange(k) for k in m], indexing="ij"), -1).reshape(-1, 3)
+    x = (g[:, None, :] + base[None, :, :] + 0.25).reshape(-1, 3) * (box / m)
+    x = x + np.random.default_rng(seed).normal(0.0, jitter, x.shape)
+    return _argon(x, box, seed, temp, dtype)
+
+
+def argon_droplet(radius: float, box, center, seed: int = 5, jitter: float = 0.01, temp: float = 90.0, dtype=np.float64):
+    """A sphere carved out of an FCC argon crystal at the reference density (vacuum around it), wrapped into the box."""
+    box = np.asarray(box, float)
+    a = (4.0 / ARGON_DENSITY) ** (1.0 / 3.0)
+    k = int(np.ceil(radius / a)) + 1
+    x, _ = fcc_lattice(2 * k, a)
+    x = x - k * a + 0.25 * a
+    x = x[np.einsum("ij,ij->i", x, x) <= radius * radius]
+    x = x + np.random.default_rng(seed).normal(0.0, jitter, x.shape) + np.asarray(center, float)
+    return _argon(x, box, seed, temp, dtype)
+
+
+def argon_slab(thickness: float, box, seed: int = 9, dtype=np.float64):
+    """A liquid argon film filling x and y, `thickness` nm thick in z and centred in the box, with vacuum above and below."""
+    box = np.asarray(box, float)
+    f = fluid_in_box([box[0], box[1], thickness], seed=seed, dtype=np.float64)
+    x = f["coords"] + np.array([0.0, 0.0, 0.5 * (box[2] - thickness)])
+    return _argon(x, box, seed, 90.0, dtype)
+
+
+def nearest_partners(sysd, hub: int, count: int, skip=()):
+    """The `count` atoms nearest to atom `hub` (minimum image) that are not `hub` and not in `skip`."""
+    d = sysd["coords"].astype(np.float64) - sysd["coords"][hub].astype(np.float64)
+    d -= sysd["box"] * np.round(d / sysd["box"])
+    order = np.argsort(np.einsum("ij,ij->i", d, d), kind="stable")
+    skip = set(skip) | {hub}
+    return np.array([j for j in order if j not in skip][:count], np.int32)
+
+
 def readme_system(n: int = 100, box: float = 2.0, seed: int = 1, min_dist: float = 0.3, dtype=np.float64):
     """README.md:72-95: place_atoms-style rejection sampling (setup.jl:23-60), T = 298 K."""
     rng = np.random.default_rng(seed)
