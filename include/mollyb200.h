@@ -188,6 +188,37 @@ typedef struct {
 } mb_vv_params_t;
 int mb_simulate_vv(mb_ctx* ctx, void* coords, void* vels, const mb_vv_params_t* p);
 
+/* Device-side loggers for mb_simulate_vv (apply_loggers!, src/loggers.jl:44-56, called by simulate! at init_step and after
+ * every step, src/simulators.jl:575, :657). A step s is recorded when s % interval == 0 (GeneralObservableLogger,
+ * src/loggers.jl:96-102): the steps init_step + 1 .. init_step + n_steps, and init_step itself when log_initial != 0
+ * (run_loggers == true; false for :skipstart). An interval of 0 records nothing of that kind. At a recorded step:
+ *  - energy record (double step, pe, ke): pe = potential_energy(sys) at the positions after the drift of step s
+ *    (pairwise + specific + PME + LJDispersionCorrection, as mb_forces_energy_all); ke = 1/2 sum m v.v of the
+ *    velocities below, summed in double;
+ *  - coordinate frame: n x 3, original atom order, wrapped into the box (as mb_simulate_vv returns them);
+ *  - velocity frame: n x 3, after step s's CM removal and Andersen coupling: the velocities an unlogged call that stops
+ *    at step s returns.
+ * Frames have the context's dtype. Outputs may be host or device pointers; host frames are staged through a bounded
+ * device ring (at most 64 MiB per kind), not n_frames x n. Logging is an observer: the energy is a second evaluation
+ * into a scratch force buffer, so coordinates and velocities are bit-identical to the same call without logging.
+ * The energy evaluation runs on every energy step (its cost is one more force evaluation on those steps). */
+typedef struct {
+    int64_t energy_every;       /* interval of energy records (0 = none) */
+    int64_t coords_every;       /* interval of coordinate frames (0 = none) */
+    int64_t vels_every;         /* interval of velocity frames (0 = none) */
+    int32_t log_initial;        /* also record init_step (run_loggers == true) */
+    int32_t reserved_;
+    double* energies;           /* energy_capacity x 3 doubles: (step, pe, ke) */
+    void* coords;               /* coords_capacity x n x 3 */
+    void* vels;                 /* vels_capacity x n x 3 */
+    int64_t energy_capacity, coords_capacity, vels_capacity;  /* records the outputs hold */
+    int64_t n_energies, n_coords, n_vels;                     /* written back: records of this call */
+} mb_log_t;
+/* mb_simulate_vv that records into `log` (NULL: mb_simulate_vv). MB_ERR_INVALID, before any work, for a negative
+ * interval or capacity, a NULL output with a non-zero interval, a capacity smaller than the records the call writes, and
+ * in decomposed (multi-GPU) runs, which do not log. After MB_ERR_CAPACITY the records are invalid, like the coordinates. */
+int mb_simulate_vv_log(mb_ctx* ctx, void* coords, void* vels, const mb_vv_params_t* p, mb_log_t* log);
+
 /* remove_CM_motion! (ext/MollyCUDAExt.jl:2373; src/spatial.jl:901-929) on an n x 3 velocity array. */
 int mb_remove_cm_motion(mb_ctx* ctx, void* vels);
 /* kinetic_energy (src/energy.jl:56-70): writes 1/2 sum m v.v to *ke_host (double, host). */

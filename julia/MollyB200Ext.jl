@@ -18,6 +18,8 @@ module MollyB200Ext
 using Molly
 using CUDA
 using Random
+using StaticArrays
+using Unitful
 
 const LIB = get(ENV, "MOLLYB200_LIB", joinpath(@__DIR__, "..", "molly.jl_b200", "libmollyb200.so"))
 
@@ -46,6 +48,24 @@ struct MBVVParams
     andersen_prob::Float64
     rng_ctr1::UInt64
     rng_key::UInt64
+end
+
+# mb_log_t; mutable so that ccall can write the record counts back
+mutable struct MBLog
+    energy_every::Int64
+    coords_every::Int64
+    vels_every::Int64
+    log_initial::Int32
+    reserved_::Int32
+    energies::Ptr{Float64}
+    coords::Ptr{Cvoid}
+    vels::Ptr{Cvoid}
+    energy_capacity::Int64
+    coords_capacity::Int64
+    vels_capacity::Int64
+    n_energies::Int64
+    n_coords::Int64
+    n_vels::Int64
 end
 
 const MB_LJ, MB_COULOMB, MB_CRF, MB_EWALD_REAL = Int32(0), Int32(1), Int32(2), Int32(3)
@@ -247,7 +267,9 @@ end
 
 # ---- simulate!(sys, ::VelocityVerlet, n) ----------------------------------------------------------------
 # Taken over only when nothing but the pairwise path contributes forces and nothing has to run on the host
-# every step; loggers fire between chunks of gcd(logger n_steps) steps (SURVEY.md Appendix A.11).
+# every step. When every logger is one the engine records (device_log_kind), the whole run is one mb_simulate_vv_log call
+# and the records are pushed into the loggers' histories afterwards; otherwise loggers fire between chunks of
+# gcd(logger n_steps) steps (SURVEY.md Appendix A.11). Like the rest of this file, this has only been checked by reading.
 function takeover_params(sys, sim::VelocityVerlet, n_steps, init_step, rng)
     # LJDispersionCorrection adds no force (lennard_jones.jl:252-275); anything else (PME, implicit solvent) -> stock path
     all(gi -> gi isa Molly.LJDispersionCorrection, sys.general_inters) || return nothing
@@ -275,6 +297,9 @@ function Molly.simulate!(sys::System{3, <:CuArray, T}, sim::VelocityVerlet, n_st
     end
     ctx = context_for(sys, descs)
     set_specific!(ctx, sys)
+    if run_loggers != false && !isempty(sys.loggers) && all(l -> !isnothing(device_log_kind(l)), values(sys.loggers))
+        return simulate_logged!(sys, ctx, p, n_steps, init_step, run_loggers)
+    end
     chunk = run_loggers == false || isempty(sys.loggers) ? n_steps :
             max(1, reduce(gcd, (l.n_steps for l in values(sys.loggers))))
     done = 0
@@ -287,6 +312,74 @@ function Molly.simulate!(sys::System{3, <:CuArray, T}, sim::VelocityVerlet, n_st
                     ctx.handle, pointer(sys.coords), pointer(sys.velocities), Ref(pp)))
         done += m
         Molly.apply_loggers!(sys, nothing, nothing, init_step + done, run_loggers)
+    end
+    return sys
+end
+
+# The loggers the engine records on the device (src/loggers.jl:134-278): GeneralObservableLoggers whose observable is one
+# of these functions. Others return nothing (chunked path).
+function device_log_kind(l)
+    l isa Molly.GeneralObservableLogger || return nothing
+    f = l.observable
+    f === Molly.potential_energy_wrapper && return :pe
+    f === Molly.kinetic_energy_wrapper && return :ke
+    f === Molly.total_energy_wrapper && return :total
+    f === Molly.temperature_wrapper && return :temp
+    f === Molly.coordinates_wrapper && return :coords
+    f === Molly.velocities_wrapper && return :vels
+    return nothing
+end
+
+# steps a logger of interval `every` is recorded at (simulators.jl:575, :657; loggers.jl:44-56, :96-102)
+function record_steps(every, n_steps, init_step, run_loggers)
+    every <= 0 && return Int[]
+    steps = collect(((init_step ÷ every) + 1) * every:every:(init_step + n_steps))
+    run_loggers == true && init_step % every == 0 && pushfirst!(steps, init_step)
+    return steps
+end
+
+function simulate_logged!(sys::System{3, <:CuArray, T}, ctx, p, n_steps, init_step, run_loggers) where T
+    kinds = Dict(name => device_log_kind(l) for (name, l) in pairs(sys.loggers))
+    gcd_of(sel) = reduce(gcd, (l.n_steps for (name, l) in pairs(sys.loggers) if kinds[name] in sel); init=0)
+    e_every, x_every, v_every = gcd_of((:pe, :ke, :total, :temp)), gcd_of((:coords,)), gcd_of((:vels,))
+    e_steps = record_steps(e_every, n_steps, init_step, run_loggers)
+    x_steps = record_steps(x_every, n_steps, init_step, run_loggers)
+    v_steps = record_steps(v_every, n_steps, init_step, run_loggers)
+    n = length(sys)
+    erec = CUDA.zeros(Float64, 3, max(1, length(e_steps)))   # (step, pe, ke) per column
+    xrec = CUDA.zeros(T, 3, n, max(1, length(x_steps)))
+    vrec = CUDA.zeros(T, 3, n, max(1, length(v_steps)))
+    lg = MBLog(isempty(e_steps) ? 0 : e_every, isempty(x_steps) ? 0 : x_every, isempty(v_steps) ? 0 : v_every,
+               Int32(run_loggers == true), Int32(0),
+               reinterpret(Ptr{Float64}, pointer(erec)), reinterpret(Ptr{Cvoid}, pointer(xrec)),
+               reinterpret(Ptr{Cvoid}, pointer(vrec)), length(e_steps), length(x_steps), length(v_steps), 0, 0, 0)
+    GC.@preserve erec xrec vrec begin
+        check(ccall((:mb_simulate_vv_log, LIB), Cint,
+                    (Ptr{Cvoid}, CuPtr{Cvoid}, CuPtr{Cvoid}, Ref{MBVVParams}, Ref{MBLog}),
+                    ctx.handle, pointer(sys.coords), pointer(sys.velocities), Ref(p), lg))
+    end
+    e = Array(erec)
+    eu, du, vu = sys.energy_units, unit(eltype(eltype(sys.coords))), unit(eltype(eltype(sys.velocities)))
+    for (name, l) in pairs(sys.loggers)
+        k = kinds[name]
+        if k in (:coords, :vels)
+            steps, rec = k == :coords ? (x_steps, xrec) : (v_steps, vrec)
+            for (j, s) in enumerate(steps)
+                s % l.n_steps == 0 || continue
+                frame = reinterpret(SVector{3, T}, vec(rec[:, :, j]))
+                push!(l.history, Array(frame) .* (k == :coords ? du : vu))
+            end
+        else
+            for (j, s) in enumerate(e_steps)
+                s % l.n_steps == 0 || continue
+                pe, ke = e[2, j], e[3, j]
+                v = k == :pe ? pe * eu : k == :ke ? ke * eu : k == :total ? (pe + ke) * eu : 2 * ke * eu / (sys.df * sys.k)
+                if k == :temp && eu != Unitful.NoUnits
+                    v = uconvert(u"K", v)   # temperature(sys), src/energy.jl:158-176
+                end
+                push!(l.history, v)
+            end
+        end
     end
     return sys
 end

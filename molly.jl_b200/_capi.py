@@ -20,6 +20,7 @@ EXPORTED = [
     "mb_stats", "mb_synchronize", "mb_set_capacity_scale", "mb_set_launch_config", "mb_comm_unique_id",
     "mb_comm_init", "mb_decomp_plan", "mb_set_profiling", "mb_set_specific", "mb_forces_energy_all", "mb_set_pme", "mb_pme_plan",
     "mb_set_lj_dispersion_correction", "mb_random_velocities", "mb_kinetic_energy_tensor", "mb_set_box_triclinic",
+    "mb_simulate_vv_log",
 ]
 
 
@@ -49,6 +50,15 @@ class MBVVParams(C.Structure):
     _fields_ = [
         ("dt", C.c_double), ("n_steps", C.c_int64), ("init_step", C.c_int64), ("remove_cm_every", C.c_int32),
         ("andersen_kT", C.c_double), ("andersen_prob", C.c_double), ("rng_ctr1", C.c_uint64), ("rng_key", C.c_uint64),
+    ]
+
+
+class MBLog(C.Structure):
+    _fields_ = [
+        ("energy_every", C.c_int64), ("coords_every", C.c_int64), ("vels_every", C.c_int64), ("log_initial", C.c_int32),
+        ("reserved_", C.c_int32), ("energies", C.c_void_p), ("coords", C.c_void_p), ("vels", C.c_void_p),
+        ("energy_capacity", C.c_int64), ("coords_capacity", C.c_int64), ("vels_capacity", C.c_int64),
+        ("n_energies", C.c_int64), ("n_coords", C.c_int64), ("n_vels", C.c_int64),
     ]
 
 
@@ -87,6 +97,7 @@ def load():
     L.mb_energy.argtypes = [vp, vp, vp, i64]
     L.mb_forces_energy.argtypes = [vp, vp, vp, vp, vp, i64]
     L.mb_simulate_vv.argtypes = [vp, vp, vp, C.POINTER(MBVVParams)]
+    L.mb_simulate_vv_log.argtypes = [vp, vp, vp, C.POINTER(MBVVParams), C.POINTER(MBLog)]
     L.mb_remove_cm_motion.argtypes = [vp, vp]
     L.mb_kinetic_energy.argtypes = [vp, vp, C.POINTER(dbl)]
     L.mb_rebuild_neighbors.argtypes = [vp, vp]

@@ -11,6 +11,8 @@ julia/MollyB200Ext.jl, see INTEGRATION.md):
     VelocityVerlet, AndersenThermostat, simulate    src/simulators.jl:287-295, :547-668; src/coupling.jl:184-212
     forces, forces_virial, potential_energy         src/force.jl:678-720, src/energy.jl:202-248
     kinetic_energy, temperature, remove_CM_motion   src/energy.jl:44-175, src/spatial.jl:901-929
+    *EnergyLogger, TemperatureLogger, Coordinates-  src/loggers.jl:44-102, :134-278 (recorded on the device inside
+    Logger, VelocitiesLogger, values                simulate)
 
 Everything numerical happens in libmollyb200.so on the GPU; this module only marshals arrays.
 Units are Molly's (nm, ps, g/mol, kJ/mol) with the Unitful wrappers stripped.
@@ -18,6 +20,7 @@ Units are Molly's (nm, ps, g/mol, kJ/mol) with the Unitful wrappers stripped.
 from __future__ import annotations
 
 import ctypes as C
+import math
 from dataclasses import dataclass, field
 from typing import Optional, Sequence
 
@@ -340,6 +343,132 @@ class VelocityVerlet:
 
 
 # ------------------------------------------------------------------------------------------------
+# loggers: recorded on the device inside simulate (mb_simulate_vv_log)
+# ------------------------------------------------------------------------------------------------
+class _DeviceLogger:
+    """GeneralObservableLogger (src/loggers.jl:63-102): records at step s when s % n_steps == 0. `history` grows over
+    consecutive simulate calls. For a System with host (numpy) state the entries are numpy values; for a System with
+    torch CUDA state they are CUDA tensors the engine wrote."""
+    kind = ""  # "energy", "coords" or "vels": which engine record the logger reads
+
+    def __init__(self, n_steps: int):
+        if int(n_steps) <= 0:
+            raise ValueError(f"n_steps must be positive, found {n_steps}")
+        self.n_steps = int(n_steps)
+        self.history = []
+
+    def __repr__(self):
+        return f"{type(self).__name__}({self.n_steps}) with {len(self.history)} entries"
+
+
+class PotentialEnergyLogger(_DeviceLogger):
+    """potential_energy(sys) of pairwise + specific + general interactions (src/loggers.jl:251-260)."""
+    kind = "energy"
+
+
+class KineticEnergyLogger(_DeviceLogger):
+    """kinetic_energy(sys) (src/loggers.jl:225-234)."""
+    kind = "energy"
+
+
+class TotalEnergyLogger(_DeviceLogger):
+    """potential + kinetic energy (src/loggers.jl:272-278)."""
+    kind = "energy"
+
+
+class TemperatureLogger(_DeviceLogger):
+    """temperature(sys) with the degrees of freedom of `temperature` (src/loggers.jl:134-143)."""
+    kind = "energy"
+
+
+class CoordinatesLogger(_DeviceLogger):
+    """Coordinates wrapped into the box, original atom order (src/loggers.jl:153-166)."""
+    kind = "coords"
+
+
+class VelocitiesLogger(_DeviceLogger):
+    """Velocities after the step's CM removal and coupling (src/loggers.jl:201-214)."""
+    kind = "vels"
+
+
+def values(logger):
+    """values(logger) — src/loggers.jl:85: the stored observations."""
+    return logger.history
+
+
+def _check_run_loggers(run_loggers):
+    if not (run_loggers is True or run_loggers is False or run_loggers == "skipstart"):
+        raise ValueError(f'run_loggers must be True, False or "skipstart", found {run_loggers!r}')
+
+
+def record_steps(every: int, n_steps: int, init_step: int = 0, run_loggers=True) -> list:
+    """Steps at which simulate(..., n_steps, init_step, run_loggers) records a logger of interval `every`: apply_loggers!
+    runs at init_step only when run_loggers is True (src/simulators.jl:575) and after every step unless it is False
+    (:657, src/loggers.jl:44-56); a logger keeps step s when s % every == 0 (:96-102)."""
+    _check_run_loggers(run_loggers)
+    if every <= 0 or run_loggers is False:
+        return []
+    first = (init_step // every + 1) * every
+    steps = list(range(first, init_step + n_steps + 1, every))
+    if run_loggers is True and init_step % every == 0:
+        steps.insert(0, init_step)
+    return steps
+
+
+_LOG_FIELDS = {"energy": ("energy_every", "energies", "energy_capacity"),
+               "coords": ("coords_every", "coords", "coords_capacity"),
+               "vels": ("vels_every", "vels", "vels_capacity")}
+
+
+class _LogPlan:
+    """One simulate call's records. The engine records each kind (energies, coordinate frames, velocity frames) at the gcd
+    of the intervals of the loggers that read it; each logger then keeps the records of its own steps."""
+
+    def __init__(self, sys, n_steps: int, init_step: int, run_loggers):
+        self.sys = sys
+        self.loggers = list(sys.loggers.values())
+        self.steps, self.buf = {}, {}
+        d = capi.MBLog()
+        d.log_initial = int(run_loggers is True)
+        device = hasattr(sys.coords, "data_ptr")
+        for kind in ("energy", "coords", "vels"):
+            intervals = [lg.n_steps for lg in self.loggers if lg.kind == kind]
+            every = math.gcd(*intervals) if intervals else 0
+            steps = record_steps(every, n_steps, init_step, run_loggers)
+            shape = (len(steps), 3) if kind == "energy" else (len(steps), sys.n, 3)
+            if device:
+                import torch
+                dt = torch.float64 if kind == "energy" else sys.coords.dtype
+                buf = torch.zeros(shape, dtype=dt, device=sys.coords.device)
+            else:
+                buf = np.zeros(shape, np.float64 if kind == "energy" else sys.dtype)
+            self.steps[kind], self.buf[kind] = steps, buf
+            if steps:  # (an interval with no record in this call is passed as 0)
+                f_every, f_out, f_cap = _LOG_FIELDS[kind]
+                setattr(d, f_every, every)
+                setattr(d, f_out, _ptr(buf))
+                setattr(d, f_cap, len(steps))
+        self.desc = d
+
+    def push(self):
+        """Append this call's records to the loggers' histories (only after the call succeeded)."""
+        e = self.buf["energy"]
+        pe, ke = e[:, 1], e[:, 2]
+        df = 3 * self.sys.n - 3
+        derived = {PotentialEnergyLogger: pe, KineticEnergyLogger: ke, TotalEnergyLogger: pe + ke,
+                   TemperatureLogger: 2.0 * ke / (df * self.sys.k)}
+        for lg in self.loggers:
+            vals = self.buf[lg.kind] if lg.kind != "energy" else derived[type(lg)]
+            for k, s in enumerate(self.steps[lg.kind]):
+                if s % lg.n_steps == 0:
+                    lg.history.append(vals[k])
+
+
+_LOGGER_TYPES = (PotentialEnergyLogger, KineticEnergyLogger, TotalEnergyLogger, TemperatureLogger, CoordinatesLogger,
+                 VelocitiesLogger)
+
+
+# ------------------------------------------------------------------------------------------------
 # System
 # ------------------------------------------------------------------------------------------------
 class System:
@@ -350,7 +479,7 @@ class System:
     """
 
     def __init__(self, atoms, coords, boundary, velocities=None, pairwise_inters=(), neighbor_finder=None,
-                 dtype=np.float32, device: int = 0, k=BOLTZMANN_K, specific_inter_lists=(), general_inters=()):
+                 dtype=np.float32, device: int = 0, k=BOLTZMANN_K, specific_inter_lists=(), general_inters=(), loggers=None):
         self.dtype = np.dtype(dtype)
         if isinstance(atoms, np.ndarray) and atoms.dtype.names:
             self.atoms = np.ascontiguousarray(atoms.astype(atom_dtype(self.dtype)))
@@ -366,6 +495,11 @@ class System:
         self.general_inters = tuple(general_inters)
         self.device = device
         self.k = k
+        self.loggers = dict(loggers or {})
+        for name, lg in self.loggers.items():
+            if type(lg) not in _LOGGER_TYPES:  # (no silent skip: the engine cannot record it)
+                raise TypeError(f"logger {name!r}: {type(lg).__name__} is not supported; the engine records "
+                                + ", ".join(t.__name__ for t in _LOGGER_TYPES))
         self._ctx = None
 
     def _as_state(self, a):
@@ -539,8 +673,11 @@ def find_neighbors(sys: System, *args, **kwargs):
     return None
 
 
-def simulate(sys: System, sim: VelocityVerlet, n_steps: int, init_step: int = 0, rng=None, max_retries: int = 2):
-    """simulate!(sys, sim::VelocityVerlet, n_steps) — src/simulators.jl:547-668. Mutates sys.coords / velocities."""
+def simulate(sys: System, sim: VelocityVerlet, n_steps: int, init_step: int = 0, rng=None, max_retries: int = 2,
+             run_loggers=True):
+    """simulate!(sys, sim::VelocityVerlet, n_steps; run_loggers) — src/simulators.jl:547-668. Mutates sys.coords /
+    velocities and appends to the histories of sys.loggers (recorded on the device, see _LogPlan)."""
+    _check_run_loggers(run_loggers)
     ctx = sys.engine()
     p = capi.MBVVParams()
     p.dt = float(sim.dt)
@@ -561,9 +698,13 @@ def simulate(sys: System, sim: VelocityVerlet, n_steps: int, init_step: int = 0,
     p.rng_key = int(rng.integers(0, 2 ** 63))
     host = not hasattr(sys.coords, "data_ptr")
     backup = (sys.coords.copy(), sys.velocities.copy()) if host else None
+    plan = _LogPlan(sys, int(n_steps), int(init_step), run_loggers) if sys.loggers and run_loggers is not False else None
     scale = 1.0
     for attempt in range(max_retries + 1):
-        rc = sys._L.mb_simulate_vv(ctx, _ptr(sys.coords), _ptr(sys.velocities), C.byref(p))
+        if plan is None:
+            rc = sys._L.mb_simulate_vv(ctx, _ptr(sys.coords), _ptr(sys.velocities), C.byref(p))
+        else:  # a retry overwrites the records of the failed attempt
+            rc = sys._L.mb_simulate_vv_log(ctx, _ptr(sys.coords), _ptr(sys.velocities), C.byref(p), C.byref(plan.desc))
         if rc == capi.MB_ERR_CAPACITY and backup is not None and attempt < max_retries:
             sys.coords[...], sys.velocities[...] = backup
             scale *= 2.0
@@ -571,6 +712,8 @@ def simulate(sys: System, sim: VelocityVerlet, n_steps: int, init_step: int = 0,
             continue
         capi.check(rc)
         break
+    if plan is not None:
+        plan.push()
     return sys
 
 

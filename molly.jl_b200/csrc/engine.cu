@@ -297,7 +297,7 @@ class EngineBase {
                                const int32_t* sj) = 0;
     virtual int set_neighbor_policy(double r_list, int rebuild_every) = 0;
     virtual int forces_energy(const void* coords, void* fs, void* pe, void* vir, int64_t step_n, bool with_specific) = 0;
-    virtual int simulate_vv(void* coords, void* vels, const mb_vv_params_t* p) = 0;
+    virtual int simulate_vv(void* coords, void* vels, const mb_vv_params_t* p, mb_log_t* log) = 0;
     virtual int remove_cm(void* vels) = 0;
     virtual int kinetic_energy(const void* vels, double* out) = 0;
     virtual int rebuild(const void* coords) = 0;
@@ -849,9 +849,10 @@ class Engine : public EngineBase {
     }
     bool has_lists() const { return sp_n_[0] + sp_n_[1] + sp_n_[2] > 0; }
     bool has_specific() const { return has_lists() || pme_on_; }  // everything that is added after the pair kernel
-    // add the bonded forces to f4 (slot order on the brick path, original order on the all-pairs path);
+    // add the bonded forces to f4 (slot order on the brick path, original order on the all-pairs path; default d_f4_);
     // with energy: per-kernel partials are summed into d_sp_energy_ (double, device)
-    int launch_bonded(bool energy) {
+    int launch_bonded(bool energy, T4* f4 = nullptr) {
+        if (!f4) f4 = d_f4_.as<T4>();
         if (!has_specific()) return MB_OK;
         MB_CUDA(d_sp_partial_.ensure(64 * sizeof(double)));  // (set_specific sizes it for the lists; PME alone needs it to exist)
         const int* slot_of = (path_ == 1) ? d_inv_orig_.as<int>() : nullptr;
@@ -873,7 +874,6 @@ class Engine : public EngineBase {
         }
         if (total_blk > 0) {
             const T4* pos = d_pos4_.as<T4>();
-            T4* f4 = d_f4_.as<T4>();
             if (tric_.on) {
                 if (energy) bonded_kernel<T, true, Tric<T>><<<total_blk, BONDED_THREADS, 0, stream_>>>(L, slot_of, pos, f4, tric_, part);
                 else bonded_kernel<T, false, Tric<T>><<<total_blk, BONDED_THREADS, 0, stream_>>>(L, slot_of, pos, f4, tric_, part);
@@ -888,7 +888,7 @@ class Engine : public EngineBase {
             }
         }
         MB_CUDA(cudaGetLastError());
-        if (pme_on_) MB_TRY(launch_pme(energy));
+        if (pme_on_) MB_TRY(launch_pme(energy, f4));
         return MB_OK;
     }
 
@@ -983,7 +983,7 @@ class Engine : public EngineBase {
         pme_ready_ = true;
         return MB_OK;
     }
-    int launch_pme(bool energy) {
+    int launch_pme(bool energy, T4* f4) {
         MB_TRY(pme_prepare());
         const int nb = (int)((n_ + PME_THREADS - 1) / PME_THREADS);
         const size_t total = (size_t)pme_g_.K[0] * pme_g_.K[1] * pme_g_.K[2];
@@ -1006,12 +1006,12 @@ class Engine : public EngineBase {
         if (energy) pme_conv_kernel<T, true><<<conv_blk, PME_THREADS, 0, stream_>>>(pme_g_, f_div, factor, boxfactor, d_pme_bsm_[0].as<double>(), d_pme_bsm_[1].as<double>(), d_pme_bsm_[2].as<double>(), grid, part);
         else pme_conv_kernel<T, false><<<conv_blk, PME_THREADS, 0, stream_>>>(pme_g_, f_div, factor, boxfactor, d_pme_bsm_[0].as<double>(), d_pme_bsm_[1].as<double>(), d_pme_bsm_[2].as<double>(), grid, part);
         MB_TRY(fft(1));
-        pme_interp_kernel<T><<<nb, PME_THREADS, 0, stream_>>>((int)n_, pme_g_, d_pos4_.as<T4>(), grid, d_f4_.as<T4>());
+        pme_interp_kernel<T><<<nb, PME_THREADS, 0, stream_>>>((int)n_, pme_g_, d_pos4_.as<T4>(), grid, f4);
         launches_ += 3;
         if (n_ex > 0) {
             const int* slot_of = (path_ == 1) ? d_inv_orig_.as<int>() : nullptr;
-            if (energy) ewald_exclusion_kernel<T, true><<<ex_blk, PME_THREADS, 0, stream_>>>(n_ex, d_pme_pairs_.as<int>(), slot_of, d_pos4_.as<T4>(), d_f4_.as<T4>(), pme_g_, pme_alpha_, f_div, part + conv_blk);
-            else ewald_exclusion_kernel<T, false><<<ex_blk, PME_THREADS, 0, stream_>>>(n_ex, d_pme_pairs_.as<int>(), slot_of, d_pos4_.as<T4>(), d_f4_.as<T4>(), pme_g_, pme_alpha_, f_div, part + conv_blk);
+            if (energy) ewald_exclusion_kernel<T, true><<<ex_blk, PME_THREADS, 0, stream_>>>(n_ex, d_pme_pairs_.as<int>(), slot_of, d_pos4_.as<T4>(), f4, pme_g_, pme_alpha_, f_div, part + conv_blk);
+            else ewald_exclusion_kernel<T, false><<<ex_blk, PME_THREADS, 0, stream_>>>(n_ex, d_pme_pairs_.as<int>(), slot_of, d_pos4_.as<T4>(), f4, pme_g_, pme_alpha_, f_div, part + conv_blk);
             launches_++;
         }
         if (energy) {
@@ -1458,12 +1458,12 @@ class Engine : public EngineBase {
         if (cutm_ == CUTM_SHIFTED) return energy ? launch_force_t<COUL, UNIFORM, CUTM_SHIFTED, true>(out, b0, nbr) : launch_force_t<COUL, UNIFORM, CUTM_SHIFTED, false>(out, b0, nbr);
         return energy ? launch_force_t<COUL, UNIFORM, CUTM_PLAIN, true>(out, b0, nbr) : launch_force_t<COUL, UNIFORM, CUTM_PLAIN, false>(out, b0, nbr);
     }
-    // owned_only: in a decomposed run the step loop evaluates only this rank's slab of bricks
-    int launch_force(bool energy, bool owned_only = false) {
+    // owned_only: in a decomposed run the step loop evaluates only this rank's slab of bricks; f4: force target (default d_f4_)
+    int launch_force(bool energy, bool owned_only = false, T4* f4 = nullptr) {
         const int b0 = owned_only ? own_b0_ : 0;
         const int nbr = owned_only ? own_nb_ : g_.nbricks;
         ForceOut<T> out;
-        out.f4 = d_f4_.as<T4>();
+        out.f4 = f4 ? f4 : d_f4_.as<T4>();
         out.pe_partial = d_pe_partial_.as<double>();
         out.vir_partial = d_pe_partial_.as<double>() + std::max(g_.nbricks, 4 * sm_count_);
         out.gate = gate_;  // one-shot: set by the decomposed step in front of this launch
@@ -1676,7 +1676,7 @@ class Engine : public EngineBase {
     };
     int enqueue_step(const StepCfg& c, int do_cm_now, bool clear_cm_after_k1, bool capture,
                      cudaGraphConditionalHandle handle, cudaGraph_t graph, cudaGraph_t* body_out, bool host_rebuild_hint,
-                     bool defer_cm = false) {
+                     bool defer_cm = false, int log_mask = 0) {
         const bool dec = decomposed() && path_ == 1;
         const int s0 = dec ? own_s0_ : 0, n_own = dec ? own_n_ : (int)n_;
         const int nb = std::max(1, (n_own + 255) / 256);
@@ -1775,6 +1775,33 @@ class Engine : public EngineBase {
             andersen_kernel<T><<<nb2, 256, 0, stream_>>>(s0b, n_ownb, (int)n_, c.kT, c.prob, d_orig_.as<int>(), d_mass_.as<T>(), d_vel4_.as<T4>(), cm, ctl);
             launches_++;
         }
+        if (log_mask) MB_TRY(enqueue_log(c, log_mask));
+        MB_CUDA(cudaGetLastError());
+        return MB_OK;
+    }
+    // Record the state after the current step (LOG_* mask; single-GPU runs). The energy is a second evaluation at the same
+    // positions by the ENERGY variants into a scratch force buffer: the trajectory keeps the forces of the plain kernels,
+    // so logging does not change it.
+    int enqueue_log(const StepCfg& c, int mask) {
+        int n_pe = 0;
+        if (mask & LOG_ENERGY) {
+            T4* scratch = d_f4_log_.as<T4>();
+            if (path_ == 0) {
+                MB_TRY(launch_allpairs(true, d_pos4_.as<T4>(), d_lj2_.as<T2>(), scratch));
+                n_pe = (int)((n_ + AP_THREADS - 1) / AP_THREADS);
+            } else {
+                MB_TRY(launch_force(true, false, scratch));
+                n_pe = force_grid_;
+            }
+            MB_TRY(launch_bonded(true, scratch));
+        }
+        const int nb = (int)((n_ + LOG_THREADS - 1) / LOG_THREADS);
+        log_kernel<T><<<nb, LOG_THREADS, 0, stream_>>>((int)n_, mask, path_ == 0 ? g_ap_ : g_, d_pos4_.as<T4>(), d_vel4_.as<T4>(),
+                                                       d_orig_.as<int>(), d_mass_.as<T>(), d_cm_.as<CmState<T>>(), d_ctl_.as<Control>(),
+                                                       thermo_in_k1(c), d_pe_partial_.as<double>(), n_pe,
+                                                       has_specific() ? d_sp_energy_.as<double>() : nullptr,
+                                                       d_log_desc_.as<LogDesc<T>>(), d_log_part_.as<double>());
+        launches_++;
         MB_CUDA(cudaGetLastError());
         return MB_OK;
     }
@@ -1794,24 +1821,40 @@ class Engine : public EngineBase {
         return th;
     }
 
+    // log_mask: the LOG_* records the step graph ends with (0: a plain step). The logging kernel's destinations are read from
+    // the device descriptor (d_log_desc_), so they are not part of the key.
     struct GraphKey {
-        int path, do_cm, thermostat, geom_version, rebuild_every;
+        int path, do_cm, thermostat, geom_version, rebuild_every, log_mask;
         double dt, kT, prob;
         int64_t n;
         bool operator==(const GraphKey& o) const {
             return path == o.path && do_cm == o.do_cm && thermostat == o.thermostat && geom_version == o.geom_version &&
-                   rebuild_every == o.rebuild_every && dt == o.dt && kT == o.kT && prob == o.prob && n == o.n;
+                   rebuild_every == o.rebuild_every && log_mask == o.log_mask && dt == o.dt && kT == o.kT && prob == o.prob && n == o.n;
         }
     };
-    void destroy_graph() {
-        if (graph_exec_) cudaGraphExecDestroy(graph_exec_);
-        if (graph_) cudaGraphDestroy(graph_);
-        graph_exec_ = nullptr;
-        graph_ = nullptr;
+    // one executable step graph per log mask; the host loop picks one per step
+    struct StepGraph {
+        cudaGraph_t graph = nullptr;
+        cudaGraphExec_t exec = nullptr;
+        GraphKey key;
+        int64_t launches = 0;  // kernels per step outside the rebuild body
+    };
+    void destroy_graph(int mask) {
+        StepGraph& sg = graphs_[mask];
+        if (sg.exec) cudaGraphExecDestroy(sg.exec);
+        if (sg.graph) cudaGraphDestroy(sg.graph);
+        sg.exec = nullptr;
+        sg.graph = nullptr;
     }
-    // Capture one MD step (K1, decide, [IF rebuild], force, K2, [thermostat]) into an executable graph.
+    void destroy_graph() {
+        for (int m = 0; m < 8; m++) destroy_graph(m);
+    }
+    // Capture one MD step (K1, decide, [IF rebuild], force, K2, [thermostat], [log records]) into an executable graph.
     int build_step_graph(const StepCfg& c, const GraphKey& key) {
-        destroy_graph();
+        const int mask = key.log_mask;
+        destroy_graph(mask);
+        cudaGraph_t& gr = graphs_[mask].graph;
+        cudaGraphExec_t& gx = graphs_[mask].exec;
         const bool prof_was = prof_.enabled;
         prof_.enabled = false;
         const int64_t launches_before = launches_;
@@ -1822,19 +1865,19 @@ class Engine : public EngineBase {
                 cudaStreamEndCapture(stream_, &junk);
             }
             cudaGetLastError();
-            destroy_graph();
+            destroy_graph(mask);
             prof_.enabled = prof_was;
             launches_ = launches_before;
             return rc;
         };
-        if (cudaGraphCreate(&graph_, 0) != cudaSuccess) return fail(MB_ERR_CUDA);
+        if (cudaGraphCreate(&gr, 0) != cudaSuccess) return fail(MB_ERR_CUDA);
         cudaGraphConditionalHandle handle = 0;
-        if (path_ == 1 && cudaGraphConditionalHandleCreate(&handle, graph_, 0, cudaGraphCondAssignDefault) != cudaSuccess)
+        if (path_ == 1 && cudaGraphConditionalHandleCreate(&handle, gr, 0, cudaGraphCondAssignDefault) != cudaSuccess)
             return fail(MB_ERR_CUDA);
-        if (cudaStreamBeginCaptureToGraph(stream_, graph_, nullptr, nullptr, 0, cudaStreamCaptureModeRelaxed) != cudaSuccess)
+        if (cudaStreamBeginCaptureToGraph(stream_, gr, nullptr, nullptr, 0, cudaStreamCaptureModeRelaxed) != cudaSuccess)
             return fail(MB_ERR_CUDA);
         cudaGraph_t body = nullptr;
-        if (enqueue_step(c, c.do_cm, false, true, handle, graph_, &body, false) != MB_OK) return fail(MB_ERR_CUDA);
+        if (enqueue_step(c, c.do_cm, false, true, handle, gr, &body, false, false, mask) != MB_OK) return fail(MB_ERR_CUDA);
         cudaGraph_t out = nullptr;
         if (cudaStreamEndCapture(stream_, &out) != cudaSuccess) return fail(MB_ERR_CUDA);
         const int64_t step_nodes = launches_ - launches_before;
@@ -1845,18 +1888,51 @@ class Engine : public EngineBase {
             if (enqueue_rebuild(true, false) != MB_OK) return fail(MB_ERR_CUDA);
             if (cudaStreamEndCapture(stream_, &out) != cudaSuccess) return fail(MB_ERR_CUDA);
         }
-        if (cudaGraphInstantiate(&graph_exec_, graph_, 0) != cudaSuccess) return fail(MB_ERR_CUDA);
+        if (cudaGraphInstantiate(&gx, gr, 0) != cudaSuccess) return fail(MB_ERR_CUDA);
         prof_.enabled = prof_was;
         launches_ = launches_before;
-        graph_step_launches_ = step_nodes;
-        graph_key_ = key;
+        graphs_[mask].launches = step_nodes;
+        graphs_[mask].key = key;
         return MB_OK;
     }
 
-    int simulate_vv(void* coords, void* vels, const mb_vv_params_t* p) override {
+    // records of one interval in a call: steps s in (init_step, init_step + n_steps] with s % every == 0, and init_step
+    // itself when `initial` (GeneralObservableLogger's rule, src/loggers.jl:96-102)
+    static int64_t log_count(int64_t every, int64_t init_step, int64_t n_steps, bool initial) {
+        if (every <= 0) return 0;
+        auto fdiv = [every](int64_t a) { return a >= 0 ? a / every : -((-a + every - 1) / every); };
+        return fdiv(init_step + n_steps) - fdiv(init_step) + ((initial && init_step % every == 0) ? 1 : 0);
+    }
+    static int log_mask_at(const mb_log_t* L, int64_t step) {
+        if (!L) return 0;
+        int m = 0;
+        if (L->energy_every > 0 && step % L->energy_every == 0) m |= LOG_ENERGY;
+        if (L->coords_every > 0 && step % L->coords_every == 0) m |= LOG_COORDS;
+        if (L->vels_every > 0 && step % L->vels_every == 0) m |= LOG_VELS;
+        return m;
+    }
+
+    int simulate_vv(void* coords, void* vels, const mb_vv_params_t* p, mb_log_t* log) override {
         MB_TRY(prepare());
         if (!coords || !vels || !p) return set_error(MB_ERR_INVALID, "null argument");
         if (p->n_steps < 0 || !(p->dt > 0)) return set_error(MB_ERR_INVALID, "n_steps < 0 or dt <= 0");
+        int64_t log_n[3] = {0, 0, 0};  // energy records, coordinate frames, velocity frames this call writes
+        void* log_out[3] = {nullptr, nullptr, nullptr};
+        if (log) {
+            if (decomposed()) return set_error(MB_ERR_INVALID, "mb_simulate_vv_log: logging is not available in decomposed (multi-GPU) runs");
+            const int64_t every[3] = {log->energy_every, log->coords_every, log->vels_every};
+            const int64_t cap[3] = {log->energy_capacity, log->coords_capacity, log->vels_capacity};
+            log_out[0] = log->energies; log_out[1] = log->coords; log_out[2] = log->vels;
+            for (int k = 0; k < 3; k++) {
+                if (every[k] < 0 || cap[k] < 0) return set_error(MB_ERR_INVALID, "mb_simulate_vv_log: negative interval or capacity");
+                if (every[k] > 0 && !log_out[k]) return set_error(MB_ERR_INVALID, "mb_simulate_vv_log: null output for a non-zero interval");
+                log_n[k] = log_count(every[k], p->init_step, p->n_steps, log->log_initial != 0);
+                if (log_n[k] > cap[k])
+                    return set_error(MB_ERR_INVALID, "mb_simulate_vv_log: capacity too small: this call writes " + std::to_string(log_n[k]) +
+                                                         (k == 0 ? " energy records" : k == 1 ? " coordinate frames" : " velocity frames"));
+            }
+            log->n_energies = log->n_coords = log->n_vels = 0;
+        }
         const bool c_dev = is_device_ptr(coords), v_dev = is_device_ptr(vels);
         const T* xc = nullptr;
         const T* vc = nullptr;
@@ -1899,6 +1975,52 @@ class Engine : public EngineBase {
             c.skin_half2 = g_.skin_half2;  // geometry is chosen by the first build
             c.flag_ptr = (rebuild_every_ == 0 && !decomposed()) ? &ctl->rebuild : &ctl->disp;
         }
+        // logger destinations: device outputs are written in place; host outputs go through device staging (all energy
+        // records, copied at the end; a bounded ring of frames, copied out whenever it is full)
+        const size_t frame_bytes = 3 * (size_t)n_ * sizeof(T);
+        bool log_dev[3] = {false, false, false};
+        int64_t ring[2] = {0, 0}, framed[2] = {0, 0};
+        if (log) {
+            LogDesc<T> desc;
+            memset(&desc, 0, sizeof(desc));
+            for (int k = 0; k < 3; k++) log_dev[k] = log_n[k] > 0 && is_device_ptr(log_out[k]);
+            if (log_n[0] > 0) {
+                if (!log_dev[0]) MB_CUDA(d_log_rec_.ensure((size_t)log_n[0] * 3 * sizeof(double)));
+                desc.rec = log_dev[0] ? reinterpret_cast<double*>(log_out[0]) : d_log_rec_.as<double>();
+                MB_CUDA(d_f4_log_.ensure(((size_t)n_ + 16) * sizeof(T4)));
+                MB_CUDA(d_sp_energy_.ensure(sizeof(double)));
+                if (disp_rc_ > 0) {
+                    MB_TRY(dispersion_prepare());
+                    desc.pe_const = (disp_f6_ + disp_f12_) / (box_[0] * box_[1] * box_[2]);
+                }
+            }
+            for (int k = 0; k < 2; k++) {
+                if (log_n[k + 1] == 0) continue;
+                if (log_dev[k + 1]) {
+                    ring[k] = log_n[k + 1];
+                    desc.frames[k] = reinterpret_cast<T*>(log_out[k + 1]);
+                } else {
+                    ring[k] = std::min<int64_t>(log_n[k + 1], std::max<int64_t>(1, (int64_t)(64u << 20) / (int64_t)frame_bytes));
+                    MB_CUDA(d_log_frames_[k].ensure((size_t)ring[k] * frame_bytes));
+                    desc.frames[k] = d_log_frames_[k].as<T>();
+                }
+                desc.ring[k] = ring[k];
+            }
+            MB_CUDA(d_log_desc_.ensure(sizeof(desc)));
+            MB_CUDA(d_log_part_.ensure((size_t)((n_ + LOG_THREADS - 1) / LOG_THREADS) * sizeof(double)));
+            MB_CUDA(cudaMemcpyAsync(d_log_desc_.p, &desc, sizeof(desc), cudaMemcpyHostToDevice, stream_));  // (synchronised below)
+        }
+        // a host frame ring is copied out when full
+        auto frames_logged = [&](int mask) -> int {
+            for (int k = 0; k < 2; k++) {
+                if (!(mask & (LOG_COORDS << k))) continue;
+                framed[k]++;
+                if (!log_dev[k + 1] && framed[k] % ring[k] == 0)
+                    MB_CUDA(cudaMemcpyAsync(reinterpret_cast<char*>(log_out[k + 1]) + (size_t)(framed[k] - ring[k]) * frame_bytes,
+                                            d_log_frames_[k].p, (size_t)ring[k] * frame_bytes, cudaMemcpyDeviceToHost, stream_));
+            }
+            return MB_OK;
+        };
         // step bookkeeping lives on the device (tail of Control)
         {
             struct Tail { int rebuild_every; long long step, init_step; unsigned int rng[4]; unsigned int max_disp2_bits, call_max_disp2_bits; } t;
@@ -1943,25 +2065,42 @@ class Engine : public EngineBase {
                 launches_++;
             }
         }
+        if (log && log->log_initial) {  // apply_loggers! at init_step (run_loggers == true), after F0
+            const int m = log_mask_at(log, p->init_step);
+            if (m) {
+                MB_TRY(enqueue_log(c, m));
+                MB_TRY(frames_logged(m));
+            }
+        }
 
         // CUDA-graph path: static per-step sequence (remove_CM_motion in {0,1}, no stage timers requested)
         bool use_graph = graph_enabled_ && !graph_failed_ && !prof_.enabled && c.do_cm >= 0 && p->n_steps >= 4 &&
                          !(cm_pending && c.do_cm == 0) && !dec &&  // the decomposed step issues NCCL calls with per-rebuild sizes
                          !pme_on_;                                  // cuFFT launches stay outside the captured step for now
         if (use_graph) {
-            GraphKey key{path_, c.do_cm, c.thermostat ? 1 : 0, geom_version_, rebuild_every_, p->dt, p->andersen_kT, p->andersen_prob, n_};
-            if (!graph_exec_ || !(key == graph_key_)) {
-                if (build_step_graph(c, key) != MB_OK) {
-                    graph_failed_ = true;  // stay on the stream path for this context
-                    use_graph = false;
+            // one executable per log mask this call uses (the plain step and the log steps)
+            bool need[8] = {false, false, false, false, false, false, false, false};
+            for (int64_t k = 1; k <= p->n_steps; k++) need[log_mask_at(log, p->init_step + k)] = true;
+            for (int m = 0; m < 8 && use_graph; m++) {
+                if (!need[m]) continue;
+                GraphKey key{path_, c.do_cm, c.thermostat ? 1 : 0, geom_version_, rebuild_every_, m, p->dt, p->andersen_kT, p->andersen_prob, n_};
+                if (!graphs_[m].exec || !(key == graphs_[m].key)) {
+                    if (build_step_graph(c, key) != MB_OK) {
+                        graph_failed_ = true;  // stay on the stream path for this context
+                        use_graph = false;
+                    }
                 }
             }
         }
         graph_used_ = use_graph;
         if (use_graph) {
-            for (int64_t k = 1; k <= p->n_steps; k++) MB_CUDA(cudaGraphLaunch(graph_exec_, stream_));
-            launches_ += graph_step_launches_ * p->n_steps;  // rebuild-body kernels are not counted
-            n_force_evals_ += p->n_steps;
+            for (int64_t k = 1; k <= p->n_steps; k++) {
+                const int m = log_mask_at(log, p->init_step + k);
+                MB_CUDA(cudaGraphLaunch(graphs_[m].exec, stream_));
+                launches_ += graphs_[m].launches;  // rebuild-body kernels are not counted
+                n_force_evals_ += (m & LOG_ENERGY) ? 2 : 1;
+                if (m) MB_TRY(frames_logged(m));
+            }
             n_steps_ += p->n_steps;
         } else {
             for (int64_t k = 1; k <= p->n_steps; k++) {
@@ -1977,7 +2116,9 @@ class Engine : public EngineBase {
                 } else {
                     hint = rebuild_every_ > 0 && k > 1 && (step_n - 1) % rebuild_every_ == 0;
                 }
-                MB_TRY(enqueue_step(c, do_cm, clear_after_k1, false, 0, nullptr, nullptr, hint, /*defer_cm=*/k < p->n_steps));
+                const int m = log_mask_at(log, step_n);
+                MB_TRY(enqueue_step(c, do_cm, clear_after_k1, false, 0, nullptr, nullptr, hint, /*defer_cm=*/k < p->n_steps, m));
+                if (m) MB_TRY(frames_logged(m));
                 cm_pending = (do_cm != 0) && !(c.thermostat && dec);  // (the standalone thermostat kernel consumes v_cm)
                 n_steps_++;
             }
@@ -2000,6 +2141,20 @@ class Engine : public EngineBase {
         launches_++;
         if (!c_dev) MB_CUDA(cudaMemcpyAsync(coords, xo, 3 * (size_t)n_ * sizeof(T), cudaMemcpyDeviceToHost, stream_));
         if (!v_dev) MB_CUDA(cudaMemcpyAsync(vels, vo, 3 * (size_t)n_ * sizeof(T), cudaMemcpyDeviceToHost, stream_));
+        if (log) {
+            if (log_n[0] > 0 && !log_dev[0])
+                MB_CUDA(cudaMemcpyAsync(log_out[0], d_log_rec_.p, (size_t)log_n[0] * 3 * sizeof(double), cudaMemcpyDeviceToHost, stream_));
+            for (int k = 0; k < 2; k++) {
+                const int64_t rest = ring[k] > 0 ? framed[k] % ring[k] : 0;
+                if (!log_dev[k + 1] && rest > 0)
+                    MB_CUDA(cudaMemcpyAsync(reinterpret_cast<char*>(log_out[k + 1]) + (size_t)(framed[k] - rest) * frame_bytes,
+                                            d_log_frames_[k].p, (size_t)rest * frame_bytes, cudaMemcpyDeviceToHost, stream_));
+            }
+            // (after MB_ERR_CAPACITY below these records are as invalid as the coordinates)
+            log->n_energies = log_n[0];
+            log->n_coords = framed[0];
+            log->n_vels = framed[1];
+        }
         MB_CUDA(cudaGetLastError());
         if (path_ == 1) MB_TRY(check_overflow_sync());
         else MB_CUDA(cudaStreamSynchronize(stream_));
@@ -2156,11 +2311,9 @@ class Engine : public EngineBase {
     PairParams<T> P_;
     Geom<T> g_, g_ap_;
     Tric<T> tric_ = {};  // TriclinicBoundary (on = 0: cubic / rectangular box)
-    int64_t launches_ = 0, n_force_evals_ = 0, n_steps_ = 0, graph_step_launches_ = 0;
+    int64_t launches_ = 0, n_force_evals_ = 0, n_steps_ = 0;
     Prof prof_;
-    cudaGraph_t graph_ = nullptr;
-    cudaGraphExec_t graph_exec_ = nullptr;
-    GraphKey graph_key_;
+    StepGraph graphs_[8];
     bool graph_enabled_ = true, graph_failed_ = false, graph_used_ = false, own_stream_ = false;
     int geom_version_ = 0;
     // spatial decomposition (z-slabs of cell layers; one rank per GPU)
@@ -2207,6 +2360,9 @@ class Engine : public EngineBase {
     DevBuf d_task_tab_, d_sched_;  // per-brick task tables; brick ticket + finished-CTA counter of the force kernel
     int force_grid_ = 0;           // CTAs of the last force launch (= number of energy partials)
     DevBuf d_partial_, d_pe_partial_;
+    // device-side loggers: descriptor, KE partials, scratch forces of the energy evaluation, energy records and frame rings
+    // staged for host outputs
+    DevBuf d_log_desc_, d_log_part_, d_f4_log_, d_log_rec_, d_log_frames_[2];
 };
 
 }  // namespace mb
@@ -2316,7 +2472,11 @@ int mb_random_velocities(mb_ctx* ctx, void* vels, double kT, uint64_t rng_ctr1, 
     return ctx->e->random_velocities(vels, kT, rng_ctr1, rng_key);
 }
 int mb_kinetic_energy_tensor(mb_ctx* ctx, const void* vels, double* ke_tensor9_host) { MB_CTX_GUARD(ctx); return ctx->e->kinetic_tensor(vels, ke_tensor9_host); }
-int mb_simulate_vv(mb_ctx* ctx, void* coords, void* vels, const mb_vv_params_t* p) { MB_CTX_GUARD(ctx); return ctx->e->simulate_vv(coords, vels, p); }
+int mb_simulate_vv(mb_ctx* ctx, void* coords, void* vels, const mb_vv_params_t* p) { MB_CTX_GUARD(ctx); return ctx->e->simulate_vv(coords, vels, p, nullptr); }
+int mb_simulate_vv_log(mb_ctx* ctx, void* coords, void* vels, const mb_vv_params_t* p, mb_log_t* log) {
+    MB_CTX_GUARD(ctx);
+    return ctx->e->simulate_vv(coords, vels, p, log);
+}
 int mb_remove_cm_motion(mb_ctx* ctx, void* vels) { MB_CTX_GUARD(ctx); return ctx->e->remove_cm(vels); }
 int mb_kinetic_energy(mb_ctx* ctx, const void* vels, double* ke_host) { MB_CTX_GUARD(ctx); return ctx->e->kinetic_energy(vels, ke_host); }
 int mb_rebuild_neighbors(mb_ctx* ctx, const void* coords) { MB_CTX_GUARD(ctx); return ctx->e->rebuild(coords); }

@@ -70,6 +70,24 @@ __global__ void ingest_kernel(int n, Geom<T> g, const T* __restrict__ coords, co
 }
 
 // ---- export: slot order -> original order, wrapped coordinates, pending CM velocity applied ----
+// position p wrapped into the box as export_kernel does it, stored at dst[0..2] (the logger's coordinate frames; export_kernel
+// keeps its own copy of these lines: calling this helper changes its SASS)
+template <typename T>
+__device__ __forceinline__ void store_wrapped(const Geom<T>& g, typename VT<T>::T4 p, T* dst) {
+    T x[3] = {p.x, p.y, p.z};
+    if (g.tric.on) {
+        tric_wrap<T>(g.tric, x[0], x[1], x[2]);
+        for (int d = 0; d < 3; d++) dst[d] = x[d];
+    } else {
+#pragma unroll
+        for (int d = 0; d < 3; d++) {
+            T v = x[d] - ffloor(x[d] * g.invL[d]) * g.L[d];
+            if (v >= g.L[d]) v -= g.L[d];
+            if (v < (T)0) v = (T)0;
+            dst[d] = v;
+        }
+    }
+}
 template <typename T>
 __global__ void export_kernel(int n, Geom<T> g, const typename VT<T>::T4* __restrict__ pos4,
                               const typename VT<T>::T4* __restrict__ vel4, const int* __restrict__ orig,
@@ -456,6 +474,89 @@ __global__ void andersen_kernel(int s0, int n_own, int n, T kT, double prob, con
     }
     __syncthreads();
     if (s_last && threadIdx.x == 0) cm->valid = 0;
+}
+
+// ---- device-side loggers (mb_simulate_vv_log) -----------------------------------------------------------------
+// What one logged step records; which of the three a step records is the launch's mask (LOG_*).
+enum { LOG_ENERGY = 1, LOG_COORDS = 2, LOG_VELS = 4 };
+template <typename T>
+struct LogDesc {
+    double* rec;                  // energy records (step, pe, ke), one per logged step
+    T* frames[2];                 // coordinate / velocity frames (n x 3, original order): the output or a staging ring
+    long long ring[2];            // frames the ring holds (the output's capacity when it is the output itself)
+    unsigned long long count[3];  // energy records, coordinate frames, velocity frames written in this call
+    double pe_const;              // energy terms without a kernel (LJDispersionCorrection)
+};
+constexpr int LOG_THREADS = 256;
+// A read-only observer of the state after step ctl->step: applies the pending v_cm and previews the Andersen draw that the
+// next drift kernel (or the standalone thermostat closing the call) will apply, with the same operations, so the logged
+// velocities are those export_kernel would return after this step. KE = 1/2 sum m v.v in double, per-CTA partials added in
+// index order by the last CTA, which also adds the pair-energy partials of the ENERGY force launch in index order and
+// writes the record.
+template <typename T>
+__global__ void __launch_bounds__(LOG_THREADS)
+    log_kernel(int n, int mask, Geom<T> g, const typename VT<T>::T4* __restrict__ pos4, const typename VT<T>::T4* __restrict__ vel4,
+               const int* __restrict__ orig, const T* __restrict__ mass, const CmState<T>* __restrict__ cm, Control* __restrict__ ctl,
+               Thermo<T> th, const double* __restrict__ pe_partial, int n_pe, const double* __restrict__ sp_energy,
+               LogDesc<T>* __restrict__ d, double* __restrict__ ke_partial) {
+    const int s = blockIdx.x * blockDim.x + threadIdx.x;
+    double k = 0;
+    if (s < n) {
+        const int o = orig[s];
+        typename VT<T>::T4 v = vel4[s];
+        if (cm->valid) { v.x -= cm->v[0]; v.y -= cm->v[1]; v.z -= cm->v[2]; }
+        if (th.on && ctl->step > ctl->init_step)
+            andersen_apply<T>(v, o, th.n, mass[s], th.kT, th.prob, (uint32_t)ctl->step, ctl->rng[0], ctl->rng[1], ctl->rng[2], ctl->rng[3]);
+        const double vx = v.x, vy = v.y, vz = v.z;
+        k = 0.5 * (double)mass[s] * (vx * vx + vy * vy + vz * vz);
+        if (mask & LOG_COORDS)
+            store_wrapped<T>(g, pos4[s], d->frames[0] + ((size_t)(d->count[1] % d->ring[0]) * n + o) * 3);
+        if (mask & LOG_VELS) {
+            T* dst = d->frames[1] + ((size_t)(d->count[2] % d->ring[1]) * n + o) * 3;
+            dst[0] = v.x; dst[1] = v.y; dst[2] = v.z;
+        }
+    }
+    __shared__ double s_red[LOG_THREADS / 32][2];
+    __shared__ bool s_last;
+    const int tid = threadIdx.x, lane = tid & 31, wid = tid >> 5;
+    for (int o = 16; o > 0; o >>= 1) k += __shfl_xor_sync(0xffffffffu, k, o);
+    if (lane == 0) s_red[wid][0] = k;
+    __syncthreads();
+    if (tid == 0) {
+        double a = 0;
+        for (int w = 0; w < LOG_THREADS / 32; w++) a += s_red[w][0];
+        ke_partial[blockIdx.x] = a;
+        __threadfence();
+        unsigned int t = atomicInc(&ctl->ticket, gridDim.x - 1);
+        s_last = (t == gridDim.x - 1);
+    }
+    __syncthreads();
+    if (!s_last) return;
+    __threadfence();
+    double ke = 0, pe = 0;
+    for (int i = tid; i < (int)gridDim.x; i += LOG_THREADS) ke += ke_partial[i];
+    if (mask & LOG_ENERGY)
+        for (int i = tid; i < n_pe; i += LOG_THREADS) pe += pe_partial[i];
+    for (int o = 16; o > 0; o >>= 1) {
+        ke += __shfl_xor_sync(0xffffffffu, ke, o);
+        pe += __shfl_xor_sync(0xffffffffu, pe, o);
+    }
+    __syncthreads();
+    if (lane == 0) { s_red[wid][0] = ke; s_red[wid][1] = pe; }
+    __syncthreads();
+    if (tid == 0) {
+        ke = pe = 0;
+        for (int w = 0; w < LOG_THREADS / 32; w++) { ke += s_red[w][0]; pe += s_red[w][1]; }
+        if (mask & LOG_ENERGY) {
+            if (sp_energy) pe += *sp_energy;
+            pe += d->pe_const;
+            double* r = d->rec + 3 * (size_t)d->count[0];
+            r[0] = (double)ctl->step; r[1] = pe; r[2] = ke;
+            d->count[0]++;
+        }
+        if (mask & LOG_COORDS) d->count[1]++;
+        if (mask & LOG_VELS) d->count[2]++;
+    }
 }
 
 // kinetic energy: 1/2 sum m v.v (src/energy.jl:56-70), partials per CTA then host sum
