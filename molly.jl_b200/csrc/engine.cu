@@ -60,6 +60,17 @@ struct DevBuf {
     }
 };
 
+// a caller's array: `dev` is the array itself when it is device memory, or its device staging copy (`staged`)
+struct CallerBuf {
+    void* user;
+    void* dev;
+    bool staged;
+    template <typename U>
+    U* as() const {
+        return reinterpret_cast<U*>(dev);
+    }
+};
+
 static bool is_device_ptr(const void* p) {
     if (!p) return false;
     cudaPointerAttributes a;
@@ -69,6 +80,15 @@ static bool is_device_ptr(const void* p) {
         return false;
     }
     return a.type == cudaMemoryTypeDevice || a.type == cudaMemoryTypeManaged;
+}
+
+// Kernel variant selection: calls f(std::integral_constant<..., C>{}) for the first C of the list that equals the run-time
+// value v, or for the last one when none does. f is instantiated for exactly the listed constants, so a launch site writes
+// its launch once and names the variants that exist, e.g. with_const<true, false>(energy, [&](auto EN) { k<T, EN><<<...>>>(...); }).
+template <auto C0, auto... Cs, typename V, typename F>
+static auto with_const(V v, F&& f) {
+    if constexpr (sizeof...(Cs) == 0) return f(std::integral_constant<decltype(C0), C0>{});
+    else return v == C0 ? f(std::integral_constant<decltype(C0), C0>{}) : with_const<Cs...>(v, f);
 }
 
 // Optional per-category device timing with CUDA events on the engine's stream (mb_set_profiling).
@@ -647,6 +667,7 @@ class Engine : public EngineBase {
         MB_CUDA(d_stage_a_.ensure(3 * np * sizeof(T)));
         MB_CUDA(d_stage_b_.ensure(3 * np * sizeof(T)));
         MB_CUDA(d_stage_c_.ensure(3 * np * sizeof(T)));
+        MB_CUDA(d_scalars_.ensure(10 * sizeof(T)));  // [pe, vir(9)] of forces_energy
         // exclusion CSR
         auto up = [&](DevBuf& b, const std::vector<int>& v) -> cudaError_t {
             if (v.empty()) return cudaSuccess;
@@ -660,6 +681,11 @@ class Engine : public EngineBase {
         for (size_t i = 0; i + 1 < sp_ptr_.size(); i++) max_special_host_ = std::max(max_special_host_, sp_ptr_[i + 1] - sp_ptr_[i]);
         const int vvb = (int)((n_ + VV_THREADS - 1) / VV_THREADS);
         MB_CUDA(d_partial_.ensure((size_t)std::max(vvb, 2048) * 8 * sizeof(double)));
+        // geometry of the all-pairs path: the box only (no cells, no skin)
+        memset(&g_ap_, 0, sizeof(g_ap_));
+        for (int d = 0; d < 3; d++) { g_ap_.L[d] = (T)box_[d]; g_ap_.invL[d] = (T)(1.0 / box_[d]); }
+        g_ap_.skin_half2 = std::numeric_limits<T>::infinity();
+        g_ap_.tric = tric_;
         floor_ = CapFloor();
         have_list_ = false;
         dirty_ = false;
@@ -747,6 +773,9 @@ class Engine : public EngineBase {
         g.n_irows = g.b[1] * g.b[2];
         return MB_OK;
     }
+
+    // geometry of the current path (wrap, ingest, log and export kernels)
+    const Geom<T>& geom() const { return path_ == 1 ? g_ : g_ap_; }
 
     ExtMap<T> ext_map() const {
         ExtMap<T> m;
@@ -849,13 +878,14 @@ class Engine : public EngineBase {
     }
     bool has_lists() const { return sp_n_[0] + sp_n_[1] + sp_n_[2] > 0; }
     bool has_specific() const { return has_lists() || pme_on_; }  // everything that is added after the pair kernel
+    // the slot of every atom for kernels that index atoms in original order (null: the all-pairs path keeps that order)
+    const int* slot_of() const { return path_ == 1 ? d_inv_orig_.as<int>() : nullptr; }
     // add the bonded forces to f4 (slot order on the brick path, original order on the all-pairs path; default d_f4_);
     // with energy: per-kernel partials are summed into d_sp_energy_ (double, device)
     int launch_bonded(bool energy, T4* f4 = nullptr) {
         if (!f4) f4 = d_f4_.as<T4>();
         if (!has_specific()) return MB_OK;
         MB_CUDA(d_sp_partial_.ensure(64 * sizeof(double)));  // (set_specific sizes it for the lists; PME alone needs it to exist)
-        const int* slot_of = (path_ == 1) ? d_inv_orig_.as<int>() : nullptr;
         BoxT bx;
         for (int d = 0; d < 3; d++) bx.L[d] = box_[d];
         if (energy) {
@@ -873,14 +903,13 @@ class Engine : public EngineBase {
             total_blk += L.nblk[kind];
         }
         if (total_blk > 0) {
-            const T4* pos = d_pos4_.as<T4>();
-            if (tric_.on) {
-                if (energy) bonded_kernel<T, true, Tric<T>><<<total_blk, BONDED_THREADS, 0, stream_>>>(L, slot_of, pos, f4, tric_, part);
-                else bonded_kernel<T, false, Tric<T>><<<total_blk, BONDED_THREADS, 0, stream_>>>(L, slot_of, pos, f4, tric_, part);
-            } else {
-                if (energy) bonded_kernel<T, true, BoxT><<<total_blk, BONDED_THREADS, 0, stream_>>>(L, slot_of, pos, f4, bx, part);
-                else bonded_kernel<T, false, BoxT><<<total_blk, BONDED_THREADS, 0, stream_>>>(L, slot_of, pos, f4, bx, part);
-            }
+            auto go = [&](auto box) {
+                with_const<true, false>(energy, [&](auto EN) {
+                    bonded_kernel<T, EN, decltype(box)><<<total_blk, BONDED_THREADS, 0, stream_>>>(L, slot_of(), d_pos4_.as<T4>(), f4, box, part);
+                });
+            };
+            if (tric_.on) go(tric_);
+            else go(bx);
             launches_++;
             if (energy) {
                 sum_partials_kernel<<<1, 256, 0, stream_>>>(total_blk, part, d_sp_energy_.as<double>());
@@ -1003,15 +1032,18 @@ class Engine : public EngineBase {
             return rc == 0 ? MB_OK : set_error(MB_ERR_CUDA, "cufftExec failed");
         };
         MB_TRY(fft(-1));
-        if (energy) pme_conv_kernel<T, true><<<conv_blk, PME_THREADS, 0, stream_>>>(pme_g_, f_div, factor, boxfactor, d_pme_bsm_[0].as<double>(), d_pme_bsm_[1].as<double>(), d_pme_bsm_[2].as<double>(), grid, part);
-        else pme_conv_kernel<T, false><<<conv_blk, PME_THREADS, 0, stream_>>>(pme_g_, f_div, factor, boxfactor, d_pme_bsm_[0].as<double>(), d_pme_bsm_[1].as<double>(), d_pme_bsm_[2].as<double>(), grid, part);
+        with_const<true, false>(energy, [&](auto EN) {
+            pme_conv_kernel<T, EN><<<conv_blk, PME_THREADS, 0, stream_>>>(pme_g_, f_div, factor, boxfactor, d_pme_bsm_[0].as<double>(),
+                                                                         d_pme_bsm_[1].as<double>(), d_pme_bsm_[2].as<double>(), grid, part);
+        });
         MB_TRY(fft(1));
         pme_interp_kernel<T><<<nb, PME_THREADS, 0, stream_>>>((int)n_, pme_g_, d_pos4_.as<T4>(), grid, f4);
         launches_ += 3;
         if (n_ex > 0) {
-            const int* slot_of = (path_ == 1) ? d_inv_orig_.as<int>() : nullptr;
-            if (energy) ewald_exclusion_kernel<T, true><<<ex_blk, PME_THREADS, 0, stream_>>>(n_ex, d_pme_pairs_.as<int>(), slot_of, d_pos4_.as<T4>(), f4, pme_g_, pme_alpha_, f_div, part + conv_blk);
-            else ewald_exclusion_kernel<T, false><<<ex_blk, PME_THREADS, 0, stream_>>>(n_ex, d_pme_pairs_.as<int>(), slot_of, d_pos4_.as<T4>(), f4, pme_g_, pme_alpha_, f_div, part + conv_blk);
+            with_const<true, false>(energy, [&](auto EN) {
+                ewald_exclusion_kernel<T, EN><<<ex_blk, PME_THREADS, 0, stream_>>>(n_ex, d_pme_pairs_.as<int>(), slot_of(), d_pos4_.as<T4>(), f4,
+                                                                                  pme_g_, pme_alpha_, f_div, part + conv_blk);
+            });
             launches_++;
         }
         if (energy) {
@@ -1259,7 +1291,8 @@ class Engine : public EngineBase {
     int launch_build(bool count_only) {
         const size_t smem = build_smem_bytes();
         const bool has_ex = !ex_ptr_.empty() || !sp_ptr_.empty();
-        auto go = [&](auto kern) -> int {
+        MB_TRY((with_const<true, false>(count_only, [&](auto CO) { return with_const<true, false>(has_ex, [&](auto EX) -> int {
+            auto kern = build_lists_kernel<T, CO, EX>;
             MB_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
             // few bricks (small systems, narrow slabs): several CTAs share a brick's atoms so that the SMs are filled
             const int split = std::max(1, std::min(4, (4 * sm_count_ + own_nbricks() - 1) / std::max(own_nbricks(), 1)));
@@ -1271,9 +1304,7 @@ class Engine : public EngineBase {
                                                      count_only ? nullptr : d_counts_.as<ushort2>(),
                                                      count_only ? nullptr : d_task_tab_.as<int2>(), own_brick0(), split);
             return MB_OK;
-        };
-        if (count_only) { if (has_ex) MB_TRY(go(build_lists_kernel<T, true, true>)); else MB_TRY(go(build_lists_kernel<T, true, false>)); }
-        else { if (has_ex) MB_TRY(go(build_lists_kernel<T, false, true>)); else MB_TRY(go(build_lists_kernel<T, false, false>)); }
+        }); })));
         launches_++;
         MB_CUDA(cudaGetLastError());
         return MB_OK;
@@ -1337,16 +1368,20 @@ class Engine : public EngineBase {
         return MB_OK;
     }
 
+    // slot-order state from coords_dev (n x 3 device array) in original order, with identity slots
+    void init_slots(const T* coords_dev) {
+        init_slots_kernel<T><<<(int)((n_ + 255) / 256), 256, 0, stream_>>>((int)n_, coords_dev, d_charge_in_.as<T>(), d_ljp_in_.as<T2>(),
+                                                                           d_mass_in_.as<T>(), d_pos4_.as<T4>(), d_vel4_.as<T4>(),
+                                                                           d_lj2_.as<T2>(), d_orig_.as<int>(), d_inv_orig_.as<int>(),
+                                                                           d_mass_.as<T>(), d_xref4_.as<T4>());
+        launches_++;
+    }
     // Synchronous first build: derives halo capacity and list stride from the actual configuration.
     // coords_dev: n x 3 device array in original order.
     int first_build(const T* coords_dev) {
-        const int nb = (int)((n_ + 255) / 256);
         build_nb_ = -1;  // lists for every brick (capacities are global; mb_forces evaluates the whole box)
         own_valid_ = false;
-        init_slots_kernel<T><<<nb, 256, 0, stream_>>>((int)n_, coords_dev, d_charge_in_.as<T>(), d_ljp_in_.as<T2>(),
-                                                      d_mass_in_.as<T>(), d_pos4_.as<T4>(), d_vel4_.as<T4>(), d_lj2_.as<T2>(),
-                                                      d_orig_.as<int>(), d_inv_orig_.as<int>(), d_mass_.as<T>(), d_xref4_.as<T4>());
-        launches_++;
+        init_slots(coords_dev);
         static const int zeros[5] = {0, 0, 0, 0, 0};  // peak_ghost .. peak_neighbors
         MB_CUDA(cudaMemcpyAsync(&d_ctl_.as<Control>()->peak_ghost, zeros, sizeof(zeros), cudaMemcpyHostToDevice, stream_));
         for (;;) {  // ends: every retry makes the brick smaller, and a single cell that does not fit is refused
@@ -1433,91 +1468,83 @@ class Engine : public EngineBase {
     }
 
     // ------------------------------------------------------------------------------------------
-    template <int COUL, bool UNIFORM, int CUTM, bool ENERGY>
-    int launch_force_t(ForceOut<T> out, int brick0, int nbr) {
-        int nbuf, per_sm;
-        force_shape(nbuf, per_sm);
-        const size_t smem = (size_t)nbuf * force_stage();
-        const int grid = std::max(1, std::min(nbr, per_sm * sm_count_));
-        force_grid_ = grid;
-        auto kern = brick_force_kernel<T, COUL, UNIFORM, CUTM, ENERGY>;
-        MB_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-        prof_.begin(Prof::FORCE);
-        kern<<<grid, FORCE_THREADS, smem, stream_>>>(g_, P_, d_hdrs_.as<BrickHdr>(), d_runs_.as<Run>(), d_task_tab_.as<int2>(),
-                                                     d_pos4e_.as<T4>(), d_lj2e_.as<T2>(), d_list_.as<unsigned short>(),
-                                                     d_slist_.as<unsigned short>(), out, brick0, nbr, nbuf, d_sched_.as<unsigned int>());
-        prof_.end(Prof::FORCE);
-        launches_++;
-        n_force_evals_++;
-        MB_CUDA(cudaGetLastError());
-        return MB_OK;
-    }
-    template <int COUL, bool UNIFORM>
-    int launch_force_c(bool energy, ForceOut<T> out, int b0, int nbr) {
-        if (cutm_ == CUTM_TWO_POINT) return energy ? launch_force_t<COUL, UNIFORM, CUTM_TWO_POINT, true>(out, b0, nbr) : launch_force_t<COUL, UNIFORM, CUTM_TWO_POINT, false>(out, b0, nbr);
-        if (cutm_ == CUTM_SHIFTED) return energy ? launch_force_t<COUL, UNIFORM, CUTM_SHIFTED, true>(out, b0, nbr) : launch_force_t<COUL, UNIFORM, CUTM_SHIFTED, false>(out, b0, nbr);
-        return energy ? launch_force_t<COUL, UNIFORM, CUTM_PLAIN, true>(out, b0, nbr) : launch_force_t<COUL, UNIFORM, CUTM_PLAIN, false>(out, b0, nbr);
-    }
-    // owned_only: in a decomposed run the step loop evaluates only this rank's slab of bricks; f4: force target (default d_f4_)
-    int launch_force(bool energy, bool owned_only = false, T4* f4 = nullptr) {
-        const int b0 = owned_only ? own_b0_ : 0;
-        const int nbr = owned_only ? own_nb_ : g_.nbricks;
-        ForceOut<T> out;
-        out.f4 = f4 ? f4 : d_f4_.as<T4>();
+    // energy/virial partials of a pair-force launch: pe[n], vir[6 n] (read by reduce_partials_kernel and log_kernel)
+    struct Partials { const double *pe, *vir; int n; };
+    // Pair forces of the current path (all-pairs or brick kernel) into f4, with energy and virial partials when `energy`
+    // (returned through `parts`). owned_only: in a decomposed run the step loop evaluates only this rank's slab of bricks.
+    int launch_pairs(bool energy, T4* f4, bool owned_only = false, Partials* parts = nullptr) {
+        ForceOut<T> out = {};
+        int grid, vir_at, nbuf = 0, per_sm, nbr = 0, b0 = 0;
+        size_t smem = 0;
+        if (path_ == 0) {
+            grid = vir_at = (int)((n_ + AP_THREADS - 1) / AP_THREADS);
+            MB_CUDA(d_pe_partial_.ensure((size_t)grid * 7 * sizeof(double)));
+        } else {
+            b0 = owned_only ? own_b0_ : 0;
+            nbr = owned_only ? own_nb_ : g_.nbricks;
+            force_shape(nbuf, per_sm);
+            smem = (size_t)nbuf * force_stage();
+            grid = std::max(1, std::min(nbr, per_sm * sm_count_));
+            vir_at = std::max(g_.nbricks, 4 * sm_count_);  // (alloc_brick_tables sizes the partials for any grid)
+            out.f4 = f4;
+            out.gate = gate_;  // one-shot: set by the decomposed step in front of this launch
+            memset(&gate_, 0, sizeof(gate_));
+        }
         out.pe_partial = d_pe_partial_.as<double>();
-        out.vir_partial = d_pe_partial_.as<double>() + std::max(g_.nbricks, 4 * sm_count_);
-        out.gate = gate_;  // one-shot: set by the decomposed step in front of this launch
-        memset(&gate_, 0, sizeof(gate_));
-        switch (P_.coul_kind) {
-            case COUL_NONE:
-                return P_.uniform_lj ? launch_force_c<COUL_NONE, true>(energy, out, b0, nbr) : launch_force_c<COUL_NONE, false>(energy, out, b0, nbr);
-            case COUL_PLAIN: return launch_force_c<COUL_PLAIN, false>(energy, out, b0, nbr);
-            case COUL_CRF: return launch_force_c<COUL_CRF, false>(energy, out, b0, nbr);
-            default: return launch_force_c<COUL_EWALD, false>(energy, out, b0, nbr);
-        }
-    }
-
-    template <int COUL>
-    int launch_allpairs_c(bool energy, const T4* posq, const T2* lj2, T4* f4, int nblk) {
-        double* pe = d_pe_partial_.as<double>();
-        double* vir = pe + nblk;
-        T Lx = (T)box_[0], Ly = (T)box_[1], Lz = (T)box_[2];
-#define MB_AP(SH, EN)                                                                                              \
-    allpairs_force_kernel<T, COUL, SH, EN><<<nblk, AP_THREADS, 0, stream_>>>((int)n_, P_, Lx, Ly, Lz, tric_, posq, lj2, \
-                                                                              ex_ptr_dev(), ex_idx_dev(), sp_ptr_dev(), \
-                                                                              sp_idx_dev(), f4, pe, vir)
-        prof_.begin(Prof::FORCE);
-        if (cutm_ == CUTM_TWO_POINT) { if (energy) MB_AP(CUTM_TWO_POINT, true); else MB_AP(CUTM_TWO_POINT, false); }
-        else if (cutm_ == CUTM_SHIFTED) { if (energy) MB_AP(CUTM_SHIFTED, true); else MB_AP(CUTM_SHIFTED, false); }
-        else { if (energy) MB_AP(CUTM_PLAIN, true); else MB_AP(CUTM_PLAIN, false); }
-        prof_.end(Prof::FORCE);
-#undef MB_AP
+        out.vir_partial = out.pe_partial + vir_at;
+        MB_TRY((with_const<COUL_NONE, COUL_PLAIN, COUL_CRF, COUL_EWALD>(P_.coul_kind, [&](auto COUL) {
+            return with_const<CUTM_TWO_POINT, CUTM_SHIFTED, CUTM_PLAIN>(cutm_, [&](auto CUTM) {
+                return with_const<true, false>(energy, [&](auto EN) -> int {
+                    if (path_ == 0) {
+                        prof_.begin(Prof::FORCE);
+                        allpairs_force_kernel<T, COUL, CUTM, EN><<<grid, AP_THREADS, 0, stream_>>>(
+                            (int)n_, P_, (T)box_[0], (T)box_[1], (T)box_[2], tric_, d_pos4_.as<T4>(), d_lj2_.as<T2>(), ex_ptr_dev(),
+                            ex_idx_dev(), sp_ptr_dev(), sp_idx_dev(), f4, out.pe_partial, out.vir_partial);
+                        prof_.end(Prof::FORCE);
+                        return MB_OK;
+                    }
+                    // the uniform-LJ variants exist only without Coulomb (prepare sets uniform_lj only then)
+                    return with_const<COUL == COUL_NONE, false>(P_.uniform_lj != 0, [&](auto UNI) -> int {
+                        auto kern = brick_force_kernel<T, COUL, UNI, CUTM, EN>;
+                        MB_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+                        prof_.begin(Prof::FORCE);
+                        kern<<<grid, FORCE_THREADS, smem, stream_>>>(g_, P_, d_hdrs_.as<BrickHdr>(), d_runs_.as<Run>(), d_task_tab_.as<int2>(),
+                                                                     d_pos4e_.as<T4>(), d_lj2e_.as<T2>(), d_list_.as<unsigned short>(),
+                                                                     d_slist_.as<unsigned short>(), out, b0, nbr, nbuf,
+                                                                     d_sched_.as<unsigned int>());
+                        prof_.end(Prof::FORCE);
+                        return MB_OK;
+                    });
+                });
+            });
+        })));
         launches_++;
         n_force_evals_++;
         MB_CUDA(cudaGetLastError());
+        if (parts) *parts = Partials{out.pe_partial, out.vir_partial, grid};
         return MB_OK;
-    }
-    int launch_allpairs(bool energy, const T4* posq, const T2* lj2, T4* f4) {
-        const int nblk = (int)((n_ + AP_THREADS - 1) / AP_THREADS);
-        MB_CUDA(d_pe_partial_.ensure((size_t)nblk * 7 * sizeof(double)));
-        switch (P_.coul_kind) {
-            case COUL_NONE: return launch_allpairs_c<COUL_NONE>(energy, posq, lj2, f4, nblk);
-            case COUL_PLAIN: return launch_allpairs_c<COUL_PLAIN>(energy, posq, lj2, f4, nblk);
-            case COUL_CRF: return launch_allpairs_c<COUL_CRF>(energy, posq, lj2, f4, nblk);
-            default: return launch_allpairs_c<COUL_EWALD>(energy, posq, lj2, f4, nblk);
-        }
     }
 
-    // host/device argument views ----------------------------------------------------------------
-    // returns a device pointer holding `count` T values of `user` (copying if user is a host pointer)
-    int view_in(const void* user, size_t count, DevBuf& stage, const T** out) {
-        if (!user) { *out = nullptr; return MB_OK; }
-        if (is_device_ptr(user)) { *out = reinterpret_cast<const T*>(user); return MB_OK; }
-        MB_CUDA(stage.ensure(count * sizeof(T)));
-        MB_CUDA(cudaMemcpyAsync(stage.p, user, count * sizeof(T), cudaMemcpyHostToDevice, stream_));
-        *out = stage.as<T>();
+    // A caller's array in host or device memory, as the kernels see it (CallerBuf): for a host array the staging buffer
+    // `stage` (from byte `stage_off`), filled from the array when `upload` (inputs, and outputs with ADD semantics).
+    // copy_back hands a host array its result.
+    int caller_buf(const void* user, size_t bytes, DevBuf& stage, bool upload, CallerBuf& b, size_t stage_off = 0) {
+        b.user = b.dev = const_cast<void*>(user);
+        b.staged = user && !is_device_ptr(user);
+        if (!b.staged) return MB_OK;
+        MB_CUDA(stage.ensure(stage_off + bytes));
+        b.dev = reinterpret_cast<char*>(stage.p) + stage_off;
+        if (upload) MB_CUDA(cudaMemcpyAsync(b.dev, user, bytes, cudaMemcpyHostToDevice, stream_));
         return MB_OK;
     }
+    // `bytes` of the staged result into a host array at byte `user_off` (stream-ordered: the caller synchronises)
+    int copy_back(const CallerBuf& b, size_t bytes, size_t user_off = 0) {
+        if (b.staged) MB_CUDA(cudaMemcpyAsync(reinterpret_cast<char*>(b.user) + user_off, b.dev, bytes, cudaMemcpyDeviceToHost, stream_));
+        return MB_OK;
+    }
+    // a caller's n x 3 array of T
+    int caller_xyz(const void* user, DevBuf& stage, bool upload, CallerBuf& b) { return caller_buf(user, 3 * (size_t)n_ * sizeof(T), stage, upload, b); }
+    int copy_back_xyz(const CallerBuf& b) { return copy_back(b, 3 * (size_t)n_ * sizeof(T)); }
 
     // ------------------------------------------------------------------------------------------
     // make the slot-order state reflect `coords` (and vels), rebuilding the list when required
@@ -1584,78 +1611,55 @@ class Engine : public EngineBase {
         (void)step_n;
         MB_TRY(prepare());
         if (!coords) return set_error(MB_ERR_INVALID, "coords is null");
-        const T* xc = nullptr;
-        MB_TRY(view_in(coords, 3 * (size_t)n_, d_stage_a_, &xc));
+        CallerBuf xb;
+        MB_TRY(caller_xyz(coords, d_stage_a_, true, xb));
         const bool energy = (pe != nullptr) || (vir != nullptr);
-        const int nb = (int)((n_ + 255) / 256);
-        int n_partials = 0;
-        const int* orig = nullptr;
         if (path_ == 0) {
-            // original order; posq packed into pos4
-            init_slots_kernel<T><<<nb, 256, 0, stream_>>>((int)n_, xc, d_charge_in_.as<T>(), d_ljp_in_.as<T2>(), d_mass_in_.as<T>(),
-                                                          d_pos4_.as<T4>(), d_vel4_.as<T4>(), d_lj2_.as<T2>(), d_orig_.as<int>(),
-                                                          d_inv_orig_.as<int>(), d_mass_.as<T>(), d_xref4_.as<T4>());
-            launches_++;
-            MB_TRY(launch_allpairs(energy, d_pos4_.as<T4>(), d_lj2_.as<T2>(), d_f4_.as<T4>()));
-            n_partials = (int)((n_ + AP_THREADS - 1) / AP_THREADS);
+            init_slots(xb.as<T>());  // original order; posq packed into pos4
         } else {
             if (decomposed()) have_list_ = false;  // forces()/potential_energy() evaluate the whole box on every rank
-            MB_TRY(sync_state_from(xc, nullptr));
-            MB_TRY(launch_force(energy));
-            n_partials = force_grid_;
-            orig = d_orig_.as<int>();
+            MB_TRY(sync_state_from(xb.as<T>(), nullptr));
         }
+        Partials parts;
+        MB_TRY(launch_pairs(energy, d_f4_.as<T4>(), false, &parts));
         if (with_specific) MB_TRY(launch_bonded(pe != nullptr));
         // outputs (ADD semantics)
         if (fs) {
-            if (is_device_ptr(fs)) {
-                scatter_forces_kernel<T><<<nb, 256, 0, stream_>>>((int)n_, d_f4_.as<T4>(), orig, reinterpret_cast<T*>(fs));
-                launches_++;
-            } else {
-                MB_CUDA(d_stage_b_.ensure(3 * (size_t)n_ * sizeof(T)));
-                MB_CUDA(cudaMemcpyAsync(d_stage_b_.p, fs, 3 * (size_t)n_ * sizeof(T), cudaMemcpyHostToDevice, stream_));
-                scatter_forces_kernel<T><<<nb, 256, 0, stream_>>>((int)n_, d_f4_.as<T4>(), orig, d_stage_b_.as<T>());
-                launches_++;
-                MB_CUDA(cudaMemcpyAsync(fs, d_stage_b_.p, 3 * (size_t)n_ * sizeof(T), cudaMemcpyDeviceToHost, stream_));
-            }
+            CallerBuf fb;
+            MB_TRY(caller_xyz(fs, d_stage_b_, true, fb));
+            scatter_forces_kernel<T><<<(int)((n_ + 255) / 256), 256, 0, stream_>>>((int)n_, d_f4_.as<T4>(), path_ == 1 ? d_orig_.as<int>() : nullptr,
+                                                                                 fb.as<T>());
+            launches_++;
+            MB_TRY(copy_back_xyz(fb));
         }
         if (energy) {
-            // stage scalars on device: [pe, vir(9)]
-            MB_CUDA(d_scalars_.ensure(16 * sizeof(T)));
-            T host_sc[16] = {0};
-            bool pe_dev = pe && is_device_ptr(pe), vir_dev = vir && is_device_ptr(vir);
-            T* pe_target = nullptr;
-            T* vir_target = nullptr;
-            if (pe) {
-                if (pe_dev) pe_target = reinterpret_cast<T*>(pe);
-                else { host_sc[0] = *reinterpret_cast<T*>(pe); pe_target = d_scalars_.as<T>(); }
-            }
-            if (vir) {
-                if (vir_dev) vir_target = reinterpret_cast<T*>(vir);
-                else { memcpy(host_sc + 1, vir, 9 * sizeof(T)); vir_target = d_scalars_.as<T>() + 1; }
-            }
-            if ((pe && !pe_dev) || (vir && !vir_dev))
-                MB_CUDA(cudaMemcpyAsync(d_scalars_.p, host_sc, 16 * sizeof(T), cudaMemcpyHostToDevice, stream_));
-            double* pp = d_pe_partial_.as<double>();
-            const double* vp = (path_ == 1) ? pp + std::max(g_.nbricks, 4 * sm_count_) : pp + n_partials;
-            reduce_partials_kernel<T><<<1, 256, 0, stream_>>>(n_partials, pp, vp, pe_target, vir_target, nullptr);
+            // pe and vir of a host caller share one staging block [pe, vir(9)]: one upload, one download
+            T sc[10] = {0};
+            CallerBuf peb, virb;
+            MB_TRY(caller_buf(pe, sizeof(T), d_scalars_, false, peb));
+            MB_TRY(caller_buf(vir, 9 * sizeof(T), d_scalars_, false, virb, sizeof(T)));
+            const bool staged = peb.staged || virb.staged;
+            if (peb.staged) sc[0] = *reinterpret_cast<T*>(pe);
+            if (virb.staged) memcpy(sc + 1, vir, 9 * sizeof(T));
+            if (staged) MB_CUDA(cudaMemcpyAsync(d_scalars_.p, sc, sizeof(sc), cudaMemcpyHostToDevice, stream_));
+            reduce_partials_kernel<T><<<1, 256, 0, stream_>>>(parts.n, parts.pe, parts.vir, peb.as<T>(), virb.as<T>(), nullptr);
             launches_++;
-            if (with_specific && has_specific() && pe_target) {
-                add_double_kernel<T><<<1, 1, 0, stream_>>>(d_sp_energy_.as<double>(), pe_target);
+            if (with_specific && has_specific() && pe) {
+                add_double_kernel<T><<<1, 1, 0, stream_>>>(d_sp_energy_.as<double>(), peb.as<T>());
                 launches_++;
             }
             if (with_specific && disp_rc_ > 0) {  // LJDispersionCorrection: E = (f6 + f12) / V; virial 2 U6 + 4 U12 on the diagonal
                 MB_TRY(dispersion_prepare());
                 const double vol = box_[0] * box_[1] * box_[2];
                 const double u6 = disp_f6_ / vol, u12 = disp_f12_ / vol;
-                add_scalars_kernel<T><<<1, 1, 0, stream_>>>(pe_target, (T)(u6 + u12), vir_target, (T)(2.0 * u6 + 4.0 * u12));
+                add_scalars_kernel<T><<<1, 1, 0, stream_>>>(peb.as<T>(), (T)(u6 + u12), virb.as<T>(), (T)(2.0 * u6 + 4.0 * u12));
                 launches_++;
             }
-            if ((pe && !pe_dev) || (vir && !vir_dev)) {
-                MB_CUDA(cudaMemcpyAsync(host_sc, d_scalars_.p, 16 * sizeof(T), cudaMemcpyDeviceToHost, stream_));
+            if (staged) {
+                MB_CUDA(cudaMemcpyAsync(sc, d_scalars_.p, sizeof(sc), cudaMemcpyDeviceToHost, stream_));
                 MB_CUDA(cudaStreamSynchronize(stream_));
-                if (pe && !pe_dev) *reinterpret_cast<T*>(pe) = host_sc[0];
-                if (vir && !vir_dev) memcpy(vir, host_sc + 1, 9 * sizeof(T));
+                if (peb.staged) *reinterpret_cast<T*>(pe) = sc[0];
+                if (virb.staged) memcpy(vir, sc + 1, 9 * sizeof(T));
             }
         }
         MB_CUDA(cudaGetLastError());
@@ -1674,18 +1678,25 @@ class Engine : public EngineBase {
         bool thermostat;
         int* flag_ptr;
     };
-    int enqueue_step(const StepCfg& c, int do_cm_now, bool clear_cm_after_k1, bool capture,
-                     cudaGraphConditionalHandle handle, cudaGraph_t graph, cudaGraph_t* body_out, bool host_rebuild_hint,
-                     bool defer_cm = false, int log_mask = 0) {
+    // what one step does beyond the plain VelocityVerlet step
+    struct StepOpts {
+        int do_cm = 0;                   // remove_CM_motion after this step's kick
+        bool clear_cm_after_k1 = false;  // K1 consumed the pending v_cm and nothing overwrites it this step
+        bool rebuild_hint = false;       // a fixed-interval rebuild is due (stream path)
+        bool defer_cm = false;           // decomposed: the next step's K1 sums the slabs' momenta itself
+        int log_mask = 0;                // LOG_* records after the step
+    };
+    // capture mode: the graph being built, the handle of its conditional rebuild node and where that node's body goes
+    struct Capture { cudaGraphConditionalHandle handle; cudaGraph_t graph; cudaGraph_t* body; };
+    int enqueue_step(const StepCfg& c, const StepOpts& o, const Capture* cap = nullptr) {
         const bool dec = decomposed() && path_ == 1;
         const int s0 = dec ? own_s0_ : 0, n_own = dec ? own_n_ : (int)n_;
         const int nb = std::max(1, (n_own + 255) / 256);
-        const int vvb = std::max(1, std::min((n_own + 2 * VV_THREADS - 1) / (2 * VV_THREADS), 8 * sm_count_));  // two atoms per thread
         Control* ctl = d_ctl_.as<Control>();
         CmState<T>* cm = d_cm_.as<CmState<T>>();
         // decomposed run over peer memory (peer.cuh): K1 mirrors the boundary slots into the neighbours while it drifts
         const unsigned long long epoch = dec ? ++epoch_ : 0ull;
-        const bool p2p_halo = dec && p2p_active() && !host_rebuild_hint;  // rebuild steps all-gather the state instead
+        const bool p2p_halo = dec && p2p_active() && !o.rebuild_hint;  // rebuild steps all-gather the state instead
         PeerPush<T> push;
         memset(&push, 0, sizeof(push));
         if (p2p_halo) push = make_push(epoch, true);
@@ -1698,20 +1709,22 @@ class Engine : public EngineBase {
         }
         prof_.begin(Prof::VV);
         const Thermo<T> th = thermo_in_k1(c);
-        auto k1 = th.on ? vv_kick_drift_kernel<T, true> : vv_kick_drift_kernel<T, false>;
-        k1<<<std::max(1, std::min((nb + 1) / 2, 5 * sm_count_)), 256, 0, stream_>>>(  // two atoms per thread, one wave (48 registers: 5 CTAs per SM)
-            s0, n_own, c.dt, c.dt_half, c.skin_half2, cm, d_f4_.as<T4>(), d_xref4_.as<T4>(), d_pos4_.as<T4>(), d_vel4_.as<T4>(),
-            c.flag_ptr, ctl, handle, capture && path_ == 1 ? 1 : 0, push, ext_map(), th);
+        with_const<true, false>(th.on != 0, [&](auto TH) {
+            // two atoms per thread, one wave (48 registers: 5 CTAs per SM)
+            vv_kick_drift_kernel<T, TH><<<std::max(1, std::min((nb + 1) / 2, 5 * sm_count_)), 256, 0, stream_>>>(
+                s0, n_own, c.dt, c.dt_half, c.skin_half2, cm, d_f4_.as<T4>(), d_xref4_.as<T4>(), d_pos4_.as<T4>(), d_vel4_.as<T4>(),
+                c.flag_ptr, ctl, cap ? cap->handle : 0, cap && path_ == 1 ? 1 : 0, push, ext_map(), th);
+        });
         prof_.end(Prof::VV);
         launches_++;
-        if (clear_cm_after_k1) {
+        if (o.clear_cm_after_k1) {
             clear_cm_kernel<T><<<1, 1, 0, stream_>>>(cm);
             launches_++;
         }
         if (path_ == 0) {
-            wrap_kernel<T><<<nb, 256, 0, stream_>>>((int)n_, g_ap_, d_pos4_.as<T4>());
+            wrap_kernel<T><<<nb, 256, 0, stream_>>>((int)n_, geom(), d_pos4_.as<T4>());
             launches_++;
-        } else if (capture) {
+        } else if (cap) {
             // splice a conditional IF node into the capture; its body is filled in by the caller
             cudaStreamCaptureStatus status;
             const cudaGraphNode_t* deps = nullptr;
@@ -1720,15 +1733,15 @@ class Engine : public EngineBase {
             MB_CUDA(cudaStreamGetCaptureInfo_v2(stream_, &status, nullptr, &gcap, &deps, &ndeps));
             cudaGraphNodeParams cp = {cudaGraphNodeTypeConditional};
             cp.type = cudaGraphNodeTypeConditional;
-            cp.conditional.handle = handle;
+            cp.conditional.handle = cap->handle;
             cp.conditional.type = cudaGraphCondTypeIf;
             cp.conditional.size = 1;
             cudaGraphNode_t cnode;
-            MB_CUDA(cudaGraphAddNode(&cnode, graph, deps, ndeps, &cp));
-            *body_out = cp.conditional.phGraph_out[0];
+            MB_CUDA(cudaGraphAddNode(&cnode, cap->graph, deps, ndeps, &cp));
+            *cap->body = cp.conditional.phGraph_out[0];
             MB_CUDA(cudaStreamUpdateCaptureDependencies(stream_, &cnode, 1, cudaStreamSetCaptureDependencies));
         } else if (dec) {
-            if (host_rebuild_hint) {
+            if (o.rebuild_hint) {
                 // neighbour rebuild on a decomposed box: replicate positions and velocities, rebuild (identical sort on every
                 // rank, lists only for the owned slab), then refresh the slot ranges and halo segments
                 MB_TRY(allgather_state());
@@ -1741,31 +1754,30 @@ class Engine : public EngineBase {
                 MB_TRY(halo_exchange());
             }
         } else {
-            if (rebuild_every_ == 0 || host_rebuild_hint) MB_TRY(enqueue_rebuild(true, false));
+            if (rebuild_every_ == 0 || o.rebuild_hint) MB_TRY(enqueue_rebuild(true, false));
         }
         const int s0b = dec ? own_s0_ : 0, n_ownb = dec ? own_n_ : (int)n_;  // ownership may have changed in the rebuild
         const int nb2 = std::max(1, (n_ownb + 255) / 256);
         const int vvb2 = std::max(1, std::min((n_ownb + 2 * VV_THREADS - 1) / (2 * VV_THREADS), 8 * sm_count_));
-        if (path_ == 0) MB_TRY(launch_allpairs(false, d_pos4_.as<T4>(), d_lj2_.as<T2>(), d_f4_.as<T4>()));
-        else MB_TRY(launch_force(false, dec));
+        MB_TRY(launch_pairs(false, d_f4_.as<T4>(), dec));
         MB_TRY(launch_bonded(false));
         const bool p2p_sig = dec && p2p_active();  // (after a rebuild: the new ownership's peers)
         PeerSignal sig;
         memset(&sig, 0, sizeof(sig));
-        if (p2p_sig) sig = make_signal(epoch, do_cm_now != 0);
+        if (p2p_sig) sig = make_signal(epoch, o.do_cm != 0);
         prof_.begin(Prof::VV);
-        vv_kick2_kernel<T><<<vvb2, VV_THREADS, 0, stream_>>>(s0b, n_ownb, c.dt_half, do_cm_now, c.inv_mass, d_f4_.as<T4>(), d_mass_.as<T>(),
+        vv_kick2_kernel<T><<<vvb2, VV_THREADS, 0, stream_>>>(s0b, n_ownb, c.dt_half, o.do_cm, c.inv_mass, d_f4_.as<T4>(), d_mass_.as<T>(),
                                                              d_vel4_.as<T4>(), d_partial_.as<double>(), ctl, cm, 0,
                                                              dec ? d_mom_.as<double>() : nullptr, sig);
         prof_.end(Prof::VV);
         launches_++;
-        if (p2p_sig && do_cm_now && defer_cm && !c.thermostat) {
+        if (p2p_sig && o.do_cm && o.defer_cm && !c.thermostat) {
             cm_deferred_epoch_ = epoch;  // the next step's K1 adds the slabs' sums itself
-        } else if (p2p_sig && do_cm_now) {
+        } else if (p2p_sig && o.do_cm) {
             // sum(m v) of all slabs arrived by peer stores: add them in rank order
             peer_cm_kernel<T><<<1, 32, 0, stream_>>>(comm_of(rank_), nranks_, epoch, c.inv_mass, cm);
             launches_++;
-        } else if (dec && do_cm_now) {
+        } else if (dec && o.do_cm) {
             // global sum(m v): one 24-byte all-reduce per step, then v_cm for the lazy subtraction
             MB_NCCL(g_nccl.AllReduce(d_mom_.as<double>(), d_mom_.as<double>() + 4, 3, ncclDouble, ncclSum, comm_, stream_));
             cm_from_sum_kernel<T><<<1, 1, 0, stream_>>>(d_mom_.as<double>() + 4, c.inv_mass, cm);
@@ -1775,7 +1787,7 @@ class Engine : public EngineBase {
             andersen_kernel<T><<<nb2, 256, 0, stream_>>>(s0b, n_ownb, (int)n_, c.kT, c.prob, d_orig_.as<int>(), d_mass_.as<T>(), d_vel4_.as<T4>(), cm, ctl);
             launches_++;
         }
-        if (log_mask) MB_TRY(enqueue_log(c, log_mask));
+        if (o.log_mask) MB_TRY(enqueue_log(c, o.log_mask));
         MB_CUDA(cudaGetLastError());
         return MB_OK;
     }
@@ -1783,22 +1795,16 @@ class Engine : public EngineBase {
     // positions by the ENERGY variants into a scratch force buffer: the trajectory keeps the forces of the plain kernels,
     // so logging does not change it.
     int enqueue_log(const StepCfg& c, int mask) {
-        int n_pe = 0;
+        Partials parts = {d_pe_partial_.as<double>(), nullptr, 0};
         if (mask & LOG_ENERGY) {
             T4* scratch = d_f4_log_.as<T4>();
-            if (path_ == 0) {
-                MB_TRY(launch_allpairs(true, d_pos4_.as<T4>(), d_lj2_.as<T2>(), scratch));
-                n_pe = (int)((n_ + AP_THREADS - 1) / AP_THREADS);
-            } else {
-                MB_TRY(launch_force(true, false, scratch));
-                n_pe = force_grid_;
-            }
+            MB_TRY(launch_pairs(true, scratch, false, &parts));
             MB_TRY(launch_bonded(true, scratch));
         }
         const int nb = (int)((n_ + LOG_THREADS - 1) / LOG_THREADS);
-        log_kernel<T><<<nb, LOG_THREADS, 0, stream_>>>((int)n_, mask, path_ == 0 ? g_ap_ : g_, d_pos4_.as<T4>(), d_vel4_.as<T4>(),
+        log_kernel<T><<<nb, LOG_THREADS, 0, stream_>>>((int)n_, mask, geom(), d_pos4_.as<T4>(), d_vel4_.as<T4>(),
                                                        d_orig_.as<int>(), d_mass_.as<T>(), d_cm_.as<CmState<T>>(), d_ctl_.as<Control>(),
-                                                       thermo_in_k1(c), d_pe_partial_.as<double>(), n_pe,
+                                                       thermo_in_k1(c), parts.pe, parts.n,
                                                        has_specific() ? d_sp_energy_.as<double>() : nullptr,
                                                        d_log_desc_.as<LogDesc<T>>(), d_log_part_.as<double>());
         launches_++;
@@ -1877,7 +1883,11 @@ class Engine : public EngineBase {
         if (cudaStreamBeginCaptureToGraph(stream_, gr, nullptr, nullptr, 0, cudaStreamCaptureModeRelaxed) != cudaSuccess)
             return fail(MB_ERR_CUDA);
         cudaGraph_t body = nullptr;
-        if (enqueue_step(c, c.do_cm, false, true, handle, gr, &body, false, false, mask) != MB_OK) return fail(MB_ERR_CUDA);
+        StepOpts o;
+        o.do_cm = c.do_cm;
+        o.log_mask = mask;
+        const Capture cap = {handle, gr, &body};
+        if (enqueue_step(c, o, &cap) != MB_OK) return fail(MB_ERR_CUDA);
         cudaGraph_t out = nullptr;
         if (cudaStreamEndCapture(stream_, &out) != cudaSuccess) return fail(MB_ERR_CUDA);
         const int64_t step_nodes = launches_ - launches_before;
@@ -1912,32 +1922,92 @@ class Engine : public EngineBase {
         return m;
     }
 
+    // The device-side loggers of one simulate_vv call. Device outputs are written in place; host outputs go through device
+    // staging: all energy records, copied at the end, and a bounded ring of frames per kind, copied out whenever it is full.
+    struct LogRun {
+        mb_log_t* log = nullptr;
+        int64_t n[3] = {0, 0, 0};  // energy records, coordinate frames, velocity frames this call writes
+        CallerBuf out[3] = {};
+        int64_t ring[2] = {0, 0}, framed[2] = {0, 0};
+        size_t frame_bytes = 0;
+    };
+    // validate the request, plan the destinations and upload the logging kernel's descriptor (read by log_kernel only)
+    int log_begin(mb_log_t* log, const mb_vv_params_t* p, LogRun& lr) {
+        lr.log = log;
+        if (!log) return MB_OK;
+        if (decomposed()) return set_error(MB_ERR_INVALID, "mb_simulate_vv_log: logging is not available in decomposed (multi-GPU) runs");
+        const int64_t every[3] = {log->energy_every, log->coords_every, log->vels_every};
+        const int64_t cap[3] = {log->energy_capacity, log->coords_capacity, log->vels_capacity};
+        void* const outs[3] = {log->energies, log->coords, log->vels};
+        for (int k = 0; k < 3; k++) {
+            if (every[k] < 0 || cap[k] < 0) return set_error(MB_ERR_INVALID, "mb_simulate_vv_log: negative interval or capacity");
+            if (every[k] > 0 && !outs[k]) return set_error(MB_ERR_INVALID, "mb_simulate_vv_log: null output for a non-zero interval");
+            lr.n[k] = log_count(every[k], p->init_step, p->n_steps, log->log_initial != 0);
+            if (lr.n[k] > cap[k])
+                return set_error(MB_ERR_INVALID, "mb_simulate_vv_log: capacity too small: this call writes " + std::to_string(lr.n[k]) +
+                                                     (k == 0 ? " energy records" : k == 1 ? " coordinate frames" : " velocity frames"));
+        }
+        log->n_energies = log->n_coords = log->n_vels = 0;
+        lr.frame_bytes = 3 * (size_t)n_ * sizeof(T);
+        LogDesc<T> desc;
+        memset(&desc, 0, sizeof(desc));
+        if (lr.n[0] > 0) {
+            MB_TRY(caller_buf(outs[0], (size_t)lr.n[0] * 3 * sizeof(double), d_log_rec_, false, lr.out[0]));
+            desc.rec = static_cast<double*>(lr.out[0].dev);
+            MB_CUDA(d_f4_log_.ensure(((size_t)n_ + 16) * sizeof(T4)));
+            MB_CUDA(d_sp_energy_.ensure(sizeof(double)));
+            if (disp_rc_ > 0) {
+                MB_TRY(dispersion_prepare());
+                desc.pe_const = (disp_f6_ + disp_f12_) / (box_[0] * box_[1] * box_[2]);
+            }
+        }
+        for (int k = 0; k < 2; k++) {
+            if (lr.n[k + 1] == 0) continue;
+            const int64_t ring = std::min<int64_t>(lr.n[k + 1], std::max<int64_t>(1, (int64_t)(64u << 20) / (int64_t)lr.frame_bytes));
+            MB_TRY(caller_buf(outs[k + 1], (size_t)ring * lr.frame_bytes, d_log_frames_[k], false, lr.out[k + 1]));
+            lr.ring[k] = lr.out[k + 1].staged ? ring : lr.n[k + 1];
+            desc.frames[k] = static_cast<T*>(lr.out[k + 1].dev);
+            desc.ring[k] = lr.ring[k];
+        }
+        MB_CUDA(d_log_desc_.ensure(sizeof(desc)));
+        MB_CUDA(d_log_part_.ensure((size_t)((n_ + LOG_THREADS - 1) / LOG_THREADS) * sizeof(double)));
+        MB_CUDA(cudaMemcpyAsync(d_log_desc_.p, &desc, sizeof(desc), cudaMemcpyHostToDevice, stream_));
+        return MB_OK;
+    }
+    // after a step that recorded `mask`: a full host frame ring is copied out
+    int log_step(LogRun& lr, int mask) {
+        for (int k = 0; k < 2; k++) {
+            if (!(mask & (LOG_COORDS << k))) continue;
+            lr.framed[k]++;
+            if (lr.framed[k] % lr.ring[k] == 0)
+                MB_TRY(copy_back(lr.out[k + 1], (size_t)lr.ring[k] * lr.frame_bytes, (size_t)(lr.framed[k] - lr.ring[k]) * lr.frame_bytes));
+        }
+        return MB_OK;
+    }
+    // end of the call: the staged energy records and the rest of the frame rings, and the counts
+    int log_end(LogRun& lr) {
+        if (!lr.log) return MB_OK;
+        if (lr.n[0] > 0) MB_TRY(copy_back(lr.out[0], (size_t)lr.n[0] * 3 * sizeof(double)));
+        for (int k = 0; k < 2; k++) {
+            const int64_t rest = lr.ring[k] > 0 ? lr.framed[k] % lr.ring[k] : 0;
+            if (rest > 0) MB_TRY(copy_back(lr.out[k + 1], (size_t)rest * lr.frame_bytes, (size_t)(lr.framed[k] - rest) * lr.frame_bytes));
+        }
+        // (after MB_ERR_CAPACITY in simulate_vv these records are as invalid as the coordinates)
+        lr.log->n_energies = lr.n[0];
+        lr.log->n_coords = lr.framed[0];
+        lr.log->n_vels = lr.framed[1];
+        return MB_OK;
+    }
+
     int simulate_vv(void* coords, void* vels, const mb_vv_params_t* p, mb_log_t* log) override {
         MB_TRY(prepare());
         if (!coords || !vels || !p) return set_error(MB_ERR_INVALID, "null argument");
         if (p->n_steps < 0 || !(p->dt > 0)) return set_error(MB_ERR_INVALID, "n_steps < 0 or dt <= 0");
-        int64_t log_n[3] = {0, 0, 0};  // energy records, coordinate frames, velocity frames this call writes
-        void* log_out[3] = {nullptr, nullptr, nullptr};
-        if (log) {
-            if (decomposed()) return set_error(MB_ERR_INVALID, "mb_simulate_vv_log: logging is not available in decomposed (multi-GPU) runs");
-            const int64_t every[3] = {log->energy_every, log->coords_every, log->vels_every};
-            const int64_t cap[3] = {log->energy_capacity, log->coords_capacity, log->vels_capacity};
-            log_out[0] = log->energies; log_out[1] = log->coords; log_out[2] = log->vels;
-            for (int k = 0; k < 3; k++) {
-                if (every[k] < 0 || cap[k] < 0) return set_error(MB_ERR_INVALID, "mb_simulate_vv_log: negative interval or capacity");
-                if (every[k] > 0 && !log_out[k]) return set_error(MB_ERR_INVALID, "mb_simulate_vv_log: null output for a non-zero interval");
-                log_n[k] = log_count(every[k], p->init_step, p->n_steps, log->log_initial != 0);
-                if (log_n[k] > cap[k])
-                    return set_error(MB_ERR_INVALID, "mb_simulate_vv_log: capacity too small: this call writes " + std::to_string(log_n[k]) +
-                                                         (k == 0 ? " energy records" : k == 1 ? " coordinate frames" : " velocity frames"));
-            }
-            log->n_energies = log->n_coords = log->n_vels = 0;
-        }
-        const bool c_dev = is_device_ptr(coords), v_dev = is_device_ptr(vels);
-        const T* xc = nullptr;
-        const T* vc = nullptr;
-        MB_TRY(view_in(coords, 3 * (size_t)n_, d_stage_a_, &xc));
-        MB_TRY(view_in(vels, 3 * (size_t)n_, d_stage_c_, &vc));
+        LogRun lr;
+        MB_TRY(log_begin(log, p, lr));
+        CallerBuf xb, vb;
+        MB_TRY(caller_xyz(coords, d_stage_a_, true, xb));
+        MB_TRY(caller_xyz(vels, d_stage_c_, true, vb));
         const int nb = (int)((n_ + 255) / 256);
         const int vvb = std::min((int)((n_ + VV_THREADS - 1) / VV_THREADS), 8 * sm_count_);
         Control* ctl = d_ctl_.as<Control>();
@@ -1953,74 +2023,19 @@ class Engine : public EngineBase {
         c.prob = p->andersen_prob;
         c.do_cm = (p->remove_cm_every == 0) ? 0 : (p->remove_cm_every == 1 ? 1 : -1);
         if (path_ == 0) {
-            init_slots_kernel<T><<<nb, 256, 0, stream_>>>((int)n_, xc, d_charge_in_.as<T>(), d_ljp_in_.as<T2>(), d_mass_in_.as<T>(),
-                                                          d_pos4_.as<T4>(), d_vel4_.as<T4>(), d_lj2_.as<T2>(), d_orig_.as<int>(),
-                                                          d_inv_orig_.as<int>(), d_mass_.as<T>(), d_xref4_.as<T4>());
-            launches_++;
+            init_slots(xb.as<T>());
             // velocities + wrap through ingest with an identity order (geometry only needs L)
-            Geom<T> g0;
-            memset(&g0, 0, sizeof(g0));
-            for (int d = 0; d < 3; d++) { g0.L[d] = (T)box_[d]; g0.invL[d] = (T)(1.0 / box_[d]); }
-            g0.skin_half2 = std::numeric_limits<T>::infinity();
-            g0.tric = tric_;
-            g_ap_ = g0;
-            ingest_kernel<T><<<nb, 256, 0, stream_>>>((int)n_, g0, xc, vc, d_orig_.as<int>(), d_xref4_.as<T4>(), d_pos4_.as<T4>(),
-                                                      d_vel4_.as<T4>(), &ctl->disp);
-            wrap_kernel<T><<<nb, 256, 0, stream_>>>((int)n_, g0, d_pos4_.as<T4>());
+            ingest_kernel<T><<<nb, 256, 0, stream_>>>((int)n_, g_ap_, xb.as<T>(), vb.as<T>(), d_orig_.as<int>(), d_xref4_.as<T4>(),
+                                                      d_pos4_.as<T4>(), d_vel4_.as<T4>(), &ctl->disp);
+            wrap_kernel<T><<<nb, 256, 0, stream_>>>((int)n_, g_ap_, d_pos4_.as<T4>());
             launches_ += 2;
             c.skin_half2 = std::numeric_limits<T>::infinity();
             c.flag_ptr = &ctl->disp;
         } else {
-            MB_TRY(sync_state_from(xc, vc));
+            MB_TRY(sync_state_from(xb.as<T>(), vb.as<T>()));
             c.skin_half2 = g_.skin_half2;  // geometry is chosen by the first build
             c.flag_ptr = (rebuild_every_ == 0 && !decomposed()) ? &ctl->rebuild : &ctl->disp;
         }
-        // logger destinations: device outputs are written in place; host outputs go through device staging (all energy
-        // records, copied at the end; a bounded ring of frames, copied out whenever it is full)
-        const size_t frame_bytes = 3 * (size_t)n_ * sizeof(T);
-        bool log_dev[3] = {false, false, false};
-        int64_t ring[2] = {0, 0}, framed[2] = {0, 0};
-        if (log) {
-            LogDesc<T> desc;
-            memset(&desc, 0, sizeof(desc));
-            for (int k = 0; k < 3; k++) log_dev[k] = log_n[k] > 0 && is_device_ptr(log_out[k]);
-            if (log_n[0] > 0) {
-                if (!log_dev[0]) MB_CUDA(d_log_rec_.ensure((size_t)log_n[0] * 3 * sizeof(double)));
-                desc.rec = log_dev[0] ? reinterpret_cast<double*>(log_out[0]) : d_log_rec_.as<double>();
-                MB_CUDA(d_f4_log_.ensure(((size_t)n_ + 16) * sizeof(T4)));
-                MB_CUDA(d_sp_energy_.ensure(sizeof(double)));
-                if (disp_rc_ > 0) {
-                    MB_TRY(dispersion_prepare());
-                    desc.pe_const = (disp_f6_ + disp_f12_) / (box_[0] * box_[1] * box_[2]);
-                }
-            }
-            for (int k = 0; k < 2; k++) {
-                if (log_n[k + 1] == 0) continue;
-                if (log_dev[k + 1]) {
-                    ring[k] = log_n[k + 1];
-                    desc.frames[k] = reinterpret_cast<T*>(log_out[k + 1]);
-                } else {
-                    ring[k] = std::min<int64_t>(log_n[k + 1], std::max<int64_t>(1, (int64_t)(64u << 20) / (int64_t)frame_bytes));
-                    MB_CUDA(d_log_frames_[k].ensure((size_t)ring[k] * frame_bytes));
-                    desc.frames[k] = d_log_frames_[k].as<T>();
-                }
-                desc.ring[k] = ring[k];
-            }
-            MB_CUDA(d_log_desc_.ensure(sizeof(desc)));
-            MB_CUDA(d_log_part_.ensure((size_t)((n_ + LOG_THREADS - 1) / LOG_THREADS) * sizeof(double)));
-            MB_CUDA(cudaMemcpyAsync(d_log_desc_.p, &desc, sizeof(desc), cudaMemcpyHostToDevice, stream_));  // (synchronised below)
-        }
-        // a host frame ring is copied out when full
-        auto frames_logged = [&](int mask) -> int {
-            for (int k = 0; k < 2; k++) {
-                if (!(mask & (LOG_COORDS << k))) continue;
-                framed[k]++;
-                if (!log_dev[k + 1] && framed[k] % ring[k] == 0)
-                    MB_CUDA(cudaMemcpyAsync(reinterpret_cast<char*>(log_out[k + 1]) + (size_t)(framed[k] - ring[k]) * frame_bytes,
-                                            d_log_frames_[k].p, (size_t)ring[k] * frame_bytes, cudaMemcpyDeviceToHost, stream_));
-            }
-            return MB_OK;
-        };
         // step bookkeeping lives on the device (tail of Control)
         {
             struct Tail { int rebuild_every; long long step, init_step; unsigned int rng[4]; unsigned int max_disp2_bits, call_max_disp2_bits; } t;
@@ -2055,8 +2070,7 @@ class Engine : public EngineBase {
             build_nb_ = own_nb_;
             MB_TRY(p2p_setup());  // collective; falls back to the NCCL transport on every rank if any mapping fails
         }
-        if (path_ == 0) MB_TRY(launch_allpairs(false, d_pos4_.as<T4>(), d_lj2_.as<T2>(), d_f4_.as<T4>()));
-        else MB_TRY(launch_force(false, dec));
+        MB_TRY(launch_pairs(false, d_f4_.as<T4>(), dec));
         MB_TRY(launch_bonded(false));
         if (dec) {
             const unsigned long long e0 = ++epoch_;  // this force evaluation read the replicated state: tell the pushers
@@ -2069,7 +2083,7 @@ class Engine : public EngineBase {
             const int m = log_mask_at(log, p->init_step);
             if (m) {
                 MB_TRY(enqueue_log(c, m));
-                MB_TRY(frames_logged(m));
+                MB_TRY(log_step(lr, m));
             }
         }
 
@@ -2099,7 +2113,7 @@ class Engine : public EngineBase {
                 MB_CUDA(cudaGraphLaunch(graphs_[m].exec, stream_));
                 launches_ += graphs_[m].launches;  // rebuild-body kernels are not counted
                 n_force_evals_ += (m & LOG_ENERGY) ? 2 : 1;
-                if (m) MB_TRY(frames_logged(m));
+                MB_TRY(log_step(lr, m));
             }
             n_steps_ += p->n_steps;
         } else {
@@ -2116,9 +2130,14 @@ class Engine : public EngineBase {
                 } else {
                     hint = rebuild_every_ > 0 && k > 1 && (step_n - 1) % rebuild_every_ == 0;
                 }
-                const int m = log_mask_at(log, step_n);
-                MB_TRY(enqueue_step(c, do_cm, clear_after_k1, false, 0, nullptr, nullptr, hint, /*defer_cm=*/k < p->n_steps, m));
-                if (m) MB_TRY(frames_logged(m));
+                StepOpts o;
+                o.do_cm = do_cm;
+                o.clear_cm_after_k1 = clear_after_k1;
+                o.rebuild_hint = hint;
+                o.defer_cm = k < p->n_steps;
+                o.log_mask = log_mask_at(log, step_n);
+                MB_TRY(enqueue_step(c, o));
+                MB_TRY(log_step(lr, o.log_mask));
                 cm_pending = (do_cm != 0) && !(c.thermostat && dec);  // (the standalone thermostat kernel consumes v_cm)
                 n_steps_++;
             }
@@ -2134,27 +2153,12 @@ class Engine : public EngineBase {
             if (rebuild_every_ == 0) MB_TRY(adapt_interval());
         }
         // export
-        T* xo = c_dev ? reinterpret_cast<T*>(coords) : d_stage_a_.as<T>();
-        T* vo = v_dev ? reinterpret_cast<T*>(vels) : d_stage_c_.as<T>();
-        export_kernel<T><<<nb, 256, 0, stream_>>>((int)n_, path_ == 0 ? g_ap_ : g_, d_pos4_.as<T4>(), d_vel4_.as<T4>(), d_orig_.as<int>(), cm,
-                                                  xo, vo);
+        export_kernel<T><<<nb, 256, 0, stream_>>>((int)n_, geom(), d_pos4_.as<T4>(), d_vel4_.as<T4>(), d_orig_.as<int>(), cm, xb.as<T>(),
+                                                  vb.as<T>());
         launches_++;
-        if (!c_dev) MB_CUDA(cudaMemcpyAsync(coords, xo, 3 * (size_t)n_ * sizeof(T), cudaMemcpyDeviceToHost, stream_));
-        if (!v_dev) MB_CUDA(cudaMemcpyAsync(vels, vo, 3 * (size_t)n_ * sizeof(T), cudaMemcpyDeviceToHost, stream_));
-        if (log) {
-            if (log_n[0] > 0 && !log_dev[0])
-                MB_CUDA(cudaMemcpyAsync(log_out[0], d_log_rec_.p, (size_t)log_n[0] * 3 * sizeof(double), cudaMemcpyDeviceToHost, stream_));
-            for (int k = 0; k < 2; k++) {
-                const int64_t rest = ring[k] > 0 ? framed[k] % ring[k] : 0;
-                if (!log_dev[k + 1] && rest > 0)
-                    MB_CUDA(cudaMemcpyAsync(reinterpret_cast<char*>(log_out[k + 1]) + (size_t)(framed[k] - rest) * frame_bytes,
-                                            d_log_frames_[k].p, (size_t)rest * frame_bytes, cudaMemcpyDeviceToHost, stream_));
-            }
-            // (after MB_ERR_CAPACITY below these records are as invalid as the coordinates)
-            log->n_energies = log_n[0];
-            log->n_coords = framed[0];
-            log->n_vels = framed[1];
-        }
+        MB_TRY(copy_back_xyz(xb));
+        MB_TRY(copy_back_xyz(vb));
+        MB_TRY(log_end(lr));
         MB_CUDA(cudaGetLastError());
         if (path_ == 1) MB_TRY(check_overflow_sync());
         else MB_CUDA(cudaStreamSynchronize(stream_));
@@ -2162,61 +2166,58 @@ class Engine : public EngineBase {
     }
 
     // ------------------------------------------------------------------------------------------
+    // Per-CTA partials of `width` doubles each, written by launch(d_partial_) over nblk CTAs, summed on the host in block
+    // order per component into out[width]
+    template <typename Launch>
+    int sum_partials_host(int nblk, int width, Launch launch, double* out) {
+        MB_CUDA(d_partial_.ensure((size_t)nblk * width * sizeof(double)));
+        launch(d_partial_.as<double>());
+        launches_++;
+        std::vector<double> part((size_t)nblk * width);
+        MB_CUDA(cudaMemcpyAsync(part.data(), d_partial_.p, part.size() * sizeof(double), cudaMemcpyDeviceToHost, stream_));
+        MB_CUDA(cudaStreamSynchronize(stream_));
+        for (int d = 0; d < width; d++) out[d] = 0;
+        for (int b = 0; b < nblk; b++) for (int d = 0; d < width; d++) out[d] += part[(size_t)width * b + d];
+        return MB_OK;
+    }
     int remove_cm(void* vels) override {
         MB_TRY(prepare());
         if (!vels) return set_error(MB_ERR_INVALID, "null velocities");
-        const bool dev = is_device_ptr(vels);
-        const T* vc = nullptr;
-        MB_TRY(view_in(vels, 3 * (size_t)n_, d_stage_c_, &vc));
+        CallerBuf vb;
+        MB_TRY(caller_xyz(vels, d_stage_c_, true, vb));
         const int nb = (int)((n_ + 255) / 256);
-        MB_CUDA(d_partial_.ensure((size_t)nb * 3 * sizeof(double)));
-        momentum_kernel<T><<<nb, 256, 0, stream_>>>((int)n_, vc, d_mass_in_.as<T>(), d_partial_.as<double>());
-        launches_++;
-        std::vector<double> part((size_t)nb * 3);
-        MB_CUDA(cudaMemcpyAsync(part.data(), d_partial_.p, part.size() * sizeof(double), cudaMemcpyDeviceToHost, stream_));
-        MB_CUDA(cudaStreamSynchronize(stream_));
-        double s[3] = {0, 0, 0};
-        for (int b = 0; b < nb; b++) for (int d = 0; d < 3; d++) s[d] += part[3 * (size_t)b + d];
-        T* vw = const_cast<T*>(vc);
+        double s[3];
+        MB_TRY(sum_partials_host(nb, 3, [&](double* part) {
+            momentum_kernel<T><<<nb, 256, 0, stream_>>>((int)n_, vb.as<T>(), d_mass_in_.as<T>(), part);
+        }, s));
         subtract_velocity_kernel<T><<<nb, 256, 0, stream_>>>((int)n_, (T)(s[0] / total_mass_), (T)(s[1] / total_mass_),
-                                                             (T)(s[2] / total_mass_), vw);
+                                                             (T)(s[2] / total_mass_), vb.as<T>());
         launches_++;
-        if (!dev) MB_CUDA(cudaMemcpyAsync(vels, vw, 3 * (size_t)n_ * sizeof(T), cudaMemcpyDeviceToHost, stream_));
+        MB_TRY(copy_back_xyz(vb));
         MB_CUDA(cudaStreamSynchronize(stream_));
         return MB_OK;
     }
     int kinetic_energy(const void* vels, double* out) override {
         MB_TRY(prepare());
         if (!vels || !out) return set_error(MB_ERR_INVALID, "null argument");
-        const T* vc = nullptr;
-        MB_TRY(view_in(vels, 3 * (size_t)n_, d_stage_c_, &vc));
+        CallerBuf vb;
+        MB_TRY(caller_xyz(vels, d_stage_c_, true, vb));
         const int nb = (int)((n_ + 255) / 256);
-        MB_CUDA(d_partial_.ensure((size_t)nb * 3 * sizeof(double)));
-        kinetic_kernel<T><<<nb, 256, 0, stream_>>>((int)n_, vc, d_mass_in_.as<T>(), d_partial_.as<double>());
-        launches_++;
-        std::vector<double> part(nb);
-        MB_CUDA(cudaMemcpyAsync(part.data(), d_partial_.p, part.size() * sizeof(double), cudaMemcpyDeviceToHost, stream_));
-        MB_CUDA(cudaStreamSynchronize(stream_));
-        double s = 0;
-        for (double v : part) s += v;
-        *out = s;
-        return MB_OK;
+        return sum_partials_host(nb, 1, [&](double* part) {
+            kinetic_kernel<T><<<nb, 256, 0, stream_>>>((int)n_, vb.as<T>(), d_mass_in_.as<T>(), part);
+        }, out);
     }
     // kinetic energy tensor 1/2 sum m v (x) v (src/energy.jl:56-70) into out9 (3x3, symmetric, host doubles)
     int kinetic_tensor(const void* vels, double* out9) override {
         MB_TRY(prepare());
         if (!vels || !out9) return set_error(MB_ERR_INVALID, "null argument");
-        const T* vc = nullptr;
-        MB_TRY(view_in(vels, 3 * (size_t)n_, d_stage_c_, &vc));
+        CallerBuf vb;
+        MB_TRY(caller_xyz(vels, d_stage_c_, true, vb));
         const int nb = (int)((n_ + 255) / 256);
-        MB_CUDA(d_partial_.ensure((size_t)nb * 6 * sizeof(double)));
-        kinetic_tensor_kernel<T><<<nb, 256, 0, stream_>>>((int)n_, vc, d_mass_in_.as<T>(), d_partial_.as<double>());
-        launches_++;
-        std::vector<double> part((size_t)nb * 6);
-        MB_CUDA(cudaMemcpyAsync(part.data(), d_partial_.p, part.size() * sizeof(double), cudaMemcpyDeviceToHost, stream_));
-        MB_CUDA(cudaStreamSynchronize(stream_));
-        double k[6] = {0, 0, 0, 0, 0, 0};
-        for (int b = 0; b < nb; b++) for (int d = 0; d < 6; d++) k[d] += part[6 * (size_t)b + d];
+        double k[6];
+        MB_TRY(sum_partials_host(nb, 6, [&](double* part) {
+            kinetic_tensor_kernel<T><<<nb, 256, 0, stream_>>>((int)n_, vb.as<T>(), d_mass_in_.as<T>(), part);
+        }, k));
         out9[0] = k[0]; out9[4] = k[1]; out9[8] = k[2];
         out9[1] = out9[3] = k[3]; out9[2] = out9[6] = k[4]; out9[5] = out9[7] = k[5];
         return MB_OK;
@@ -2225,27 +2226,23 @@ class Engine : public EngineBase {
     int random_velocities(void* vels, double kT, uint64_t ctr1, uint64_t key) override {
         MB_TRY(prepare());
         if (!vels || !(kT >= 0)) return set_error(MB_ERR_INVALID, "mb_random_velocities: null velocities or negative kT");
-        const bool dev = is_device_ptr(vels);
-        T* vo = reinterpret_cast<T*>(vels);
-        if (!dev) {
-            MB_CUDA(d_stage_c_.ensure(3 * (size_t)n_ * sizeof(T)));
-            vo = d_stage_c_.as<T>();
-        }
+        CallerBuf vb;
+        MB_TRY(caller_xyz(vels, d_stage_c_, false, vb));
         const int nb = (int)((n_ + 255) / 256);
         random_velocities_kernel<T><<<nb, 256, 0, stream_>>>((int)n_, (T)kT, d_mass_in_.as<T>(), (uint32_t)ctr1, (uint32_t)(ctr1 >> 32),
-                                                             (uint32_t)key, (uint32_t)(key >> 32), vo);
+                                                             (uint32_t)key, (uint32_t)(key >> 32), vb.as<T>());
         launches_++;
-        if (!dev) MB_CUDA(cudaMemcpyAsync(vels, vo, 3 * (size_t)n_ * sizeof(T), cudaMemcpyDeviceToHost, stream_));
+        MB_TRY(copy_back_xyz(vb));
         MB_CUDA(cudaStreamSynchronize(stream_));
         return MB_OK;
     }
     int rebuild(const void* coords) override {
         MB_TRY(prepare());
         if (path_ == 0) return MB_OK;
-        const T* xc = nullptr;
-        MB_TRY(view_in(coords, 3 * (size_t)n_, d_stage_a_, &xc));
+        CallerBuf xb;
+        MB_TRY(caller_xyz(coords, d_stage_a_, true, xb));
         have_list_ = false;
-        MB_TRY(sync_state_from(xc, nullptr));
+        MB_TRY(sync_state_from(xb.as<T>(), nullptr));
         MB_CUDA(cudaStreamSynchronize(stream_));
         return MB_OK;
     }
@@ -2358,7 +2355,6 @@ class Engine : public EngineBase {
     DevBuf d_erow_total_, d_erow_start_, d_erow_fill_, d_ecell_start_;  // extended (ghost-padded) grid
     DevBuf d_ext_of_, d_gptr_, d_ghosts_, d_pos4e_, d_lj2e_, d_orig_e_;    // slot -> extended map, ghost table, extended arrays
     DevBuf d_task_tab_, d_sched_;  // per-brick task tables; brick ticket + finished-CTA counter of the force kernel
-    int force_grid_ = 0;           // CTAs of the last force launch (= number of energy partials)
     DevBuf d_partial_, d_pe_partial_;
     // device-side loggers: descriptor, KE partials, scratch forces of the energy evaluation, energy records and frame rings
     // staged for host outputs
@@ -2373,7 +2369,6 @@ class Engine : public EngineBase {
 struct mb_ctx {
     std::unique_ptr<mb::EngineBase> e;
     int device;
-    int dtype;
 };
 
 #define MB_CTX_GUARD(ctx)                                                         \
@@ -2407,7 +2402,6 @@ int mb_ctx_create(int device, int dtype, void* cuda_stream, mb_ctx** out) {
         return mb::set_error(MB_ERR_NOGPU, std::string("device ") + prop.name + " is not sm_90 (H100-class); this library is built for sm_90a only");
     mb_ctx* c = new mb_ctx();
     c->device = device;
-    c->dtype = dtype;
     cudaStream_t s = reinterpret_cast<cudaStream_t>(cuda_stream);
     if (dtype == 32) c->e.reset(new mb::Engine<float>(device, s));
     else c->e.reset(new mb::Engine<double>(device, s));
