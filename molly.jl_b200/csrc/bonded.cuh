@@ -74,19 +74,6 @@ __device__ __forceinline__ void add_force(typename VT<T>::T4* f4, int slot, Vec3
 
 constexpr int BONDED_THREADS = 128;
 
-template <typename T>
-__device__ __forceinline__ void block_energy(double e, double* __restrict__ partial) {
-    __shared__ double s_red[BONDED_THREADS / 32];
-    for (int o = 16; o > 0; o >>= 1) e += __shfl_xor_sync(0xffffffffu, e, o);
-    if ((threadIdx.x & 31) == 0) s_red[threadIdx.x >> 5] = e;
-    __syncthreads();
-    if (threadIdx.x == 0) {
-        double s = 0;
-        for (int w = 0; w < BONDED_THREADS / 32; w++) s += s_red[w];
-        partial[blockIdx.x] = s;
-    }
-}
-
 // slot_of: original atom index -> slot (inv_orig), or nullptr when positions are in original order
 template <typename T, bool ENERGY, typename B>
 __device__ __forceinline__ double bond_term(int t, int n, const int* __restrict__ idx, const T* __restrict__ par,
@@ -199,22 +186,18 @@ __global__ void __launch_bounds__(BONDED_THREADS)
         blk -= L.nblk[0] + L.nblk[1];
         e = torsion_term<T, ENERGY, B>(blk * BONDED_THREADS + threadIdx.x, L.n[2], L.idx[2], static_cast<const T*>(L.par[2]), slot_of, pos4, f4, box);
     }
-    if (ENERGY) block_energy<T>(e, partial);
+    if (ENERGY) {
+        e = block_sum<BONDED_THREADS>(e);
+        if (threadIdx.x == 0) partial[blockIdx.x] = e;
+    }
 }
 
-// pe_partial[0..n) summed in index order -> *acc += sum (single thread block)
+// pe_partial[0..n) summed in index order -> *acc += sum (one CTA of SUM_THREADS)
 __global__ void sum_partials_kernel(int n, const double* __restrict__ partial, double* acc) {
-    __shared__ double s_red[8];
     double v = 0;
     for (int i = threadIdx.x; i < n; i += blockDim.x) v += partial[i];
-    for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
-    if ((threadIdx.x & 31) == 0) s_red[threadIdx.x >> 5] = v;
-    __syncthreads();
-    if (threadIdx.x == 0) {
-        double s = 0;
-        for (int w = 0; w < (int)(blockDim.x >> 5); w++) s += s_red[w];
-        *acc += s;
-    }
+    v = block_sum<SUM_THREADS>(v);
+    if (threadIdx.x == 0) *acc += v;
 }
 
 template <typename T>

@@ -164,6 +164,57 @@ __device__ __forceinline__ T shfl_xor(T v, int m) {
 }
 
 // ---------------------------------------------------------------------------------------------
+// Deterministic CTA sums of doubles (energies, virials, momenta, kinetic sums): the same inputs give the same bits on
+// every run, whatever order the warps finish in.
+// ---------------------------------------------------------------------------------------------
+// v[0..W) of every thread summed over the CTA, each component on its own: an xor butterfly within each warp (offsets 16, 8,
+// 4, 2, 1), then the warp sums added to 0 in warp-index order. NT = blockDim.x. The result is valid in thread 0 only. The
+// scratch is NT/32 x W doubles, one array per (NT, W) and kernel; a second call with the same (NT, W) reuses it, so a
+// barrier must lie between thread 0's read of the first result and the second call.
+constexpr int SUM_THREADS = 256;  // block size of the kernels that do nothing but such a sum (velocity sums, single-CTA sums of partials)
+template <int NT, int W>
+__device__ __forceinline__ void block_sum(double (&v)[W]) {
+    static_assert(NT % 32 == 0 && NT <= 1024, "NT: whole warps of one CTA");
+    __shared__ double s_red[NT / 32][W];
+#pragma unroll
+    for (int k = 0; k < W; k++)
+#pragma unroll
+        for (int o = 16; o > 0; o >>= 1) v[k] += __shfl_xor_sync(0xffffffffu, v[k], o);
+    if ((threadIdx.x & 31) == 0)
+#pragma unroll
+        for (int k = 0; k < W; k++) s_red[threadIdx.x >> 5][k] = v[k];
+    __syncthreads();
+    if (threadIdx.x == 0) {
+#pragma unroll
+        for (int k = 0; k < W; k++) {
+            double s = 0;
+            for (int w = 0; w < NT / 32; w++) s += s_red[w][k];
+            v[k] = s;
+        }
+    }
+}
+template <int NT>
+__device__ __forceinline__ double block_sum(double v) {
+    double a[1] = {v};
+    block_sum<NT, 1>(a);
+    return a[0];
+}
+
+// True in every thread of the CTA that takes the last of gridDim.x tickets (atomicInc wraps *ticket back to 0 for the next
+// launch). Thread 0 fences before it takes the ticket: its own global stores, and those that a barrier ordered before it, are
+// visible to the last CTA, which fences again before it reads them.
+__device__ __forceinline__ bool last_cta(unsigned int* ticket) {
+    __shared__ bool s_last;
+    if (threadIdx.x == 0) {
+        __threadfence();
+        const unsigned int t = atomicInc(ticket, gridDim.x - 1);
+        s_last = (t == gridDim.x - 1);
+    }
+    __syncthreads();
+    return s_last;
+}
+
+// ---------------------------------------------------------------------------------------------
 // Philox4x32-10 counter RNG (public algorithm; Salmon et al. 2011) for the Andersen thermostat
 // (reference: src/kernels.jl:688-721 via PhiloxRNG.jl — statistical parity only, SURVEY §8c).
 // ---------------------------------------------------------------------------------------------

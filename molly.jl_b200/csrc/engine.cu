@@ -912,7 +912,7 @@ class Engine : public EngineBase {
             else go(bx);
             launches_++;
             if (energy) {
-                sum_partials_kernel<<<1, 256, 0, stream_>>>(total_blk, part, d_sp_energy_.as<double>());
+                sum_partials_kernel<<<1, SUM_THREADS, 0, stream_>>>(total_blk, part, d_sp_energy_.as<double>());
                 launches_++;
             }
         }
@@ -1047,7 +1047,7 @@ class Engine : public EngineBase {
             launches_++;
         }
         if (energy) {
-            sum_partials_kernel<<<1, 256, 0, stream_>>>(conv_blk + (n_ex > 0 ? ex_blk : 0), part, d_sp_energy_.as<double>());
+            sum_partials_kernel<<<1, SUM_THREADS, 0, stream_>>>(conv_blk + (n_ex > 0 ? ex_blk : 0), part, d_sp_energy_.as<double>());
             add_const_kernel<<<1, 1, 0, stream_>>>(d_sp_energy_.as<double>(), pme_self_e_);
             launches_ += 2;
         }
@@ -1642,7 +1642,7 @@ class Engine : public EngineBase {
             if (peb.staged) sc[0] = *reinterpret_cast<T*>(pe);
             if (virb.staged) memcpy(sc + 1, vir, 9 * sizeof(T));
             if (staged) MB_CUDA(cudaMemcpyAsync(d_scalars_.p, sc, sizeof(sc), cudaMemcpyHostToDevice, stream_));
-            reduce_partials_kernel<T><<<1, 256, 0, stream_>>>(parts.n, parts.pe, parts.vir, peb.as<T>(), virb.as<T>(), nullptr);
+            reduce_partials_kernel<T><<<1, SUM_THREADS, 0, stream_>>>(parts.n, parts.pe, parts.vir, peb.as<T>(), virb.as<T>());
             launches_++;
             if (with_specific && has_specific() && pe) {
                 add_double_kernel<T><<<1, 1, 0, stream_>>>(d_sp_energy_.as<double>(), peb.as<T>());
@@ -2188,7 +2188,7 @@ class Engine : public EngineBase {
         const int nb = (int)((n_ + 255) / 256);
         double s[3];
         MB_TRY(sum_partials_host(nb, 3, [&](double* part) {
-            momentum_kernel<T><<<nb, 256, 0, stream_>>>((int)n_, vb.as<T>(), d_mass_in_.as<T>(), part);
+            momentum_kernel<T><<<nb, SUM_THREADS, 0, stream_>>>((int)n_, vb.as<T>(), d_mass_in_.as<T>(), part);
         }, s));
         subtract_velocity_kernel<T><<<nb, 256, 0, stream_>>>((int)n_, (T)(s[0] / total_mass_), (T)(s[1] / total_mass_),
                                                              (T)(s[2] / total_mass_), vb.as<T>());
@@ -2204,7 +2204,7 @@ class Engine : public EngineBase {
         MB_TRY(caller_xyz(vels, d_stage_c_, true, vb));
         const int nb = (int)((n_ + 255) / 256);
         return sum_partials_host(nb, 1, [&](double* part) {
-            kinetic_kernel<T><<<nb, 256, 0, stream_>>>((int)n_, vb.as<T>(), d_mass_in_.as<T>(), part);
+            kinetic_kernel<T><<<nb, SUM_THREADS, 0, stream_>>>((int)n_, vb.as<T>(), d_mass_in_.as<T>(), part);
         }, out);
     }
     // kinetic energy tensor 1/2 sum m v (x) v (src/energy.jl:56-70) into out9 (3x3, symmetric, host doubles)
@@ -2216,7 +2216,7 @@ class Engine : public EngineBase {
         const int nb = (int)((n_ + 255) / 256);
         double k[6];
         MB_TRY(sum_partials_host(nb, 6, [&](double* part) {
-            kinetic_tensor_kernel<T><<<nb, 256, 0, stream_>>>((int)n_, vb.as<T>(), d_mass_in_.as<T>(), part);
+            kinetic_tensor_kernel<T><<<nb, SUM_THREADS, 0, stream_>>>((int)n_, vb.as<T>(), d_mass_in_.as<T>(), part);
         }, k));
         out9[0] = k[0]; out9[4] = k[1]; out9[8] = k[2];
         out9[1] = out9[3] = k[3]; out9[2] = out9[6] = k[4]; out9[5] = out9[7] = k[5];

@@ -389,7 +389,8 @@ __global__ void __launch_bounds__(FORCE_THREADS, (sizeof(T) == 8) ? 1 : FORCE_CT
     }
 
     if (ENERGY) {
-        // full shell: every pair was visited from both ends -> 1/2
+        // full shell: every pair was visited from both ends -> 1/2. The order is block_sum's (common.cuh), written out here:
+        // calling the helper changes the register assignment of some of the plain (!ENERGY) instantiations.
         __shared__ double s_red[FORCE_THREADS / 32][7];
         double v[7] = {(double)e_acc, (double)vir[0], (double)vir[1], (double)vir[2],
                        (double)vir[3], (double)vir[4], (double)vir[5]};
@@ -420,29 +421,19 @@ __global__ void __launch_bounds__(FORCE_THREADS, (sizeof(T) == 8) ? 1 : FORCE_CT
     }
 }
 
-// deterministic final reduction of per-CTA partials: pe_out[0] += sum, vir_out (3x3, T) += sum
+// deterministic final reduction of per-CTA partials (one CTA of SUM_THREADS): pe_out[0] += sum, vir_out (3x3, T) += sum
 template <typename T>
 __global__ void reduce_partials_kernel(int n, const double* __restrict__ pe_partial, const double* __restrict__ vir_partial,
-                                       T* pe_out, T* vir_out, double* pe_out_d) {
-    __shared__ double s_red[8][7];
-    const int tid = threadIdx.x, lane = tid & 31, wid = tid >> 5;
-    double v[7] = {0, 0, 0, 0, 0, 0, 0};
-    for (int i = tid; i < n; i += blockDim.x) {
-        v[0] += pe_partial[i];
+                                       T* pe_out, T* vir_out) {
+    double s[7] = {0, 0, 0, 0, 0, 0, 0};
+    for (int i = threadIdx.x; i < n; i += blockDim.x) {
+        s[0] += pe_partial[i];
         if (vir_partial)
-            for (int k = 0; k < 6; k++) v[1 + k] += vir_partial[(size_t)i * 6 + k];
+            for (int k = 0; k < 6; k++) s[1 + k] += vir_partial[(size_t)i * 6 + k];
     }
-    for (int k = 0; k < 7; k++)
-        for (int o = 16; o > 0; o >>= 1) v[k] += __shfl_xor_sync(0xffffffffu, v[k], o);
-    if (lane == 0)
-        for (int k = 0; k < 7; k++) s_red[wid][k] = v[k];
-    __syncthreads();
-    if (tid == 0) {
-        double s[7] = {0, 0, 0, 0, 0, 0, 0};
-        for (int w = 0; w < (int)(blockDim.x >> 5); w++)
-            for (int k = 0; k < 7; k++) s[k] += s_red[w][k];
+    block_sum<SUM_THREADS, 7>(s);
+    if (threadIdx.x == 0) {
         if (pe_out) pe_out[0] += (T)s[0];
-        if (pe_out_d) pe_out_d[0] = s[0];
         if (vir_out) {
             // column-major 3x3: W[a,b] += dr[a] f[b]; symmetric here
             vir_out[0] += (T)s[1]; vir_out[4] += (T)s[2]; vir_out[8] += (T)s[3];
@@ -529,22 +520,14 @@ __global__ void __launch_bounds__(AP_THREADS)
     }
     if (active) f4[i] = make4<T>(fx, fy, fz, (T)0);
     if (ENERGY) {
-        __shared__ double s_red[AP_THREADS / 32][7];
+        // full shell -> 1/2
         double v[7] = {(double)e_acc, (double)vir[0], (double)vir[1], (double)vir[2],
                        (double)vir[3], (double)vir[4], (double)vir[5]};
-        for (int k = 0; k < 7; k++)
-            for (int o = 16; o > 0; o >>= 1) v[k] += __shfl_xor_sync(0xffffffffu, v[k], o);
-        const int lane = tid & 31, wid = tid >> 5;
         __syncthreads();
-        if (lane == 0)
-            for (int k = 0; k < 7; k++) s_red[wid][k] = v[k];
-        __syncthreads();
-        if (tid < 7) {
-            double s = 0.0;
-            for (int w = 0; w < AP_THREADS / 32; w++) s += s_red[w][tid];
-            s *= 0.5;
-            if (tid == 0) pe_partial[blockIdx.x] = s;
-            else vir_partial[(size_t)blockIdx.x * 6 + (tid - 1)] = s;
+        block_sum<AP_THREADS, 7>(v);
+        if (tid == 0) {
+            pe_partial[blockIdx.x] = v[0] * 0.5;
+            for (int k = 0; k < 6; k++) vir_partial[(size_t)blockIdx.x * 6 + k] = v[1 + k] * 0.5;
         }
     }
 }

@@ -196,19 +196,6 @@ __global__ void __launch_bounds__(PME_THREADS)
     if (s < n) pme_spread_atom<T>(s, g, pos4, grid);
 }
 
-// per-CTA energy partial: partial[blockIdx.x] = scale * sum over the CTA
-__device__ __forceinline__ void pme_block_energy(double e, double scale, double* __restrict__ partial) {
-    __shared__ double s_red[PME_THREADS / 32];
-    for (int o = 16; o > 0; o >>= 1) e += __shfl_xor_sync(0xffffffffu, e, o);
-    if ((threadIdx.x & 31) == 0) s_red[threadIdx.x >> 5] = e;
-    __syncthreads();
-    if (threadIdx.x == 0) {
-        double s = 0;
-        for (int w = 0; w < PME_THREADS / 32; w++) s += s_red[w];
-        partial[blockIdx.x] = scale * s;
-    }
-}
-
 template <typename T, bool ENERGY>
 __global__ void __launch_bounds__(PME_THREADS)
     pme_conv_kernel(PmeGeom g, double f_div_eps, double factor, double boxfactor, const double* __restrict__ bsm_x,
@@ -218,7 +205,10 @@ __global__ void __launch_bounds__(PME_THREADS)
     const size_t idx = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
     double e = 0.0;
     if (idx < total) e = pme_conv_point<T>(idx, g, f_div_eps, factor, boxfactor, bsm_x, bsm_y, bsm_z, grid);
-    if (ENERGY) pme_block_energy(e, 0.5, partial);  // the mesh holds k and -k: E = 1/2 sum
+    if (ENERGY) {
+        e = block_sum<PME_THREADS>(e);
+        if (threadIdx.x == 0) partial[blockIdx.x] = 0.5 * e;  // the mesh holds k and -k: E = 1/2 sum
+    }
 }
 
 template <typename T>
@@ -237,7 +227,10 @@ __global__ void __launch_bounds__(PME_THREADS)
     const int t = blockIdx.x * blockDim.x + threadIdx.x;
     double e = 0.0;
     if (t < n_pairs) e = ewald_exclusion_pair<T>(t, pairs, slot_of, pos4, f4, g.L, alpha, f_div_eps);
-    if (ENERGY) pme_block_energy(e, 1.0, partial);
+    if (ENERGY) {
+        e = block_sum<PME_THREADS>(e);
+        if (threadIdx.x == 0) partial[blockIdx.x] = e;
+    }
 }
 
 __global__ void add_const_kernel(double* acc, double v) { *acc += v; }

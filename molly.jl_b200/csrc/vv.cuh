@@ -341,47 +341,20 @@ __global__ void __launch_bounds__(VV_THREADS)
         }
     }
     if (!do_cm && sig.n_peer == 0) return;
-    __shared__ double s_red[VV_THREADS / 32][3];
-    __shared__ bool s_last;
-    const int tid = threadIdx.x, lane = tid & 31, wid = tid >> 5;
-#pragma unroll
-    for (int o = 16; o > 0; o >>= 1) {
-        px += __shfl_xor_sync(0xffffffffu, px, o);
-        py += __shfl_xor_sync(0xffffffffu, py, o);
-        pz += __shfl_xor_sync(0xffffffffu, pz, o);
-    }
-    if (lane == 0) { s_red[wid][0] = px; s_red[wid][1] = py; s_red[wid][2] = pz; }
-    __syncthreads();
-    if (tid == 0) {
-        double a = 0, b = 0, c = 0;
-        for (int w = 0; w < VV_THREADS / 32; w++) { a += s_red[w][0]; b += s_red[w][1]; c += s_red[w][2]; }
-        partial[3 * (size_t)blockIdx.x] = a;
-        partial[3 * (size_t)blockIdx.x + 1] = b;
-        partial[3 * (size_t)blockIdx.x + 2] = c;
+    const int tid = threadIdx.x;
+    double p[3] = {px, py, pz};
+    block_sum<VV_THREADS, 3>(p);
+    if (tid == 0)
+        for (int k = 0; k < 3; k++) partial[3 * (size_t)blockIdx.x + k] = p[k];
+    if (last_cta(&ctl->ticket)) {
         __threadfence();
-        unsigned int t = atomicInc(&ctl->ticket, gridDim.x - 1);
-        s_last = (t == gridDim.x - 1);
-    }
-    __syncthreads();
-    if (s_last) {
-        __threadfence();
-        double a = 0, b = 0, c = 0;
-        for (int i = tid; i < (int)gridDim.x; i += VV_THREADS) {
-            a += partial[3 * (size_t)i]; b += partial[3 * (size_t)i + 1]; c += partial[3 * (size_t)i + 2];
-        }
-        // fixed-shape tree -> deterministic
-#pragma unroll
-        for (int o = 16; o > 0; o >>= 1) {
-            a += __shfl_xor_sync(0xffffffffu, a, o);
-            b += __shfl_xor_sync(0xffffffffu, b, o);
-            c += __shfl_xor_sync(0xffffffffu, c, o);
-        }
-        __syncthreads();
-        if (lane == 0) { s_red[wid][0] = a; s_red[wid][1] = b; s_red[wid][2] = c; }
-        __syncthreads();
+        double s[3] = {0, 0, 0};
+        for (int i = tid; i < (int)gridDim.x; i += VV_THREADS)
+            for (int k = 0; k < 3; k++) s[k] += partial[3 * (size_t)i + k];
+        __syncthreads();  // block_sum's scratch is reused
+        block_sum<VV_THREADS, 3>(s);
         if (tid == 0) {
-            a = b = c = 0;
-            for (int w = 0; w < VV_THREADS / 32; w++) { a += s_red[w][0]; b += s_red[w][1]; c += s_red[w][2]; }
+            const double a = s[0], b = s[1], c = s[2];
             // peer-memory transport: the force kernel in front of this one is done with the halo data ...
             for (int q = 0; q < sig.n_peer; q++) st_release_sys(sig.read_flag[q], sig.epoch);
             if (!do_cm) return;
@@ -464,16 +437,9 @@ __global__ void andersen_kernel(int s0, int n_own, int n, T kT, double prob, con
         andersen_apply<T>(v, orig[s], n, mass[s], kT, prob, step_lo, ctr1_lo, ctr1_hi, key_lo, key_hi);
         vel4[s] = v;
     }
-    // last CTA clears the pending CM state
-    __shared__ bool s_last;
+    // last CTA clears the pending CM state (the barrier puts every thread's velocity store before the ticket)
     __syncthreads();
-    if (threadIdx.x == 0) {
-        __threadfence();
-        unsigned int t = atomicInc(&ctl->ticket, gridDim.x - 1);
-        s_last = (t == gridDim.x - 1);
-    }
-    __syncthreads();
-    if (s_last && threadIdx.x == 0) cm->valid = 0;
+    if (last_cta(&ctl->ticket) && threadIdx.x == 0) cm->valid = 0;
 }
 
 // ---- device-side loggers (mb_simulate_vv_log) -----------------------------------------------------------------
@@ -516,37 +482,21 @@ __global__ void __launch_bounds__(LOG_THREADS)
             dst[0] = v.x; dst[1] = v.y; dst[2] = v.z;
         }
     }
-    __shared__ double s_red[LOG_THREADS / 32][2];
-    __shared__ bool s_last;
-    const int tid = threadIdx.x, lane = tid & 31, wid = tid >> 5;
-    for (int o = 16; o > 0; o >>= 1) k += __shfl_xor_sync(0xffffffffu, k, o);
-    if (lane == 0) s_red[wid][0] = k;
-    __syncthreads();
-    if (tid == 0) {
-        double a = 0;
-        for (int w = 0; w < LOG_THREADS / 32; w++) a += s_red[w][0];
-        ke_partial[blockIdx.x] = a;
-        __threadfence();
-        unsigned int t = atomicInc(&ctl->ticket, gridDim.x - 1);
-        s_last = (t == gridDim.x - 1);
-    }
-    __syncthreads();
-    if (!s_last) return;
+    const int tid = threadIdx.x;
+    k = block_sum<LOG_THREADS>(k);
+    if (tid == 0) ke_partial[blockIdx.x] = k;
+    if (!last_cta(&ctl->ticket)) return;
     __threadfence();
     double ke = 0, pe = 0;
     for (int i = tid; i < (int)gridDim.x; i += LOG_THREADS) ke += ke_partial[i];
     if (mask & LOG_ENERGY)
         for (int i = tid; i < n_pe; i += LOG_THREADS) pe += pe_partial[i];
-    for (int o = 16; o > 0; o >>= 1) {
-        ke += __shfl_xor_sync(0xffffffffu, ke, o);
-        pe += __shfl_xor_sync(0xffffffffu, pe, o);
-    }
+    // KE, then PE: one component each, so that both reuse the scratch of the per-CTA sum above
     __syncthreads();
-    if (lane == 0) { s_red[wid][0] = ke; s_red[wid][1] = pe; }
+    ke = block_sum<LOG_THREADS>(ke);
     __syncthreads();
+    pe = block_sum<LOG_THREADS>(pe);
     if (tid == 0) {
-        ke = pe = 0;
-        for (int w = 0; w < LOG_THREADS / 32; w++) { ke += s_red[w][0]; pe += s_red[w][1]; }
         if (mask & LOG_ENERGY) {
             if (sp_energy) pe += *sp_energy;
             pe += d->pe_const;
@@ -568,15 +518,8 @@ __global__ void kinetic_kernel(int n, const T* __restrict__ vels, const T* __res
         double vx = vels[3 * (size_t)i], vy = vels[3 * (size_t)i + 1], vz = vels[3 * (size_t)i + 2];
         k = 0.5 * (double)mass[i] * (vx * vx + vy * vy + vz * vz);
     }
-    __shared__ double s_red[32];
-    for (int o = 16; o > 0; o >>= 1) k += __shfl_xor_sync(0xffffffffu, k, o);
-    if ((threadIdx.x & 31) == 0) s_red[threadIdx.x >> 5] = k;
-    __syncthreads();
-    if (threadIdx.x == 0) {
-        double s = 0;
-        for (int w = 0; w < (int)(blockDim.x >> 5); w++) s += s_red[w];
-        partial[blockIdx.x] = s;
-    }
+    k = block_sum<SUM_THREADS>(k);
+    if (threadIdx.x == 0) partial[blockIdx.x] = k;
 }
 
 // kinetic energy tensor K = 1/2 sum m v (x) v (src/energy.jl:56-70): xx, yy, zz, xy, xz, yz partials per CTA
@@ -589,17 +532,9 @@ __global__ void kinetic_tensor_kernel(int n, const T* __restrict__ vels, const T
         const double vx = vels[3 * (size_t)i], vy = vels[3 * (size_t)i + 1], vz = vels[3 * (size_t)i + 2];
         k[0] = m * vx * vx; k[1] = m * vy * vy; k[2] = m * vz * vz; k[3] = m * vx * vy; k[4] = m * vx * vz; k[5] = m * vy * vz;
     }
-    __shared__ double s_red[32][6];
-    for (int d = 0; d < 6; d++)
-        for (int o = 16; o > 0; o >>= 1) k[d] += __shfl_xor_sync(0xffffffffu, k[d], o);
-    if ((threadIdx.x & 31) == 0)
-        for (int d = 0; d < 6; d++) s_red[threadIdx.x >> 5][d] = k[d];
-    __syncthreads();
-    if (threadIdx.x < 6) {
-        double s = 0;
-        for (int w = 0; w < (int)(blockDim.x >> 5); w++) s += s_red[w][threadIdx.x];
-        partial[6 * (size_t)blockIdx.x + threadIdx.x] = s;
-    }
+    block_sum<SUM_THREADS, 6>(k);
+    if (threadIdx.x == 0)
+        for (int d = 0; d < 6; d++) partial[6 * (size_t)blockIdx.x + d] = k[d];
 }
 
 // random_velocities! (src/spatial.jl:803-831; GPU kernel src/kernels.jl:688-703): every atom gets a Maxwell-Boltzmann
@@ -633,18 +568,9 @@ __global__ void momentum_kernel(int n, const T* __restrict__ vels, const T* __re
         T m = mass[i];
         for (int d = 0; d < 3; d++) p[d] = (double)(vels[3 * (size_t)i + d] * m);
     }
-    __shared__ double s_red[32][3];
-    for (int d = 0; d < 3; d++)
-        for (int o = 16; o > 0; o >>= 1) p[d] += __shfl_xor_sync(0xffffffffu, p[d], o);
-    if ((threadIdx.x & 31) == 0)
-        for (int d = 0; d < 3; d++) s_red[threadIdx.x >> 5][d] = p[d];
-    __syncthreads();
-    if (threadIdx.x == 0) {
-        double s[3] = {0, 0, 0};
-        for (int w = 0; w < (int)(blockDim.x >> 5); w++)
-            for (int d = 0; d < 3; d++) s[d] += s_red[w][d];
-        for (int d = 0; d < 3; d++) partial[3 * (size_t)blockIdx.x + d] = s[d];
-    }
+    block_sum<SUM_THREADS, 3>(p);
+    if (threadIdx.x == 0)
+        for (int d = 0; d < 3; d++) partial[3 * (size_t)blockIdx.x + d] = p[d];
 }
 template <typename T>
 __global__ void subtract_velocity_kernel(int n, T vx, T vy, T vz, T* __restrict__ vels) {
