@@ -219,6 +219,44 @@ typedef struct {
  * in decomposed (multi-GPU) runs, which do not log. After MB_ERR_CAPACITY the records are invalid, like the coordinates. */
 int mb_simulate_vv_log(mb_ctx* ctx, void* coords, void* vels, const mb_vv_params_t* p, mb_log_t* log);
 
+/* simulate!(sys, SteepestDescentMinimizer(step_size, max_steps, tol)) (src/simulators.jl:183-274) on the device: wrap the
+ * coordinates, E = potential energy; then for step n = init_step+1 .. init_step+max_steps: F = forces, m = max |F_i|,
+ * x <- wrap(x + h F / m), E_trial = potential energy; E_trial < E accepts (h <- 6h/5, E <- E_trial), otherwise x is restored
+ * (h <- h/5); the loop stops after the iteration in which m < tol. Energy and forces are those of mb_forces_energy_all
+ * (pairwise + specific + PME + LJDispersionCorrection). coords: n x 3, host or device, updated in place and returned
+ * wrapped, original atom order. Where this differs from the reference:
+ *  - one evaluation per iteration: forces and energy of the trial together. On accept the trial's forces are the next F;
+ *    on reject F is kept (the reference recomputes it at the restored coordinates and gets the same value);
+ *  - E and E_trial are the engine's double sums, compared in double; m = sqrt(max |F_i|^2) in double;
+ *  - f32: the moved coordinate x + h F / m is formed in double and rounded once (the reference's step size is a Float64);
+ *  - neighbours: always the exact displacement trigger (rebuild when an atom is more than skin/2 from its position at the
+ *    last build), whatever mb_set_neighbor_policy's rebuild_every says (the reference's GPU finder is exact at every call);
+ *  - m = 0 or not finite: the positions stay unchanged and the iteration is recorded as rejected with E_trial = NaN
+ *    (the reference's x + h F / m is NaN and is rejected).
+ * One iteration is one CUDA graph body (trial, conditional rebuild, evaluation, decision, accept/restore) inside a
+ * conditional WHILE node: one graph launch per call. PME, profiling and a failed capture take the stream path (one
+ * iteration per host round trip). The context's velocity and force state afterwards is unspecified (mb_simulate_vv starts
+ * from a clean one). MB_ERR_INVALID before any work for max_steps < 0, step_size <= 0, tol < 0, a trace capacity below
+ * max_steps + 1, and decomposed (multi-GPU) contexts; MB_ERR_CAPACITY as in mb_simulate_vv (results invalid, retry from
+ * the starting coordinates). */
+typedef struct {
+    double step_size;         /* h0 in nm (reference default 0.01) */
+    int64_t max_steps;        /* default 1000 */
+    double tol;               /* kJ mol^-1 nm^-1 (default 1000) */
+    int64_t init_step;
+    double* trace;            /* optional (NULL): trace_capacity x 4 doubles (step, E or E_trial, max force, accepted 0/1),
+                               * host or device. Record 0 = (init_step, E0, NaN, 1), then one per iteration */
+    int64_t trace_capacity;   /* records the trace holds: at least max_steps + 1 */
+    /* written back */
+    int64_t n_iterations;     /* iterations taken (records written = n_iterations + 1) */
+    double energy;            /* E of the returned coordinates */
+    double max_force;         /* max |F_i| at the returned coordinates */
+    double final_step_size;   /* h after the last iteration */
+    int32_t converged;        /* the last iteration's max force was below tol */
+    int32_t reserved_;
+} mb_sd_params_t;
+int mb_minimize_sd(mb_ctx* ctx, void* coords, mb_sd_params_t* p);
+
 /* remove_CM_motion! (ext/MollyCUDAExt.jl:2373; src/spatial.jl:901-929) on an n x 3 velocity array. */
 int mb_remove_cm_motion(mb_ctx* ctx, void* vels);
 /* kinetic_energy (src/energy.jl:56-70): writes 1/2 sum m v.v to *ke_host (double, host). */

@@ -8,6 +8,7 @@
 #   Molly.pairwise_forces_loop_gpu!(buffers, sys, pairwise_inters, nbs::Nothing, Val(needs_vir), step_n)   ext:845
 #   Molly.pairwise_pe_loop_gpu!(pe_vec_nounits, buffers, sys, pairwise_inters, nbs::Nothing, step_n)        ext:936
 #   Molly.simulate!(sys, sim::VelocityVerlet, n_steps; ...)                                                 simulators.jl:547
+#   Molly.simulate!(sys, sim::SteepestDescentMinimizer; ...)                                                simulators.jl:183
 # (Molly.remove_CM_motion! for CuArray Systems is NOT redefined: the stock extension owns that exact signature)
 # and falls through to the stock methods (invoke) for anything it does not recognise: non-cubic boundaries,
 # constraints, virtual sites, couplings other than AndersenThermostat, interactions outside
@@ -312,6 +313,51 @@ function Molly.simulate!(sys::System{3, <:CuArray, T}, sim::VelocityVerlet, n_st
                     ctx.handle, pointer(sys.coords), pointer(sys.velocities), Ref(pp)))
         done += m
         Molly.apply_loggers!(sys, nothing, nothing, init_step + done, run_loggers)
+    end
+    return sys
+end
+
+# ---- simulate!(sys, ::SteepestDescentMinimizer) (src/simulators.jl:183-274) ------------------------------------------------
+# Taken over when the System is engine-eligible, has no constraints, no general interactions (the engine would need their
+# energies for the log lines) and run_loggers is false: the whole minimisation is one mb_minimize_sd call, and the
+# reference's log lines are printed from the trace afterwards. Anything else runs the stock method.
+struct MBSDParams
+    step_size::Float64
+    max_steps::Int64
+    tol::Float64
+    init_step::Int64
+    trace::Ptr{Float64}
+    trace_capacity::Int64
+    n_iterations::Int64
+    energy::Float64
+    max_force::Float64
+    final_step_size::Float64
+    converged::Int32
+    reserved_::Int32
+end
+
+function Molly.simulate!(sys::System{3, <:CuArray, T}, sim::SteepestDescentMinimizer; init_step=0, run_loggers=false,
+                         kwargs...) where T
+    descs = engine_eligible(sys, sys.pairwise_inters)
+    if isnothing(descs) || run_loggers != false || !isempty(sys.general_inters) ||
+            !all(!isnothing, map(specific_desc, sys.specific_inter_lists))
+        return invoke(Molly.simulate!, Tuple{Any, SteepestDescentMinimizer}, sys, sim;
+                      init_step=init_step, run_loggers=run_loggers, kwargs...)
+    end
+    ctx = context_for(sys, descs)
+    set_specific!(ctx, sys)
+    trace = zeros(Float64, 4, sim.max_steps + 1)   # (step, E or E_trial, max force, accepted) per column
+    p = Ref(MBSDParams(Float64(ustrip(sim.step_size)), sim.max_steps, Float64(ustrip(sim.tol)), init_step,
+                       pointer(trace), sim.max_steps + 1, 0, 0.0, 0.0, 0.0, Int32(0), Int32(0)))
+    GC.@preserve trace begin
+        check(ccall((:mb_minimize_sd, LIB), Cint, (Ptr{Cvoid}, CuPtr{Cvoid}, Ref{MBSDParams}),
+                    ctx.handle, pointer(sys.coords), p))
+    end
+    eu, fu = sys.energy_units, sys.force_units
+    println(sim.log_stream, "Step ", init_step, " - potential energy ", trace[2, 1] * eu, " - max force N/A - N/A")
+    for k in 2:(p[].n_iterations + 1)
+        println(sim.log_stream, "Step ", Int(trace[1, k]), " - potential energy ", trace[2, k] * eu, " - max force ",
+                trace[3, k] * fu, " - ", trace[4, k] != 0 ? "accepted" : "rejected")
     end
     return sys
 end

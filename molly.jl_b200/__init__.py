@@ -14,4 +14,5 @@ from .api import (Atom, CubicBoundary, TriclinicBoundary, System, NoCutoff, Dist
                   atoms_from_arrays, atoms_to_array, atom_dtype, MollyB200Error, COULOMB_CONST, BOLTZMANN_K,
                   comm_unique_id, comm_init, decomp_plan, InteractionList2Atoms, InteractionList3Atoms,
                   InteractionList4Atoms, PotentialEnergyLogger, KineticEnergyLogger, TotalEnergyLogger, TemperatureLogger,
-                  CoordinatesLogger, VelocitiesLogger, values, record_steps)
+                  CoordinatesLogger, VelocitiesLogger, values, record_steps, SteepestDescentMinimizer, steepest_descent,
+                  sd_log_lines)

@@ -20,7 +20,7 @@ EXPORTED = [
     "mb_stats", "mb_synchronize", "mb_set_capacity_scale", "mb_set_launch_config", "mb_comm_unique_id",
     "mb_comm_init", "mb_decomp_plan", "mb_set_profiling", "mb_set_specific", "mb_forces_energy_all", "mb_set_pme", "mb_pme_plan",
     "mb_set_lj_dispersion_correction", "mb_random_velocities", "mb_kinetic_energy_tensor", "mb_set_box_triclinic",
-    "mb_simulate_vv_log",
+    "mb_simulate_vv_log", "mb_minimize_sd",
 ]
 
 
@@ -62,6 +62,14 @@ class MBLog(C.Structure):
     ]
 
 
+class MBSDParams(C.Structure):
+    _fields_ = [
+        ("step_size", C.c_double), ("max_steps", C.c_int64), ("tol", C.c_double), ("init_step", C.c_int64),
+        ("trace", C.c_void_p), ("trace_capacity", C.c_int64), ("n_iterations", C.c_int64), ("energy", C.c_double),
+        ("max_force", C.c_double), ("final_step_size", C.c_double), ("converged", C.c_int32), ("reserved_", C.c_int32),
+    ]
+
+
 class MollyB200Error(RuntimeError):
     def __init__(self, code, msg):
         super().__init__(f"libmollyb200 error {code}: {msg}")
@@ -98,6 +106,7 @@ def load():
     L.mb_forces_energy.argtypes = [vp, vp, vp, vp, vp, i64]
     L.mb_simulate_vv.argtypes = [vp, vp, vp, C.POINTER(MBVVParams)]
     L.mb_simulate_vv_log.argtypes = [vp, vp, vp, C.POINTER(MBVVParams), C.POINTER(MBLog)]
+    L.mb_minimize_sd.argtypes = [vp, vp, C.POINTER(MBSDParams)]
     L.mb_remove_cm_motion.argtypes = [vp, vp]
     L.mb_kinetic_energy.argtypes = [vp, vp, C.POINTER(dbl)]
     L.mb_rebuild_neighbors.argtypes = [vp, vp]

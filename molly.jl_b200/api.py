@@ -9,6 +9,7 @@ julia/MollyB200Ext.jl, see INTEGRATION.md):
     LennardJones, Coulomb, CoulombReactionField     src/interactions/lennard_jones.jl:28-35, coulomb.jl:32-70, :698-747
     GPUNeighborFinder (+ aliases)                   src/neighbors.jl:104-115
     VelocityVerlet, AndersenThermostat, simulate    src/simulators.jl:287-295, :547-668; src/coupling.jl:184-212
+    SteepestDescentMinimizer                        src/simulators.jl:183-274 (simulate dispatches on the simulator)
     forces, forces_virial, potential_energy         src/force.jl:678-720, src/energy.jl:202-248
     kinetic_energy, temperature, remove_CM_motion   src/energy.jl:44-175, src/spatial.jl:901-929
     *EnergyLogger, TemperatureLogger, Coordinates-  src/loggers.jl:44-102, :134-278 (recorded on the device inside
@@ -342,6 +343,25 @@ class VelocityVerlet:
     remove_CM_motion: int = 1
 
 
+@dataclass
+class SteepestDescentMinimizer:
+    """SteepestDescentMinimizer(step_size, max_steps, tol, log_stream) — src/simulators.jl:183-274, run on the device by
+    mb_minimize_sd (see include/mollyb200.h for where the engine may differ from the reference). step_size in nm, tol in
+    kJ mol^-1 nm^-1. log_stream: a text stream that receives the reference's per-step lines after the call (None: none)."""
+    step_size: float = 0.01
+    max_steps: int = 1000
+    tol: float = 1000.0
+    log_stream: object = None
+
+    def __post_init__(self):
+        if not self.step_size > 0:
+            raise ValueError(f"step_size must be positive, found {self.step_size}")
+        if int(self.max_steps) < 0:
+            raise ValueError(f"max_steps must be non-negative, found {self.max_steps}")
+        if not self.tol >= 0:
+            raise ValueError(f"tol must be non-negative, found {self.tol}")
+
+
 # ------------------------------------------------------------------------------------------------
 # loggers: recorded on the device inside simulate (mb_simulate_vv_log)
 # ------------------------------------------------------------------------------------------------
@@ -673,10 +693,73 @@ def find_neighbors(sys: System, *args, **kwargs):
     return None
 
 
-def simulate(sys: System, sim: VelocityVerlet, n_steps: int, init_step: int = 0, rng=None, max_retries: int = 2,
-             run_loggers=True):
-    """simulate!(sys, sim::VelocityVerlet, n_steps; run_loggers) — src/simulators.jl:547-668. Mutates sys.coords /
-    velocities and appends to the histories of sys.loggers (recorded on the device, see _LogPlan)."""
+def sd_log_lines(trace) -> list:
+    """The lines simulate!(sys, ::SteepestDescentMinimizer) prints to its log_stream (src/simulators.jl:227-260), from the
+    records (step, E or E_trial, max force, accepted) of steepest_descent."""
+    t = np.asarray(trace, np.float64).reshape(-1, 4)
+    if len(t) == 0:
+        return []
+    lines = [f"Step {int(t[0, 0])} - potential energy {t[0, 1]} - max force N/A - N/A"]
+    for step, e, m, acc in t[1:]:
+        lines.append(f"Step {int(step)} - potential energy {e} - max force {m} - {'accepted' if acc else 'rejected'}")
+    return lines
+
+
+def steepest_descent(sys: System, sim: SteepestDescentMinimizer, init_step: int = 0, max_retries: int = 2):
+    """simulate!(sys, sim::SteepestDescentMinimizer; init_step) on the device (mb_minimize_sd). Mutates sys.coords (numpy or
+    torch CUDA, in place) and returns (sys, trace): trace is (n_iterations + 1, 4) float64 records (step, E or E_trial,
+    max force, accepted), record 0 = (init_step, E0, nan, 1). Also sets sys.minimize_result (the written-back fields)."""
+    ctx = sys.engine()
+    p = capi.MBSDParams()
+    p.step_size = float(sim.step_size)
+    p.max_steps = int(sim.max_steps)
+    p.tol = float(sim.tol)
+    p.init_step = int(init_step)
+    trace = np.zeros((p.max_steps + 1, 4), np.float64)
+    p.trace = trace.ctypes.data
+    p.trace_capacity = len(trace)
+    host = not hasattr(sys.coords, "data_ptr")
+    backup = sys.coords.copy() if host else None
+    scale = 1.0
+    for attempt in range(max_retries + 1):
+        rc = sys._L.mb_minimize_sd(ctx, _ptr(sys.coords), C.byref(p))
+        if rc == capi.MB_ERR_CAPACITY and backup is not None and attempt < max_retries:
+            sys.coords[...] = backup
+            scale *= 2.0
+            capi.check(sys._L.mb_set_capacity_scale(ctx, scale))
+            continue
+        capi.check(rc)
+        break
+    trace = trace[:p.n_iterations + 1].copy()
+    sys.minimize_result = dict(n_iterations=int(p.n_iterations), energy=float(p.energy), max_force=float(p.max_force),
+                               step_size=float(p.final_step_size), converged=bool(p.converged))
+    if sim.log_stream is not None:
+        for line in sd_log_lines(trace):
+            print(line, file=sim.log_stream)
+    return sys, trace
+
+
+def simulate(sys: System, sim, n_steps: Optional[int] = None, init_step: int = 0, rng=None, max_retries: int = 2,
+             run_loggers=None):
+    """simulate!(sys, sim, ...) dispatched on the simulator's type.
+
+    VelocityVerlet: simulate!(sys, sim, n_steps; run_loggers=true) — src/simulators.jl:547-668. Mutates sys.coords /
+    velocities and appends to the histories of sys.loggers (recorded on the device, see _LogPlan).
+    SteepestDescentMinimizer: simulate!(sys, sim; run_loggers=false) — src/simulators.jl:183-274, see steepest_descent.
+    Loggers are not run during a minimisation (run_loggers must be false)."""
+    if isinstance(sim, SteepestDescentMinimizer):
+        if n_steps is not None:
+            raise TypeError("simulate(sys, ::SteepestDescentMinimizer) takes no n_steps (the minimiser's max_steps bounds it)")
+        if run_loggers is not None and run_loggers is not False:
+            raise NotImplementedError("loggers are not run during a minimisation on the device (run_loggers must be false)")
+        steepest_descent(sys, sim, init_step=init_step, max_retries=max_retries)
+        return sys
+    if not isinstance(sim, VelocityVerlet):
+        raise TypeError(f"unsupported simulator {type(sim).__name__}")
+    if n_steps is None:
+        raise TypeError("simulate(sys, ::VelocityVerlet, n_steps) needs n_steps")
+    if run_loggers is None:
+        run_loggers = True
     _check_run_loggers(run_loggers)
     ctx = sys.engine()
     p = capi.MBVVParams()

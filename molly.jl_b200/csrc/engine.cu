@@ -12,6 +12,7 @@
 #include "cells.cuh"
 #include "common.cuh"
 #include "force.cuh"
+#include "minimize.cuh"
 #include "pair.cuh"
 #include "pme.cuh"
 #include "vv.cuh"
@@ -332,6 +333,7 @@ class EngineBase {
     virtual int set_dispersion(double r_cut) = 0;
     virtual int random_velocities(void* vels, double kT, uint64_t ctr1, uint64_t key) = 0;
     virtual int kinetic_tensor(const void* vels, double* out9) = 0;
+    virtual int minimize_sd(void* coords, mb_sd_params_t* p) = 0;
 };
 
 template <typename T>
@@ -688,6 +690,7 @@ class Engine : public EngineBase {
         g_ap_.tric = tric_;
         floor_ = CapFloor();
         have_list_ = false;
+        destroy_sd_graph();  // the minimiser's graph bakes the kernel parameters in
         dirty_ = false;
         return MB_OK;
     }
@@ -1854,6 +1857,7 @@ class Engine : public EngineBase {
     }
     void destroy_graph() {
         for (int m = 0; m < 8; m++) destroy_graph(m);
+        destroy_sd_graph();
     }
     // Capture one MD step (K1, decide, [IF rebuild], force, K2, [thermostat], [log records]) into an executable graph.
     int build_step_graph(const StepCfg& c, const GraphKey& key) {
@@ -2166,6 +2170,199 @@ class Engine : public EngineBase {
     }
 
     // ------------------------------------------------------------------------------------------
+    // Steepest-descent minimisation (minimize.cuh). The kept forces and saved positions are in original order: d_sd_f_,
+    // d_sd_x_; the trial's forces go to d_f4_ (slot order), so the context's force state is not preserved.
+    // The evaluation of the current positions, the decision and the accept pass (init: the starting coordinates)
+    int enqueue_sd_eval(bool init, const Capture* cap_while) {
+        Partials parts;
+        MB_TRY(launch_pairs(true, d_f4_.as<T4>(), false, &parts));
+        MB_TRY(launch_bonded(true));
+        sd_decide_kernel<<<1, SD_THREADS, 0, stream_>>>(d_sd_st_.as<SdState>(), parts.pe, parts.n,
+                                                        has_specific() ? d_sp_energy_.as<double>() : nullptr, init ? 1 : 0,
+                                                        cap_while ? cap_while->handle : 0, cap_while ? 1 : 0);
+        const int nb = std::max(1, std::min((int)((n_ + SD_THREADS - 1) / SD_THREADS), 4 * sm_count_));
+        sd_accept_kernel<T><<<nb, SD_THREADS, 0, stream_>>>((int)n_, path_ == 1 ? d_orig_.as<int>() : nullptr, d_f4_.as<T4>(),
+                                                            d_sd_f_.as<T4>(), d_sd_x_.as<T4>(), d_pos4_.as<T4>(), ext_map(),
+                                                            d_ctl_.as<Control>(), d_sd_st_.as<SdState>());
+        launches_ += 2;
+        MB_CUDA(cudaGetLastError());
+        return MB_OK;
+    }
+    // One iteration: trial, [rebuild], evaluation, decision, accept/restore. cap_if: capture mode, where the rebuild becomes a
+    // conditional IF node (its body is captured by the caller into *cap_if->body); otherwise the gated pipeline is enqueued.
+    int enqueue_sd_iter(const Capture* cap_if, const Capture* cap_while) {
+        const int nb = std::max(1, std::min((int)((n_ + SD_THREADS - 1) / SD_THREADS), 4 * sm_count_));
+        sd_trial_kernel<T><<<nb, SD_THREADS, 0, stream_>>>((int)n_, path_ == 1 ? d_orig_.as<int>() : nullptr, d_sd_f_.as<T4>(),
+                                                           d_pos4_.as<T4>(), d_sd_x_.as<T4>(), d_xref4_.as<T4>(),
+                                                           path_ == 1 ? g_.skin_half2 : (T)0, ext_map(), d_ctl_.as<Control>(),
+                                                           d_sd_st_.as<SdState>(), cap_if ? cap_if->handle : 0, cap_if ? 1 : 0);
+        launches_++;
+        if (path_ == 0) {
+            wrap_kernel<T><<<(int)((n_ + 255) / 256), 256, 0, stream_>>>((int)n_, g_ap_, d_pos4_.as<T4>());
+            launches_++;
+        } else if (cap_if) {
+            cudaStreamCaptureStatus status;
+            const cudaGraphNode_t* deps = nullptr;
+            size_t ndeps = 0;
+            cudaGraph_t gcap = nullptr;
+            MB_CUDA(cudaStreamGetCaptureInfo_v2(stream_, &status, nullptr, &gcap, &deps, &ndeps));
+            cudaGraphNodeParams cp = {cudaGraphNodeTypeConditional};
+            cp.type = cudaGraphNodeTypeConditional;
+            cp.conditional.handle = cap_if->handle;
+            cp.conditional.type = cudaGraphCondTypeIf;
+            cp.conditional.size = 1;
+            cudaGraphNode_t cnode;
+            MB_CUDA(cudaGraphAddNode(&cnode, gcap, deps, ndeps, &cp));
+            *cap_if->body = cp.conditional.phGraph_out[0];
+            MB_CUDA(cudaStreamUpdateCaptureDependencies(stream_, &cnode, 1, cudaStreamSetCaptureDependencies));
+        } else {
+            MB_TRY(enqueue_rebuild(true, false));
+        }
+        return enqueue_sd_eval(false, cap_while);
+    }
+    void destroy_sd_graph() {
+        if (sd_graph_.exec) cudaGraphExecDestroy(sd_graph_.exec);
+        if (sd_graph_.graph) cudaGraphDestroy(sd_graph_.graph);
+        sd_graph_.exec = nullptr;
+        sd_graph_.graph = nullptr;
+    }
+    // Capture the iteration loop: a conditional WHILE node (continue flag set by the decide kernel) whose body is one
+    // iteration, with the rebuild as a nested conditional IF node on the cell-list path.
+    int build_sd_graph(const GraphKey& key) {
+        destroy_sd_graph();
+        cudaGraph_t& gr = sd_graph_.graph;
+        const int64_t launches_before = launches_, evals_before = n_force_evals_;
+        auto fail = [&](int rc) {
+            cudaStreamCaptureStatus st;
+            if (cudaStreamIsCapturing(stream_, &st) == cudaSuccess && st != cudaStreamCaptureStatusNone) {
+                cudaGraph_t junk = nullptr;
+                cudaStreamEndCapture(stream_, &junk);
+            }
+            cudaGetLastError();
+            destroy_sd_graph();
+            launches_ = launches_before;
+            n_force_evals_ = evals_before;
+            return rc;
+        };
+        if (cudaGraphCreate(&gr, 0) != cudaSuccess) return fail(MB_ERR_CUDA);
+        cudaGraphConditionalHandle h_while = 0, h_if = 0;
+        if (cudaGraphConditionalHandleCreate(&h_while, gr, 1, cudaGraphCondAssignDefault) != cudaSuccess) return fail(MB_ERR_CUDA);
+        if (path_ == 1 && cudaGraphConditionalHandleCreate(&h_if, gr, 0, cudaGraphCondAssignDefault) != cudaSuccess)
+            return fail(MB_ERR_CUDA);
+        cudaGraphNodeParams cp = {cudaGraphNodeTypeConditional};
+        cp.type = cudaGraphNodeTypeConditional;
+        cp.conditional.handle = h_while;
+        cp.conditional.type = cudaGraphCondTypeWhile;
+        cp.conditional.size = 1;
+        cudaGraphNode_t wnode;
+        if (cudaGraphAddNode(&wnode, gr, nullptr, 0, &cp) != cudaSuccess) return fail(MB_ERR_CUDA);
+        cudaGraph_t loop_body = cp.conditional.phGraph_out[0], rebuild_body = nullptr;
+        if (cudaStreamBeginCaptureToGraph(stream_, loop_body, nullptr, nullptr, 0, cudaStreamCaptureModeRelaxed) != cudaSuccess)
+            return fail(MB_ERR_CUDA);
+        const Capture cap_if = {h_if, loop_body, &rebuild_body}, cap_while = {h_while, gr, nullptr};
+        if (enqueue_sd_iter(path_ == 1 ? &cap_if : nullptr, &cap_while) != MB_OK) return fail(MB_ERR_CUDA);
+        cudaGraph_t out = nullptr;
+        if (cudaStreamEndCapture(stream_, &out) != cudaSuccess) return fail(MB_ERR_CUDA);
+        const int64_t iter_launches = launches_ - launches_before;
+        if (path_ == 1) {
+            if (!rebuild_body) return fail(MB_ERR_CUDA);
+            if (cudaStreamBeginCaptureToGraph(stream_, rebuild_body, nullptr, nullptr, 0, cudaStreamCaptureModeRelaxed) != cudaSuccess)
+                return fail(MB_ERR_CUDA);
+            if (enqueue_rebuild(true, false) != MB_OK) return fail(MB_ERR_CUDA);
+            if (cudaStreamEndCapture(stream_, &out) != cudaSuccess) return fail(MB_ERR_CUDA);
+        }
+        if (cudaGraphInstantiate(&sd_graph_.exec, gr, 0) != cudaSuccess) return fail(MB_ERR_CUDA);
+        launches_ = launches_before;
+        n_force_evals_ = evals_before;
+        sd_graph_.launches = iter_launches;
+        sd_graph_.key = key;
+        return MB_OK;
+    }
+
+    int minimize_sd(void* coords, mb_sd_params_t* p) override {
+        MB_TRY(prepare());
+        if (!coords || !p) return set_error(MB_ERR_INVALID, "null argument");
+        if (p->max_steps < 0 || !(p->step_size > 0) || !(p->tol >= 0))
+            return set_error(MB_ERR_INVALID, "mb_minimize_sd: max_steps < 0, step_size <= 0 or tol < 0");
+        if (p->trace && p->trace_capacity < p->max_steps + 1)
+            return set_error(MB_ERR_INVALID, "mb_minimize_sd: trace capacity too small: this call writes up to " +
+                                                 std::to_string(p->max_steps + 1) + " records");
+        if (decomposed()) return set_error(MB_ERR_INVALID, "mb_minimize_sd: not available in decomposed (multi-GPU) runs");
+        CallerBuf xb, tb;
+        MB_TRY(caller_xyz(coords, d_stage_a_, true, xb));
+        const size_t rec_bytes = 4 * sizeof(double);
+        MB_TRY(caller_buf(p->trace, (size_t)(p->max_steps + 1) * rec_bytes, d_sd_trace_, false, tb));
+        const size_t np = (size_t)n_ + 16;
+        MB_CUDA(d_sd_f_.ensure(np * sizeof(T4)));
+        MB_CUDA(d_sd_x_.ensure(np * sizeof(T4)));
+        MB_CUDA(d_sd_st_.ensure(sizeof(SdState)));
+        MB_CUDA(d_sp_energy_.ensure(sizeof(double)));
+        SdState st;
+        memset(&st, 0, sizeof(st));
+        st.h = p->step_size;
+        st.tol = p->tol;
+        st.init_step = p->init_step;
+        st.max_steps = p->max_steps;
+        st.trace = tb.as<double>();
+        if (disp_rc_ > 0) {
+            MB_TRY(dispersion_prepare());
+            st.pe_const = (disp_f6_ + disp_f12_) / (box_[0] * box_[1] * box_[2]);
+        }
+        MB_CUDA(cudaMemcpyAsync(d_sd_st_.p, &st, sizeof(st), cudaMemcpyHostToDevice, stream_));
+        // start: wrapped coordinates (a forced rebuild wraps them on the cell-list path)
+        if (path_ == 0) {
+            init_slots(xb.as<T>());
+            wrap_kernel<T><<<(int)((n_ + 255) / 256), 256, 0, stream_>>>((int)n_, g_ap_, d_pos4_.as<T4>());
+            launches_++;
+        } else {
+            if (have_list_) MB_TRY(set_flag_rebuild());
+            MB_TRY(sync_state_from(xb.as<T>(), nullptr));
+        }
+        MB_TRY(enqueue_sd_eval(true, nullptr));
+        const bool use_graph = graph_enabled_ && !graph_failed_ && !prof_.enabled && !pme_on_ && p->max_steps > 0;
+        graph_used_ = false;
+        if (use_graph) {
+            const GraphKey key{path_, 0, 0, geom_version_, 0, -1, 0.0, 0.0, 0.0, n_};
+            if (!sd_graph_.exec || !(key == sd_graph_.key)) {
+                if (build_sd_graph(key) != MB_OK) graph_failed_ = true;  // stay on the stream path for this context
+            }
+            graph_used_ = !graph_failed_;
+        }
+        SdState out;
+        if (graph_used_) {
+            MB_CUDA(cudaGraphLaunch(sd_graph_.exec, stream_));
+            MB_CUDA(cudaMemcpyAsync(&out, d_sd_st_.p, sizeof(out), cudaMemcpyDeviceToHost, stream_));
+            MB_CUDA(cudaStreamSynchronize(stream_));
+            launches_ += out.iter * sd_graph_.launches;  // rebuild-body kernels are not counted
+            n_force_evals_ += out.iter;
+        } else {
+            for (int64_t k = 0; k < p->max_steps; k++) {
+                int cont = 0;
+                MB_CUDA(cudaMemcpyAsync(&cont, &d_sd_st_.as<SdState>()->cont, sizeof(int), cudaMemcpyDeviceToHost, stream_));
+                MB_CUDA(cudaStreamSynchronize(stream_));
+                if (!cont) break;
+                MB_TRY(enqueue_sd_iter(nullptr, nullptr));
+            }
+            MB_CUDA(cudaMemcpyAsync(&out, d_sd_st_.p, sizeof(out), cudaMemcpyDeviceToHost, stream_));
+            MB_CUDA(cudaStreamSynchronize(stream_));
+        }
+        export_kernel<T><<<(int)((n_ + 255) / 256), 256, 0, stream_>>>((int)n_, geom(), d_pos4_.as<T4>(), d_vel4_.as<T4>(),
+                                                                      d_orig_.as<int>(), d_cm_.as<CmState<T>>(), xb.as<T>(), nullptr);
+        launches_++;
+        MB_TRY(copy_back_xyz(xb));
+        MB_TRY(copy_back(tb, (size_t)(out.iter + 1) * rec_bytes));
+        p->n_iterations = out.iter;
+        p->energy = out.E;
+        p->max_force = out.m;
+        p->final_step_size = out.h;
+        p->converged = out.converged;
+        MB_CUDA(cudaGetLastError());
+        if (path_ == 1) MB_TRY(check_overflow_sync());
+        else MB_CUDA(cudaStreamSynchronize(stream_));
+        return MB_OK;
+    }
+
+    // ------------------------------------------------------------------------------------------
     // Per-CTA partials of `width` doubles each, written by launch(d_partial_) over nblk CTAs, summed on the host in block
     // order per component into out[width]
     template <typename Launch>
@@ -2311,6 +2508,7 @@ class Engine : public EngineBase {
     int64_t launches_ = 0, n_force_evals_ = 0, n_steps_ = 0;
     Prof prof_;
     StepGraph graphs_[8];
+    StepGraph sd_graph_;  // the minimiser's iteration loop (key: path, geometry version, n)
     bool graph_enabled_ = true, graph_failed_ = false, graph_used_ = false, own_stream_ = false;
     int geom_version_ = 0;
     // spatial decomposition (z-slabs of cell layers; one rank per GPU)
@@ -2359,6 +2557,8 @@ class Engine : public EngineBase {
     // device-side loggers: descriptor, KE partials, scratch forces of the energy evaluation, energy records and frame rings
     // staged for host outputs
     DevBuf d_log_desc_, d_log_part_, d_f4_log_, d_log_rec_, d_log_frames_[2];
+    // steepest-descent minimisation: kept forces and saved positions (original order), state, trace staged for a host output
+    DevBuf d_sd_f_, d_sd_x_, d_sd_st_, d_sd_trace_;
 };
 
 }  // namespace mb
@@ -2471,6 +2671,7 @@ int mb_simulate_vv_log(mb_ctx* ctx, void* coords, void* vels, const mb_vv_params
     MB_CTX_GUARD(ctx);
     return ctx->e->simulate_vv(coords, vels, p, log);
 }
+int mb_minimize_sd(mb_ctx* ctx, void* coords, mb_sd_params_t* p) { MB_CTX_GUARD(ctx); return ctx->e->minimize_sd(coords, p); }
 int mb_remove_cm_motion(mb_ctx* ctx, void* vels) { MB_CTX_GUARD(ctx); return ctx->e->remove_cm(vels); }
 int mb_kinetic_energy(mb_ctx* ctx, const void* vels, double* ke_host) { MB_CTX_GUARD(ctx); return ctx->e->kinetic_energy(vels, ke_host); }
 int mb_rebuild_neighbors(mb_ctx* ctx, const void* coords) { MB_CTX_GUARD(ctx); return ctx->e->rebuild(coords); }
