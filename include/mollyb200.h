@@ -188,6 +188,41 @@ typedef struct {
 } mb_vv_params_t;
 int mb_simulate_vv(mb_ctx* ctx, void* coords, void* vels, const mb_vv_params_t* p);
 
+/* Velocity-rescaling thermostats for mb_simulate_vv and mb_simulate_vv_log (src/coupling.jl:82-168, :227-238), in the
+ * reference's order (src/simulators.jl:616-643): after step n's second kick and its CM removal, K = 1/2 sum m v.v of the
+ * velocities after that removal, T = 2 K / (Nf k) with Nf = 3N - 3 (the df of `temperature`), and every velocity is
+ * scaled by lambda:
+ *  - MB_VC_IMMEDIATE (ImmediateThermostat(T0)): lambda = sqrt(T0 / T);
+ *  - MB_VC_BERENDSEN (BerendsenThermostat(T0, tau)): lambda^2 = 1 + (dt / tau) (T0 / T - 1);
+ *  - MB_VC_VRESCALE (VelocityRescaleThermostat(T0, tau; n_steps), Bussi et al. 2007): only on steps with n % n_steps == 0;
+ *    c = exp(-dt n_steps / tau), Kbar = Nf k T0 / 2, A = Kbar / (Nf K), lambda^2 = c + (1 - c) A (R^2 + S) + 2 sqrt(c (1 - c) A) R,
+ *    floored at eps(Float64), with R ~ N(0, 1) and S ~ chi^2 with Nf - 1 degrees of freedom.
+ * Loggers record after the coupling. K, lambda and the draws are computed on the device by the last CTA of the step's second
+ * kick (no host round trip); lambda is applied by the next reader of the velocities (the next step's drift kernel, the
+ * loggers, the export at the end of the call). Where the engine differs from the reference:
+ *  - random numbers: the reference draws R and the Nf - 1 normals of S from the host rng. The engine draws R and S on the
+ *    device from Philox4x32-10 keyed by mb_vv_params_t's rng_ctr1 / rng_key: block j (j = 0, 1, ...) has counter
+ *    (0xFFFFFFFF - j, step, ctr1) and key `rng_key`, a range of first words the Andersen thermostat (1..2n) never uses.
+ *    Block 0 gives R (Box-Muller of its first two words); S is one chi^2 draw, 2 Gamma((Nf - 1) / 2) by Marsaglia-Tsang
+ *    with proposals from blocks 1, 2, ... (shape < 1, i.e. Nf = 2: the shape + 1 draw times U^(1/shape), U from block 0's
+ *    third word; Nf = 1: S = 0). Every draw is a function of (keys, step, block) alone. The two agree in distribution
+ *    only, as for the Andersen thermostat;
+ *  - zero temperature: K = 0 (or Nf <= 0) leaves the velocities unchanged. The reference returns early for
+ *    VelocityRescaleThermostat and produces Inf/NaN velocities for the other two;
+ *  - Berendsen with dt / tau > 1 can make lambda^2 negative: the velocities become NaN (the reference raises a DomainError).
+ * The coupling set here is used by every later call until it is changed; NULL (or kind MB_VC_NONE) switches it off.
+ * MB_ERR_INVALID, before any work: an unknown kind, kT not finite or < 0, tau not finite or <= 0 (Berendsen,
+ * velocity rescale), n_steps < 1 (velocity rescale); and from mb_simulate_vv, an Andersen thermostat in the same call or a
+ * decomposed (multi-GPU) context. */
+enum { MB_VC_NONE = 0, MB_VC_IMMEDIATE = 1, MB_VC_BERENDSEN = 2, MB_VC_VRESCALE = 3 };
+typedef struct {
+    int32_t kind;      /* MB_VC_* */
+    int32_t n_steps;   /* MB_VC_VRESCALE: couple every n_steps steps (reference default 1) */
+    double kT;         /* k T0 in kJ/mol */
+    double tau;        /* coupling_const in ps (MB_VC_BERENDSEN, MB_VC_VRESCALE) */
+} mb_vcoupling_t;
+int mb_set_velocity_coupling(mb_ctx* ctx, const mb_vcoupling_t* c);
+
 /* Device-side loggers for mb_simulate_vv (apply_loggers!, src/loggers.jl:44-56, called by simulate! at init_step and after
  * every step, src/simulators.jl:575, :657). A step s is recorded when s % interval == 0 (GeneralObservableLogger,
  * src/loggers.jl:96-102): the steps init_step + 1 .. init_step + n_steps, and init_step itself when log_initial != 0
@@ -196,7 +231,7 @@ int mb_simulate_vv(mb_ctx* ctx, void* coords, void* vels, const mb_vv_params_t* 
  *    (pairwise + specific + PME + LJDispersionCorrection, as mb_forces_energy_all); ke = 1/2 sum m v.v of the
  *    velocities below, summed in double;
  *  - coordinate frame: n x 3, original atom order, wrapped into the box (as mb_simulate_vv returns them);
- *  - velocity frame: n x 3, after step s's CM removal and Andersen coupling: the velocities an unlogged call that stops
+ *  - velocity frame: n x 3, after step s's CM removal and coupling: the velocities an unlogged call that stops
  *    at step s returns.
  * Frames have the context's dtype. Outputs may be host or device pointers; host frames are staged through a bounded
  * device ring (at most 64 MiB per kind), not n_frames x n. Logging is an observer: the energy is a second evaluation

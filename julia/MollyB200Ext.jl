@@ -11,7 +11,8 @@
 #   Molly.simulate!(sys, sim::SteepestDescentMinimizer; ...)                                                simulators.jl:183
 # (Molly.remove_CM_motion! for CuArray Systems is NOT redefined: the stock extension owns that exact signature)
 # and falls through to the stock methods (invoke) for anything it does not recognise: non-cubic boundaries,
-# constraints, virtual sites, couplings other than AndersenThermostat, interactions outside
+# constraints, virtual sites, couplings other than one AndersenThermostat, ImmediateThermostat, BerendsenThermostat or
+# VelocityRescaleThermostat, interactions outside
 # {LennardJones, Coulomb, CoulombReactionField, CoulombEwald} or unsupported cutoffs / mixing rules.
 
 module MollyB200Ext
@@ -49,6 +50,14 @@ struct MBVVParams
     andersen_prob::Float64
     rng_ctr1::UInt64
     rng_key::UInt64
+end
+
+# mb_vcoupling_t (mb_set_velocity_coupling)
+struct MBVCoupling
+    kind::Int32       # 1 Immediate, 2 Berendsen, 3 velocity rescale (MB_VC_*)
+    n_steps::Int32
+    kT::Float64
+    tau::Float64
 end
 
 # mb_log_t; mutable so that ccall can write the record counts back
@@ -276,28 +285,54 @@ function takeover_params(sys, sim::VelocityVerlet, n_steps, init_step, rng)
     all(gi -> gi isa Molly.LJDispersionCorrection, sys.general_inters) || return nothing
     all(!isnothing, map(specific_desc, sys.specific_inter_lists)) || return nothing
     kT, prob = 0.0, 0.0
-    couplings = sim.coupling isa Tuple ? sim.coupling : (sim.coupling,)
+    vc = nothing
+    couplings = filter(c -> !(c isa Molly.NoCoupling), sim.coupling isa Tuple ? sim.coupling : (sim.coupling,))
     for c in couplings
-        c isa Molly.NoCoupling && continue
+        if length(couplings) == 1 && (c isa ImmediateThermostat || c isa BerendsenThermostat || c isa VelocityRescaleThermostat)
+            vc = vcoupling_desc(sys, c)
+            isnothing(vc) && return nothing
+            continue
+        end
         c isa AndersenThermostat || return nothing
         kT = Float64(ustrip(sys.k * c.temperature))
         prob = Float64(ustrip(sim.dt / c.coupling_const))
     end
     return MBVVParams(Float64(ustrip(sim.dt)), n_steps, init_step, Int32(sim.remove_CM_motion), kT, prob,
-                      rand(rng, UInt64), rand(rng, UInt64))
+                      rand(rng, UInt64), rand(rng, UInt64)), vc
+end
+
+# the velocity-rescaling thermostats with their units stripped: k T0 in the System's energy units, tau in ps
+_ps(x) = x isa Unitful.Quantity ? Float64(ustrip(u"ps", x)) : Float64(x)
+function vcoupling_desc(sys, c)
+    kT = Float64(ustrip(sys.k * c.temperature))
+    c isa ImmediateThermostat && return MBVCoupling(Int32(1), Int32(0), kT, 0.0)
+    c isa BerendsenThermostat && return MBVCoupling(Int32(2), Int32(0), kT, _ps(c.coupling_const))
+    c.n_steps isa Integer && c.n_steps >= 1 || return nothing
+    return MBVCoupling(Int32(3), Int32(c.n_steps), kT, _ps(c.coupling_const))
+end
+
+# set (or with `nothing`, clear) the context's velocity-rescaling thermostat; done on every taken-over call
+function set_velocity_coupling!(ctx, vc)
+    if isnothing(vc)
+        check(ccall((:mb_set_velocity_coupling, LIB), Cint, (Ptr{Cvoid}, Ptr{MBVCoupling}), ctx.handle, C_NULL))
+    else
+        check(ccall((:mb_set_velocity_coupling, LIB), Cint, (Ptr{Cvoid}, Ref{MBVCoupling}), ctx.handle, Ref(vc)))
+    end
 end
 
 function Molly.simulate!(sys::System{3, <:CuArray, T}, sim::VelocityVerlet, n_steps::Integer;
                          init_step=0, rng=Random.default_rng(), run_loggers=true, kwargs...) where T
     descs = engine_eligible(sys, sys.pairwise_inters)
-    p = isnothing(descs) ? nothing : takeover_params(sys, sim, n_steps, init_step, rng)
-    if isnothing(p)
+    tp = isnothing(descs) ? nothing : takeover_params(sys, sim, n_steps, init_step, rng)
+    if isnothing(tp)
         # stock: simulate!(sys, sim::VelocityVerlet, n_steps_or_time; ...) src/simulators.jl:547
         return invoke(Molly.simulate!, Tuple{Any, VelocityVerlet, Any}, sys, sim, n_steps;
                       init_step=init_step, rng=rng, run_loggers=run_loggers, kwargs...)
     end
+    p, vc = tp
     ctx = context_for(sys, descs)
     set_specific!(ctx, sys)
+    set_velocity_coupling!(ctx, vc)
     if run_loggers != false && !isempty(sys.loggers) && all(l -> !isnothing(device_log_kind(l)), values(sys.loggers))
         return simulate_logged!(sys, ctx, p, n_steps, init_step, run_loggers)
     end

@@ -9,6 +9,7 @@ from .api import *  # noqa: F401,F403
 from .api import (Atom, CubicBoundary, TriclinicBoundary, System, NoCutoff, DistanceCutoff, ShiftedPotentialCutoff,  # noqa: F401
                   ShiftedForceCutoff, LennardJones, Coulomb, CoulombReactionField, CoulombEwald, GPUNeighborFinder,
                   DistanceNeighborFinder, CellListMapNeighborFinder, TreeNeighborFinder, AndersenThermostat,
+                  ImmediateThermostat, BerendsenThermostat, VelocityRescaleThermostat,
                   VelocityVerlet, forces, forces_virial, potential_energy, forces_energy, find_neighbors, simulate,
                   kinetic_energy, temperature, remove_CM_motion, random_velocities, wrap_coords, device_count,
                   atoms_from_arrays, atoms_to_array, atom_dtype, MollyB200Error, COULOMB_CONST, BOLTZMANN_K,

@@ -11,6 +11,7 @@ MB_LJ, MB_COULOMB, MB_CRF, MB_EWALD_REAL = 0, 1, 2, 3
 MB_CUT_NONE, MB_CUT_DISTANCE, MB_CUT_SHIFTED_POTENTIAL, MB_CUT_SHIFTED_FORCE = 0, 1, 2, 3
 MB_CUT_CUBIC_SPLINE, MB_CUT_POLYNOMIAL = 4, 5
 MB_MIX_LORENTZ, MB_MIX_GEOMETRIC = 0, 1
+MB_VC_NONE, MB_VC_IMMEDIATE, MB_VC_BERENDSEN, MB_VC_VRESCALE = 0, 1, 2, 3
 MB_OK, MB_ERR_INVALID, MB_ERR_CUDA, MB_ERR_CAPACITY, MB_ERR_STATE, MB_ERR_NOGPU = 0, -1, -2, -3, -4, -5
 
 EXPORTED = [
@@ -20,7 +21,7 @@ EXPORTED = [
     "mb_stats", "mb_synchronize", "mb_set_capacity_scale", "mb_set_launch_config", "mb_comm_unique_id",
     "mb_comm_init", "mb_decomp_plan", "mb_set_profiling", "mb_set_specific", "mb_forces_energy_all", "mb_set_pme", "mb_pme_plan",
     "mb_set_lj_dispersion_correction", "mb_random_velocities", "mb_kinetic_energy_tensor", "mb_set_box_triclinic",
-    "mb_simulate_vv_log", "mb_minimize_sd",
+    "mb_simulate_vv_log", "mb_minimize_sd", "mb_set_velocity_coupling",
 ]
 
 
@@ -51,6 +52,10 @@ class MBVVParams(C.Structure):
         ("dt", C.c_double), ("n_steps", C.c_int64), ("init_step", C.c_int64), ("remove_cm_every", C.c_int32),
         ("andersen_kT", C.c_double), ("andersen_prob", C.c_double), ("rng_ctr1", C.c_uint64), ("rng_key", C.c_uint64),
     ]
+
+
+class MBVCoupling(C.Structure):
+    _fields_ = [("kind", C.c_int32), ("n_steps", C.c_int32), ("kT", C.c_double), ("tau", C.c_double)]
 
 
 class MBLog(C.Structure):
@@ -107,6 +112,7 @@ def load():
     L.mb_simulate_vv.argtypes = [vp, vp, vp, C.POINTER(MBVVParams)]
     L.mb_simulate_vv_log.argtypes = [vp, vp, vp, C.POINTER(MBVVParams), C.POINTER(MBLog)]
     L.mb_minimize_sd.argtypes = [vp, vp, C.POINTER(MBSDParams)]
+    L.mb_set_velocity_coupling.argtypes = [vp, C.POINTER(MBVCoupling)]
     L.mb_remove_cm_motion.argtypes = [vp, vp]
     L.mb_kinetic_energy.argtypes = [vp, vp, C.POINTER(dbl)]
     L.mb_rebuild_neighbors.argtypes = [vp, vp]

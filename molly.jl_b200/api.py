@@ -9,6 +9,8 @@ julia/MollyB200Ext.jl, see INTEGRATION.md):
     LennardJones, Coulomb, CoulombReactionField     src/interactions/lennard_jones.jl:28-35, coulomb.jl:32-70, :698-747
     GPUNeighborFinder (+ aliases)                   src/neighbors.jl:104-115
     VelocityVerlet, AndersenThermostat, simulate    src/simulators.jl:287-295, :547-668; src/coupling.jl:184-212
+    ImmediateThermostat, BerendsenThermostat,       src/coupling.jl:82-168, :227-238 (applied on the device inside
+    VelocityRescaleThermostat                       simulate, see mb_set_velocity_coupling)
     SteepestDescentMinimizer                        src/simulators.jl:183-274 (simulate dispatches on the simulator)
     forces, forces_virial, potential_energy         src/force.jl:678-720, src/energy.jl:202-248
     kinetic_energy, temperature, remove_CM_motion   src/energy.jl:44-175, src/spatial.jl:901-929
@@ -334,6 +336,64 @@ class InteractionList4Atoms:
 class AndersenThermostat:
     temperature: float
     coupling_const: float
+
+
+def _check_temperature(t):
+    if not (math.isfinite(t) and t >= 0):
+        raise ValueError(f"temperature must be finite and non-negative, found {t}")
+
+
+def _check_coupling_const(tau):
+    if not (math.isfinite(tau) and tau > 0):
+        raise ValueError(f"coupling_const must be finite and positive, found {tau}")
+
+
+@dataclass
+class ImmediateThermostat:
+    """ImmediateThermostat(temperature) — src/coupling.jl:82-91: lambda = sqrt(T0 / T) every step. Temperature in K."""
+    temperature: float
+
+    def __post_init__(self):
+        _check_temperature(self.temperature)
+
+    def descriptor(self, k):
+        return capi.MBVCoupling(capi.MB_VC_IMMEDIATE, 0, k * self.temperature, 0.0)
+
+
+@dataclass
+class BerendsenThermostat:
+    """BerendsenThermostat(temperature, coupling_const) — src/coupling.jl:227-238: lambda^2 = 1 + (dt / tau) (T0 / T - 1).
+    Temperature in K, coupling_const in ps."""
+    temperature: float
+    coupling_const: float
+
+    def __post_init__(self):
+        _check_temperature(self.temperature)
+        _check_coupling_const(self.coupling_const)
+
+    def descriptor(self, k):
+        return capi.MBVCoupling(capi.MB_VC_BERENDSEN, 0, k * self.temperature, self.coupling_const)
+
+
+@dataclass
+class VelocityRescaleThermostat:
+    """VelocityRescaleThermostat(temperature, coupling_const; n_steps=1) — src/coupling.jl:114-168, the stochastic velocity
+    rescaling of Bussi et al. 2007, every n_steps steps. The draws are made on the device (see mb_set_velocity_coupling)."""
+    temperature: float
+    coupling_const: float
+    n_steps: int = 1
+
+    def __post_init__(self):
+        _check_temperature(self.temperature)
+        _check_coupling_const(self.coupling_const)
+        if isinstance(self.n_steps, bool) or int(self.n_steps) != self.n_steps or self.n_steps < 1:
+            raise ValueError(f"n_steps must be a positive integer, found {self.n_steps}")
+
+    def descriptor(self, k):
+        return capi.MBVCoupling(capi.MB_VC_VRESCALE, int(self.n_steps), k * self.temperature, self.coupling_const)
+
+
+_SCALING_THERMOSTATS = (ImmediateThermostat, BerendsenThermostat, VelocityRescaleThermostat)
 
 
 @dataclass
@@ -761,7 +821,6 @@ def simulate(sys: System, sim, n_steps: Optional[int] = None, init_step: int = 0
     if run_loggers is None:
         run_loggers = True
     _check_run_loggers(run_loggers)
-    ctx = sys.engine()
     p = capi.MBVVParams()
     p.dt = float(sim.dt)
     p.n_steps = int(n_steps)
@@ -770,12 +829,17 @@ def simulate(sys: System, sim, n_steps: Optional[int] = None, init_step: int = 0
     p.andersen_kT = 0.0
     p.andersen_prob = 0.0
     couplings = sim.coupling if isinstance(sim.coupling, (tuple, list)) else ((sim.coupling,) if sim.coupling else ())
+    vc = None
     for c in couplings:
-        if isinstance(c, AndersenThermostat):
+        if isinstance(c, _SCALING_THERMOSTATS) and len(couplings) == 1:  # (one thermostat per run)
+            vc = c.descriptor(sys.k)
+        elif isinstance(c, AndersenThermostat):
             p.andersen_kT = sys.k * c.temperature
             p.andersen_prob = sim.dt / c.coupling_const
         else:
             raise TypeError(f"unsupported coupling {c!r} (the stock Molly path handles it)")
+    ctx = sys.engine()
+    capi.check(sys._L.mb_set_velocity_coupling(ctx, C.byref(vc) if vc is not None else None))
     rng = rng or np.random.default_rng()
     p.rng_ctr1 = int(rng.integers(0, 2 ** 63))
     p.rng_key = int(rng.integers(0, 2 ** 63))

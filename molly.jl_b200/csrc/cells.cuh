@@ -51,11 +51,14 @@ struct Control {
 };
 
 // centre-of-mass velocity waiting to be subtracted by the next reader of the velocities (vv.cuh; written by K2's last CTA
-// or by the force kernel's fused second kick)
+// or by the force kernel's fused second kick), and the velocity-rescaling thermostat's factor: the next reader applies
+// v <- lam (v - v_cm), each part when its flag is set
 template <typename T>
 struct CmState {
     T v[3];
     int valid;
+    T lam;
+    int scaled;
 };
 
 struct BrickHdr {

@@ -16,6 +16,9 @@
 #include "pair.cuh"
 #include "pme.cuh"
 #include "vv.cuh"
+static_assert((int)mb::VC_NONE == (int)MB_VC_NONE && (int)mb::VC_IMMEDIATE == (int)MB_VC_IMMEDIATE &&
+                  (int)mb::VC_BERENDSEN == (int)MB_VC_BERENDSEN && (int)mb::VC_VRESCALE == (int)MB_VC_VRESCALE,
+              "vrescale.cuh kinds = MB_VC_*");
 
 namespace mb {
 
@@ -334,6 +337,7 @@ class EngineBase {
     virtual int random_velocities(void* vels, double kT, uint64_t ctr1, uint64_t key) = 0;
     virtual int kinetic_tensor(const void* vels, double* out9) = 0;
     virtual int minimize_sd(void* coords, mb_sd_params_t* p) = 0;
+    mb_vcoupling_t vcoupling = {MB_VC_NONE, 0, 0.0, 0.0};  // mb_set_velocity_coupling (validated there)
 };
 
 template <typename T>
@@ -1680,6 +1684,7 @@ class Engine : public EngineBase {
         int do_cm;        // 0/1 constant, or -1: caller decides per step (stream path only)
         bool thermostat;
         int* flag_ptr;
+        VCouple vc;       // velocity-rescaling thermostat (kind VC_NONE: none)
     };
     // what one step does beyond the plain VelocityVerlet step
     struct StepOpts {
@@ -1712,7 +1717,8 @@ class Engine : public EngineBase {
         }
         prof_.begin(Prof::VV);
         const Thermo<T> th = thermo_in_k1(c);
-        with_const<true, false>(th.on != 0, [&](auto TH) {
+        const int thk = th.on ? TH_ANDERSEN : (c.vc.kind != VC_NONE ? TH_SCALE : TH_NONE);
+        with_const<TH_NONE, TH_ANDERSEN, TH_SCALE>(thk, [&](auto TH) {
             // two atoms per thread, one wave (48 registers: 5 CTAs per SM)
             vv_kick_drift_kernel<T, TH><<<std::max(1, std::min((nb + 1) / 2, 5 * sm_count_)), 256, 0, stream_>>>(
                 s0, n_own, c.dt, c.dt_half, c.skin_half2, cm, d_f4_.as<T4>(), d_xref4_.as<T4>(), d_pos4_.as<T4>(), d_vel4_.as<T4>(),
@@ -1769,9 +1775,11 @@ class Engine : public EngineBase {
         memset(&sig, 0, sizeof(sig));
         if (p2p_sig) sig = make_signal(epoch, o.do_cm != 0);
         prof_.begin(Prof::VV);
-        vv_kick2_kernel<T><<<vvb2, VV_THREADS, 0, stream_>>>(s0b, n_ownb, c.dt_half, o.do_cm, c.inv_mass, d_f4_.as<T4>(), d_mass_.as<T>(),
-                                                             d_vel4_.as<T4>(), d_partial_.as<double>(), ctl, cm, 0,
-                                                             dec ? d_mom_.as<double>() : nullptr, sig);
+        with_const<true, false>(c.vc.kind != VC_NONE, [&](auto CP) {
+            vv_kick2_kernel<T, CP><<<vvb2, VV_THREADS, 0, stream_>>>(s0b, n_ownb, c.dt_half, o.do_cm, c.inv_mass, d_f4_.as<T4>(),
+                                                                     d_mass_.as<T>(), d_vel4_.as<T4>(), d_partial_.as<double>(), ctl, cm, 0,
+                                                                     dec ? d_mom_.as<double>() : nullptr, sig, c.vc);
+        });
         prof_.end(Prof::VV);
         launches_++;
         if (p2p_sig && o.do_cm && o.defer_cm && !c.thermostat) {
@@ -1836,9 +1844,11 @@ class Engine : public EngineBase {
         int path, do_cm, thermostat, geom_version, rebuild_every, log_mask;
         double dt, kT, prob;
         int64_t n;
+        mb_vcoupling_t vc;  // the velocity-rescaling thermostat's kind and parameters (baked into K2's arguments)
         bool operator==(const GraphKey& o) const {
             return path == o.path && do_cm == o.do_cm && thermostat == o.thermostat && geom_version == o.geom_version &&
-                   rebuild_every == o.rebuild_every && log_mask == o.log_mask && dt == o.dt && kT == o.kT && prob == o.prob && n == o.n;
+                   rebuild_every == o.rebuild_every && log_mask == o.log_mask && dt == o.dt && kT == o.kT && prob == o.prob && n == o.n &&
+                   vc.kind == o.vc.kind && vc.n_steps == o.vc.n_steps && vc.kT == o.vc.kT && vc.tau == o.vc.tau;
         }
     };
     // one executable step graph per log mask; the host loop picks one per step
@@ -2007,6 +2017,12 @@ class Engine : public EngineBase {
         MB_TRY(prepare());
         if (!coords || !vels || !p) return set_error(MB_ERR_INVALID, "null argument");
         if (p->n_steps < 0 || !(p->dt > 0)) return set_error(MB_ERR_INVALID, "n_steps < 0 or dt <= 0");
+        if (vcoupling.kind != MB_VC_NONE) {
+            if (p->andersen_kT > 0 && p->andersen_prob > 0)
+                return set_error(MB_ERR_INVALID, "mb_simulate_vv: at most one thermostat per call (Andersen and a velocity-rescaling thermostat)");
+            if (decomposed())
+                return set_error(MB_ERR_INVALID, "mb_simulate_vv: velocity-rescaling thermostats are not available in decomposed (multi-GPU) runs");
+        }
         LogRun lr;
         MB_TRY(log_begin(log, p, lr));
         CallerBuf xb, vb;
@@ -2026,6 +2042,7 @@ class Engine : public EngineBase {
         c.kT = (T)p->andersen_kT;
         c.prob = p->andersen_prob;
         c.do_cm = (p->remove_cm_every == 0) ? 0 : (p->remove_cm_every == 1 ? 1 : -1);
+        c.vc = VCouple{vcoupling.kind, vcoupling.n_steps, 3 * (long long)n_ - 3, vcoupling.kT, p->dt, vcoupling.tau, total_mass_};
         if (path_ == 0) {
             init_slots(xb.as<T>());
             // velocities + wrap through ingest with an identity order (geometry only needs L)
@@ -2060,9 +2077,9 @@ class Engine : public EngineBase {
         bool cm_pending = false;  // host mirror of cm->valid
         if (p->init_step == 0 && p->remove_cm_every != 0) {
             // remove_CM_motion! before the first force evaluation (simulators.jl:563): zero-length kick
-            vv_kick2_kernel<T><<<vvb, VV_THREADS, 0, stream_>>>(0, (int)n_, (T)0, 1, c.inv_mass, d_f4_.as<T4>(), d_mass_.as<T>(),
-                                                                d_vel4_.as<T4>(), d_partial_.as<double>(), ctl, cm, 0, nullptr,
-                                                                PeerSignal{});
+            vv_kick2_kernel<T, false><<<vvb, VV_THREADS, 0, stream_>>>(0, (int)n_, (T)0, 1, c.inv_mass, d_f4_.as<T4>(), d_mass_.as<T>(),
+                                                                       d_vel4_.as<T4>(), d_partial_.as<double>(), ctl, cm, 0, nullptr,
+                                                                       PeerSignal{}, VCouple{});
             launches_++;
             cm_pending = true;
         }
@@ -2101,7 +2118,7 @@ class Engine : public EngineBase {
             for (int64_t k = 1; k <= p->n_steps; k++) need[log_mask_at(log, p->init_step + k)] = true;
             for (int m = 0; m < 8 && use_graph; m++) {
                 if (!need[m]) continue;
-                GraphKey key{path_, c.do_cm, c.thermostat ? 1 : 0, geom_version_, rebuild_every_, m, p->dt, p->andersen_kT, p->andersen_prob, n_};
+                GraphKey key{path_, c.do_cm, c.thermostat ? 1 : 0, geom_version_, rebuild_every_, m, p->dt, p->andersen_kT, p->andersen_prob, n_, vcoupling};
                 if (!graphs_[m].exec || !(key == graphs_[m].key)) {
                     if (build_step_graph(c, key) != MB_OK) {
                         graph_failed_ = true;  // stay on the stream path for this context
@@ -2322,7 +2339,7 @@ class Engine : public EngineBase {
         const bool use_graph = graph_enabled_ && !graph_failed_ && !prof_.enabled && !pme_on_ && p->max_steps > 0;
         graph_used_ = false;
         if (use_graph) {
-            const GraphKey key{path_, 0, 0, geom_version_, 0, -1, 0.0, 0.0, 0.0, n_};
+            const GraphKey key{path_, 0, 0, geom_version_, 0, -1, 0.0, 0.0, 0.0, n_, {MB_VC_NONE, 0, 0.0, 0.0}};
             if (!sd_graph_.exec || !(key == sd_graph_.key)) {
                 if (build_sd_graph(key) != MB_OK) graph_failed_ = true;  // stay on the stream path for this context
             }
@@ -2672,6 +2689,22 @@ int mb_simulate_vv_log(mb_ctx* ctx, void* coords, void* vels, const mb_vv_params
     return ctx->e->simulate_vv(coords, vels, p, log);
 }
 int mb_minimize_sd(mb_ctx* ctx, void* coords, mb_sd_params_t* p) { MB_CTX_GUARD(ctx); return ctx->e->minimize_sd(coords, p); }
+int mb_set_velocity_coupling(mb_ctx* ctx, const mb_vcoupling_t* c) {
+    MB_CTX_GUARD(ctx);
+    if (!c) {
+        ctx->e->vcoupling = mb_vcoupling_t{MB_VC_NONE, 0, 0.0, 0.0};
+        return MB_OK;
+    }
+    if (c->kind < MB_VC_NONE || c->kind > MB_VC_VRESCALE) return mb::set_error(MB_ERR_INVALID, "mb_set_velocity_coupling: unknown kind");
+    if (c->kind != MB_VC_NONE) {
+        if (!(std::isfinite(c->kT) && c->kT >= 0)) return mb::set_error(MB_ERR_INVALID, "mb_set_velocity_coupling: kT must be finite and >= 0");
+        if (c->kind != MB_VC_IMMEDIATE && !(std::isfinite(c->tau) && c->tau > 0))
+            return mb::set_error(MB_ERR_INVALID, "mb_set_velocity_coupling: the coupling constant must be finite and > 0");
+        if (c->kind == MB_VC_VRESCALE && c->n_steps < 1) return mb::set_error(MB_ERR_INVALID, "mb_set_velocity_coupling: n_steps < 1");
+    }
+    ctx->e->vcoupling = *c;
+    return MB_OK;
+}
 int mb_remove_cm_motion(mb_ctx* ctx, void* vels) { MB_CTX_GUARD(ctx); return ctx->e->remove_cm(vels); }
 int mb_kinetic_energy(mb_ctx* ctx, const void* vels, double* ke_host) { MB_CTX_GUARD(ctx); return ctx->e->kinetic_energy(vels, ke_host); }
 int mb_rebuild_neighbors(mb_ctx* ctx, const void* coords) { MB_CTX_GUARD(ctx); return ctx->e->rebuild(coords); }

@@ -10,6 +10,7 @@
 #pragma once
 #include "cells.cuh"
 #include "peer.cuh"
+#include "vrescale.cuh"
 
 namespace mb {
 
@@ -114,6 +115,7 @@ __global__ void export_kernel(int n, Geom<T> g, const typename VT<T>::T4* __rest
     if (vels) {
         typename VT<T>::T4 v = vel4[s];
         if (cm && cm->valid) { v.x -= cm->v[0]; v.y -= cm->v[1]; v.z -= cm->v[2]; }
+        if (cm && cm->scaled) { v.x *= cm->lam; v.y *= cm->lam; v.z *= cm->lam; }
         vels[3 * (size_t)o] = v.x;
         vels[3 * (size_t)o + 1] = v.y;
         vels[3 * (size_t)o + 2] = v.z;
@@ -185,9 +187,11 @@ __device__ __forceinline__ void andersen_apply(typename VT<T>::T4& v, int orig_i
 // ---- K1: first half kick + drift + displacement check; the last CTA to finish does the step bookkeeping:
 // advance step_n, apply the fixed-interval neighbour policy (find_neighbors every n_steps, src/neighbors.jl:671) and
 // publish the rebuild decision to the CUDA graph's conditional node (when the step runs as a graph).
-// THERMO: the variant that also applies the previous step's Andersen thermostat (Philox + Box-Muller inlined) is a separate
-// instantiation so that the plain kernel keeps its register count (one atom per thread, latency-bound: occupancy matters).
-template <typename T, bool THERMO>
+// THERMO: the variants that also apply the previous step's thermostat are separate instantiations so that the plain kernel
+// keeps its register count (one atom per thread, latency-bound: occupancy matters): TH_ANDERSEN resamples (Philox +
+// Box-Muller inlined), TH_SCALE applies the pending velocity-rescaling factor after the pending v_cm.
+enum { TH_NONE = 0, TH_ANDERSEN = 1, TH_SCALE = 2 };
+template <typename T, int THERMO>
 __global__ void vv_kick_drift_kernel(int s0, int n, T dt, T dt_half, T skin_half2, const CmState<T>* __restrict__ cm,
                                      const typename VT<T>::T4* __restrict__ f4,
                                      const typename VT<T>::T4* __restrict__ xref4, typename VT<T>::T4* __restrict__ pos4,
@@ -199,11 +203,13 @@ __global__ void vv_kick_drift_kernel(int s0, int n, T dt, T dt_half, T skin_half
     // same order of operations on v - subtract the pending v_cm, resample, then this step's first kick
     bool thermo = false;
     uint32_t t_step = 0, t_c0 = 0, t_c1 = 0, t_k0 = 0, t_k1 = 0;
-    if (THERMO && th.on) {  // (no loads from the control block on the path without a thermostat)
+    if (THERMO == TH_ANDERSEN && th.on) {  // (no loads from the control block on the path without a thermostat)
         thermo = ctl->step > ctl->init_step;
         t_step = (uint32_t)ctl->step; t_c0 = ctl->rng[0]; t_c1 = ctl->rng[1]; t_k0 = ctl->rng[2]; t_k1 = ctl->rng[3];
     }
     T cx = cm->v[0], cy = cm->v[1], cz = cm->v[2];
+    const bool scl = THERMO == TH_SCALE && cm->scaled != 0;
+    const T lam = THERMO == TH_SCALE ? cm->lam : (T)1;
     if (push.n_peer > 0 || push.cm_nranks > 0) {  // decomposed run over peer memory (peer.cuh)
         __shared__ double s_cm[3];
         // the neighbours must be done with the previous halo data before it is overwritten ...
@@ -257,7 +263,8 @@ __global__ void vv_kick_drift_kernel(int s0, int n, T dt, T dt_half, T skin_half
             if (!ok[u]) continue;
             const int s = s0 + k0 + u * stride;
             if (cmv) { v[u].x -= cx; v[u].y -= cy; v[u].z -= cz; }
-            if (THERMO && thermo) andersen_apply<T>(v[u], th.orig[s], th.n, th.mass[s], th.kT, th.prob, t_step, t_c0, t_c1, t_k0, t_k1);
+            if (THERMO == TH_SCALE && scl) { v[u].x *= lam; v[u].y *= lam; v[u].z *= lam; }
+            if (THERMO == TH_ANDERSEN && thermo) andersen_apply<T>(v[u], th.orig[s], th.n, th.mass[s], th.kT, th.prob, t_step, t_c0, t_c1, t_k0, t_k1);
             const T a = v[u].w * dt_half;  // (1/m) dt/2
             v[u].x += f[u].x * a; v[u].y += f[u].y * a; v[u].z += f[u].z * a;
             p[u].x += v[u].x * dt; p[u].y += v[u].y * dt; p[u].z += v[u].z * dt;
@@ -311,14 +318,25 @@ __global__ void vv_kick_drift_kernel(int s0, int n, T dt, T dt_half, T skin_half
 // Every CTA writes its partial sum(m v); the last CTA to finish adds the partials in index order
 // (deterministic) and publishes v_cm = sum(m v) / sum(m) (src/spatial.jl:901-916). The subtraction is
 // applied lazily by the next reader of the velocities (K1, the thermostat or export).
+// COUPLE: the variant for the velocity-rescaling thermostats (single GPU) also sums m v.v in double alongside sum(m v); the
+// last CTA takes K after this step's CM removal, K - u.sum(m v) + M |u|^2 / 2 with u the v_cm as stored, and stores the
+// thermostat's factor next to v_cm (vrescale.cuh).
 constexpr int VV_THREADS = 256;
+// the thermostat's factor for kinetic energy ke after this step's CM removal, stored as pending
 template <typename T>
+__device__ __forceinline__ void vcouple_store(CmState<T>* cm, const VCouple& vc, double ke, const Control* ctl) {
+    const uint32_t rng[4] = {ctl->rng[0], ctl->rng[1], ctl->rng[2], ctl->rng[3]};
+    cm->lam = (T)vcouple_lambda(vc, ke, ctl->step, rng);
+    cm->scaled = 1;
+}
+template <typename T, bool COUPLE>
 __global__ void __launch_bounds__(VV_THREADS)
     vv_kick2_kernel(int s0, int n, T dt_half, int do_cm, double inv_total_mass, const typename VT<T>::T4* __restrict__ f4,
                     const T* __restrict__ mass, typename VT<T>::T4* __restrict__ vel4, double* __restrict__ partial,
                     Control* __restrict__ ctl, CmState<T>* __restrict__ cm, int apply_pending, double* __restrict__ mom_out,
-                    PeerSignal sig) {
-    double px = 0, py = 0, pz = 0;
+                    PeerSignal sig, VCouple vc) {
+    constexpr int W = COUPLE ? 4 : 3;
+    double px = 0, py = 0, pz = 0, kk = 0;
     const int stride = gridDim.x * blockDim.x;
     for (int sa = s0 + blockIdx.x * blockDim.x + threadIdx.x; sa < s0 + n; sa += 2 * stride) {  // two atoms in flight per thread
         const int sb = sa + stride;
@@ -335,29 +353,35 @@ __global__ void __launch_bounds__(VV_THREADS)
         vb.x += fb.x * ab; vb.y += fb.y * ab; vb.z += fb.z * ab;
         vel4[sa] = va;
         px += (double)(va.x * ma); py += (double)(va.y * ma); pz += (double)(va.z * ma);
+        if (COUPLE) kk += (double)ma * ((double)va.x * va.x + (double)va.y * va.y + (double)va.z * va.z);
         if (okb) {
             vel4[sb] = vb;
             px += (double)(vb.x * mb_); py += (double)(vb.y * mb_); pz += (double)(vb.z * mb_);
+            if (COUPLE) kk += (double)mb_ * ((double)vb.x * vb.x + (double)vb.y * vb.y + (double)vb.z * vb.z);
         }
     }
-    if (!do_cm && sig.n_peer == 0) return;
+    if (!COUPLE && !do_cm && sig.n_peer == 0) return;
     const int tid = threadIdx.x;
-    double p[3] = {px, py, pz};
-    block_sum<VV_THREADS, 3>(p);
+    double p[W] = {px, py, pz};
+    if constexpr (COUPLE) p[W - 1] = kk;
+    block_sum<VV_THREADS, W>(p);
     if (tid == 0)
-        for (int k = 0; k < 3; k++) partial[3 * (size_t)blockIdx.x + k] = p[k];
+        for (int k = 0; k < W; k++) partial[W * (size_t)blockIdx.x + k] = p[k];
     if (last_cta(&ctl->ticket)) {
         __threadfence();
-        double s[3] = {0, 0, 0};
+        double s[W] = {};
         for (int i = tid; i < (int)gridDim.x; i += VV_THREADS)
-            for (int k = 0; k < 3; k++) s[k] += partial[3 * (size_t)i + k];
+            for (int k = 0; k < W; k++) s[k] += partial[W * (size_t)i + k];
         __syncthreads();  // block_sum's scratch is reused
-        block_sum<VV_THREADS, 3>(s);
+        block_sum<VV_THREADS, W>(s);
         if (tid == 0) {
             const double a = s[0], b = s[1], c = s[2];
             // peer-memory transport: the force kernel in front of this one is done with the halo data ...
             for (int q = 0; q < sig.n_peer; q++) st_release_sys(sig.read_flag[q], sig.epoch);
-            if (!do_cm) return;
+            if (!do_cm) {
+                if constexpr (COUPLE) vcouple_store<T>(cm, vc, 0.5 * s[W - 1], ctl);
+                return;
+            }
             if (sig.n_mom > 0) {  // ... and sum(m v) goes to every rank (peer_cm_kernel adds them in rank order)
                 for (int r = 0; r < sig.n_mom; r++) {
                     volatile double* d = sig.mom_dst[r];
@@ -372,6 +396,10 @@ __global__ void __launch_bounds__(VV_THREADS)
                 cm->v[1] = (T)(b * inv_total_mass);
                 cm->v[2] = (T)(c * inv_total_mass);
                 cm->valid = 1;
+            }
+            if constexpr (COUPLE) {  // (single GPU: v_cm was stored just above)
+                const double ux = cm->v[0], uy = cm->v[1], uz = cm->v[2];
+                vcouple_store<T>(cm, vc, 0.5 * s[W - 1] + 0.5 * vc.total_mass * (ux * ux + uy * uy + uz * uz) - (ux * a + uy * b + uz * c), ctl);
             }
         }
     }
@@ -416,6 +444,7 @@ template <typename T>
 __global__ void clear_cm_kernel(CmState<T>* cm) {
     cm->v[0] = cm->v[1] = cm->v[2] = (T)0;
     cm->valid = 0;
+    cm->scaled = 0;
 }
 
 // ---- Andersen thermostat (src/coupling.jl:184-212; GPU kernel src/kernels.jl:705-721) -----------
@@ -454,7 +483,7 @@ struct LogDesc {
     double pe_const;              // energy terms without a kernel (LJDispersionCorrection)
 };
 constexpr int LOG_THREADS = 256;
-// A read-only observer of the state after step ctl->step: applies the pending v_cm and previews the Andersen draw that the
+// A read-only observer of the state after step ctl->step: applies the pending v_cm and scale factor and previews the Andersen draw that the
 // next drift kernel (or the standalone thermostat closing the call) will apply, with the same operations, so the logged
 // velocities are those export_kernel would return after this step. KE = 1/2 sum m v.v in double, per-CTA partials added in
 // index order by the last CTA, which also adds the pair-energy partials of the ENERGY force launch in index order and
@@ -471,6 +500,7 @@ __global__ void __launch_bounds__(LOG_THREADS)
         const int o = orig[s];
         typename VT<T>::T4 v = vel4[s];
         if (cm->valid) { v.x -= cm->v[0]; v.y -= cm->v[1]; v.z -= cm->v[2]; }
+        if (cm->scaled) { v.x *= cm->lam; v.y *= cm->lam; v.z *= cm->lam; }
         if (th.on && ctl->step > ctl->init_step)
             andersen_apply<T>(v, o, th.n, mass[s], th.kT, th.prob, (uint32_t)ctl->step, ctl->rng[0], ctl->rng[1], ctl->rng[2], ctl->rng[3]);
         const double vx = v.x, vy = v.y, vz = v.z;
