@@ -254,6 +254,36 @@ typedef struct {
  * in decomposed (multi-GPU) runs, which do not log. After MB_ERR_CAPACITY the records are invalid, like the coordinates. */
 int mb_simulate_vv_log(mb_ctx* ctx, void* coords, void* vels, const mb_vv_params_t* p, mb_log_t* log);
 
+/* simulate!(sys, Langevin(dt, temperature, friction; remove_CM_motion), n_steps) (src/simulators.jl:1065-1210, O step
+ * src/kernels.jl:723-756; OpenMM's LangevinMiddleIntegrator, Zhang et al. 2019). c = exp(-dt friction) (vel_scale),
+ * sqrt(1 - c^2) (noise_scale), sigma_i = noise_scale sqrt(kT / m_i). Prologue as mb_simulate_vv: wrap, CM removal when
+ * init_step == 0 and remove_cm_every != 0, neighbours, F0, loggers at init_step. Step n: v += F/m dt; x += v dt/2;
+ * v = c v + sigma_i xi with xi ~ N(0, 1)^3; x += v dt/2; wrap; CM removal when n % remove_cm_every == 0; neighbours;
+ * F = forces(x) for step n + 1; loggers. The velocities are half a step behind the positions, and the loggers (mb_log_t, as
+ * for mb_simulate_vv_log; NULL: no logging) record that state. One step is one fused kernel plus the force evaluation.
+ * Where the engine differs from the reference:
+ *  - random numbers: xi of atom i (1-based original index) at step n is the Box-Muller transform of one Philox4x32-10 block
+ *    with counter (i, n, ctr1) and key `rng_key` (the first two words give x and y, the last two z). The reference
+ *    advances ctr1 by one per step and uses counters i and i + n_atoms. Both are functions of (keys, step, atom) only, so a
+ *    run split into calls with the same keys takes the same draws; the two agree in distribution only (PhiloxRNG.jl's
+ *    transform is not vendored), as for the Andersen thermostat;
+ *  - f32: c v + sigma xi is formed in double and rounded once;
+ *  - massless atoms (1/m = 0) get no kick and no noise: v <- c v (the reference's sigma is Inf there);
+ *  - sigma_i is formed from the context's 1/m (rounded to the dtype in f32).
+ * MB_ERR_INVALID before any work for dt <= 0, n_steps < 0, kT or friction negative or not finite, a velocity coupling set
+ * on the context (mb_set_velocity_coupling; couplings with Langevin take the stock path), a decomposed (multi-GPU)
+ * context, and the logging errors of mb_simulate_vv_log. MB_ERR_CAPACITY as in mb_simulate_vv. */
+typedef struct {
+    double dt;
+    int64_t n_steps;
+    int64_t init_step;
+    int32_t remove_cm_every;    /* Langevin.remove_CM_motion (default 1; 0 = never) */
+    double kT;                  /* k * temperature in kJ/mol */
+    double friction;            /* ps^-1 */
+    uint64_t rng_ctr1, rng_key; /* the two rand(rng, UInt64) of src/simulators.jl:1135-1136 */
+} mb_langevin_params_t;
+int mb_simulate_langevin(mb_ctx* ctx, void* coords, void* vels, const mb_langevin_params_t* p, mb_log_t* log);
+
 /* simulate!(sys, SteepestDescentMinimizer(step_size, max_steps, tol)) (src/simulators.jl:183-274) on the device: wrap the
  * coordinates, E = potential energy; then for step n = init_step+1 .. init_step+max_steps: F = forces, m = max |F_i|,
  * x <- wrap(x + h F / m), E_trial = potential energy; E_trial < E accepts (h <- 6h/5, E <- E_trial), otherwise x is restored

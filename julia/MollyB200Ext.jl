@@ -9,6 +9,7 @@
 #   Molly.pairwise_pe_loop_gpu!(pe_vec_nounits, buffers, sys, pairwise_inters, nbs::Nothing, step_n)        ext:936
 #   Molly.simulate!(sys, sim::VelocityVerlet, n_steps; ...)                                                 simulators.jl:547
 #   Molly.simulate!(sys, sim::SteepestDescentMinimizer; ...)                                                simulators.jl:183
+#   Molly.simulate!(sys, sim::Langevin, n_steps; ...) with coupling === nothing                              simulators.jl:1101
 # (Molly.remove_CM_motion! for CuArray Systems is NOT redefined: the stock extension owns that exact signature)
 # and falls through to the stock methods (invoke) for anything it does not recognise: non-cubic boundaries,
 # constraints, virtual sites, couplings other than one AndersenThermostat, ImmediateThermostat, BerendsenThermostat or
@@ -48,6 +49,18 @@ struct MBVVParams
     remove_cm_every::Int32
     andersen_kT::Float64
     andersen_prob::Float64
+    rng_ctr1::UInt64
+    rng_key::UInt64
+end
+
+# mb_langevin_params_t (mb_simulate_langevin)
+struct MBLangevinParams
+    dt::Float64
+    n_steps::Int64
+    init_step::Int64
+    remove_cm_every::Int32
+    kT::Float64
+    friction::Float64
     rng_ctr1::UInt64
     rng_key::UInt64
 end
@@ -352,6 +365,40 @@ function Molly.simulate!(sys::System{3, <:CuArray, T}, sim::VelocityVerlet, n_st
     return sys
 end
 
+# ---- simulate!(sys, ::Langevin, n) (src/simulators.jl:1101-1210) ------------------------------------------------------------
+# Taken over when the coupling is nothing, the System is eligible as for VelocityVerlet, and the loggers are none, not run,
+# or all ones the engine records; the whole run is then one mb_simulate_langevin call. The velocity coupling of the context
+# is cleared first. Anything else (barostats, constraints, virtual sites, host-side loggers) runs the stock method.
+function Molly.simulate!(sys::System{3, <:CuArray, T}, sim::Langevin, n_steps::Integer;
+                         init_step=0, rng=Random.default_rng(), run_loggers=true, kwargs...) where T
+    descs = engine_eligible(sys, sys.pairwise_inters)
+    device_logs = run_loggers == false || isempty(sys.loggers) ||
+                  all(l -> !isnothing(device_log_kind(l)), values(sys.loggers))
+    if isnothing(descs) || !isnothing(sim.coupling) || !device_logs ||
+            !all(gi -> gi isa Molly.LJDispersionCorrection, sys.general_inters) ||
+            !all(!isnothing, map(specific_desc, sys.specific_inter_lists))
+        # stock: simulate!(sys, sim::Langevin, n_steps_or_time; ...) src/simulators.jl:1101
+        return invoke(Molly.simulate!, Tuple{Any, Langevin, Any}, sys, sim, n_steps;
+                      init_step=init_step, rng=rng, run_loggers=run_loggers, kwargs...)
+    end
+    ctx = context_for(sys, descs)
+    set_specific!(ctx, sys)
+    set_velocity_coupling!(ctx, nothing)
+    friction = sim.friction isa Unitful.Quantity ? Float64(ustrip(u"ps^-1", sim.friction)) : Float64(sim.friction)
+    p = MBLangevinParams(_ps(sim.dt), n_steps, init_step, Int32(sim.remove_CM_motion),
+                         Float64(ustrip(sys.k * sim.temperature)), friction,
+                         rand(rng, UInt64), rand(rng, UInt64))
+    if run_loggers != false && !isempty(sys.loggers)
+        return simulate_logged!(sys, ctx, n_steps, init_step, run_loggers) do lg
+            ccall((:mb_simulate_langevin, LIB), Cint, (Ptr{Cvoid}, CuPtr{Cvoid}, CuPtr{Cvoid}, Ref{MBLangevinParams}, Ref{MBLog}),
+                  ctx.handle, pointer(sys.coords), pointer(sys.velocities), Ref(p), lg)
+        end
+    end
+    check(ccall((:mb_simulate_langevin, LIB), Cint, (Ptr{Cvoid}, CuPtr{Cvoid}, CuPtr{Cvoid}, Ref{MBLangevinParams}, Ptr{MBLog}),
+                ctx.handle, pointer(sys.coords), pointer(sys.velocities), Ref(p), C_NULL))
+    return sys
+end
+
 # ---- simulate!(sys, ::SteepestDescentMinimizer) (src/simulators.jl:183-274) ------------------------------------------------
 # Taken over when the System is engine-eligible, has no constraints, no general interactions (the engine would need their
 # energies for the log lines) and run_loggers is false: the whole minimisation is one mb_minimize_sd call, and the
@@ -420,6 +467,12 @@ function record_steps(every, n_steps, init_step, run_loggers)
 end
 
 function simulate_logged!(sys::System{3, <:CuArray, T}, ctx, p, n_steps, init_step, run_loggers) where T
+    return simulate_logged!(sys, ctx, n_steps, init_step, run_loggers) do lg
+        ccall((:mb_simulate_vv_log, LIB), Cint, (Ptr{Cvoid}, CuPtr{Cvoid}, CuPtr{Cvoid}, Ref{MBVVParams}, Ref{MBLog}),
+              ctx.handle, pointer(sys.coords), pointer(sys.velocities), Ref(p), lg)
+    end
+end
+function simulate_logged!(run, sys::System{3, <:CuArray, T}, ctx, n_steps, init_step, run_loggers) where T
     kinds = Dict(name => device_log_kind(l) for (name, l) in pairs(sys.loggers))
     gcd_of(sel) = reduce(gcd, (l.n_steps for (name, l) in pairs(sys.loggers) if kinds[name] in sel); init=0)
     e_every, x_every, v_every = gcd_of((:pe, :ke, :total, :temp)), gcd_of((:coords,)), gcd_of((:vels,))
@@ -435,9 +488,7 @@ function simulate_logged!(sys::System{3, <:CuArray, T}, ctx, p, n_steps, init_st
                reinterpret(Ptr{Float64}, pointer(erec)), reinterpret(Ptr{Cvoid}, pointer(xrec)),
                reinterpret(Ptr{Cvoid}, pointer(vrec)), length(e_steps), length(x_steps), length(v_steps), 0, 0, 0)
     GC.@preserve erec xrec vrec begin
-        check(ccall((:mb_simulate_vv_log, LIB), Cint,
-                    (Ptr{Cvoid}, CuPtr{Cvoid}, CuPtr{Cvoid}, Ref{MBVVParams}, Ref{MBLog}),
-                    ctx.handle, pointer(sys.coords), pointer(sys.velocities), Ref(p), lg))
+        check(run(lg))
     end
     e = Array(erec)
     eu, du, vu = sys.energy_units, unit(eltype(eltype(sys.coords))), unit(eltype(eltype(sys.velocities)))

@@ -12,6 +12,7 @@ julia/MollyB200Ext.jl, see INTEGRATION.md):
     ImmediateThermostat, BerendsenThermostat,       src/coupling.jl:82-168, :227-238 (applied on the device inside
     VelocityRescaleThermostat                       simulate, see mb_set_velocity_coupling)
     SteepestDescentMinimizer                        src/simulators.jl:183-274 (simulate dispatches on the simulator)
+    Langevin                                        src/simulators.jl:1065-1210 (mb_simulate_langevin)
     forces, forces_virial, potential_energy         src/force.jl:678-720, src/energy.jl:202-248
     kinetic_energy, temperature, remove_CM_motion   src/energy.jl:44-175, src/spatial.jl:901-929
     *EnergyLogger, TemperatureLogger, Coordinates-  src/loggers.jl:44-102, :134-278 (recorded on the device inside
@@ -401,6 +402,34 @@ class VelocityVerlet:
     dt: float
     coupling: object = None
     remove_CM_motion: int = 1
+
+
+@dataclass
+class Langevin:
+    """Langevin(dt, temperature, friction; coupling=None, remove_CM_motion=1) — src/simulators.jl:1065-1100, Molly's port of
+    OpenMM's LangevinMiddleIntegrator, run on the device by mb_simulate_langevin (see include/mollyb200.h for where the
+    engine differs from the reference). dt in ps, temperature in K, friction in ps^-1. vel_scale = exp(-dt friction) and
+    noise_scale = sqrt(1 - vel_scale^2) as the reference's constructor computes them. A coupling (the reference's barostats)
+    is not run by the engine: simulate refuses it."""
+    dt: float
+    temperature: float
+    friction: float
+    coupling: object = None
+    remove_CM_motion: int = 1
+    vel_scale: float = field(init=False)
+    noise_scale: float = field(init=False)
+
+    def __post_init__(self):
+        if not (math.isfinite(self.dt) and self.dt > 0):
+            raise ValueError(f"dt must be finite and positive, found {self.dt}")
+        _check_temperature(self.temperature)
+        if not (math.isfinite(self.friction) and self.friction >= 0):
+            raise ValueError(f"friction must be finite and non-negative, found {self.friction}")
+        self.remove_CM_motion = int(self.remove_CM_motion)  # Int(remove_CM_motion): false -> 0
+        if self.remove_CM_motion < 0:
+            raise ValueError(f"remove_CM_motion must be non-negative, found {self.remove_CM_motion}")
+        self.vel_scale = math.exp(-self.dt * self.friction)
+        self.noise_scale = math.sqrt(1 - self.vel_scale ** 2)
 
 
 @dataclass
@@ -805,6 +834,8 @@ def simulate(sys: System, sim, n_steps: Optional[int] = None, init_step: int = 0
 
     VelocityVerlet: simulate!(sys, sim, n_steps; run_loggers=true) — src/simulators.jl:547-668. Mutates sys.coords /
     velocities and appends to the histories of sys.loggers (recorded on the device, see _LogPlan).
+    Langevin: simulate!(sys, sim, n_steps; run_loggers=true) — src/simulators.jl:1101-1210, the same arguments and loggers
+    as VelocityVerlet; the velocities are half a step behind the positions.
     SteepestDescentMinimizer: simulate!(sys, sim; run_loggers=false) — src/simulators.jl:183-274, see steepest_descent.
     Loggers are not run during a minimisation (run_loggers must be false)."""
     if isinstance(sim, SteepestDescentMinimizer):
@@ -814,32 +845,39 @@ def simulate(sys: System, sim, n_steps: Optional[int] = None, init_step: int = 0
             raise NotImplementedError("loggers are not run during a minimisation on the device (run_loggers must be false)")
         steepest_descent(sys, sim, init_step=init_step, max_retries=max_retries)
         return sys
-    if not isinstance(sim, VelocityVerlet):
+    if not isinstance(sim, (VelocityVerlet, Langevin)):
         raise TypeError(f"unsupported simulator {type(sim).__name__}")
     if n_steps is None:
-        raise TypeError("simulate(sys, ::VelocityVerlet, n_steps) needs n_steps")
+        raise TypeError(f"simulate(sys, ::{type(sim).__name__}, n_steps) needs n_steps")
     if run_loggers is None:
         run_loggers = True
     _check_run_loggers(run_loggers)
-    p = capi.MBVVParams()
+    couplings = sim.coupling if isinstance(sim.coupling, (tuple, list)) else ((sim.coupling,) if sim.coupling else ())
+    vc = None
+    if isinstance(sim, Langevin):
+        if couplings:
+            raise TypeError(f"unsupported coupling {couplings[0]!r} with Langevin (the stock Molly path handles it)")
+        p = capi.MBLangevinParams()
+        p.kT = sys.k * sim.temperature
+        p.friction = float(sim.friction)
+    else:
+        p = capi.MBVVParams()
+        p.andersen_kT = 0.0
+        p.andersen_prob = 0.0
+        for c in couplings:
+            if isinstance(c, _SCALING_THERMOSTATS) and len(couplings) == 1:  # (one thermostat per run)
+                vc = c.descriptor(sys.k)
+            elif isinstance(c, AndersenThermostat):
+                p.andersen_kT = sys.k * c.temperature
+                p.andersen_prob = sim.dt / c.coupling_const
+            else:
+                raise TypeError(f"unsupported coupling {c!r} (the stock Molly path handles it)")
     p.dt = float(sim.dt)
     p.n_steps = int(n_steps)
     p.init_step = int(init_step)
     p.remove_cm_every = int(sim.remove_CM_motion)
-    p.andersen_kT = 0.0
-    p.andersen_prob = 0.0
-    couplings = sim.coupling if isinstance(sim.coupling, (tuple, list)) else ((sim.coupling,) if sim.coupling else ())
-    vc = None
-    for c in couplings:
-        if isinstance(c, _SCALING_THERMOSTATS) and len(couplings) == 1:  # (one thermostat per run)
-            vc = c.descriptor(sys.k)
-        elif isinstance(c, AndersenThermostat):
-            p.andersen_kT = sys.k * c.temperature
-            p.andersen_prob = sim.dt / c.coupling_const
-        else:
-            raise TypeError(f"unsupported coupling {c!r} (the stock Molly path handles it)")
     ctx = sys.engine()
-    capi.check(sys._L.mb_set_velocity_coupling(ctx, C.byref(vc) if vc is not None else None))
+    capi.check(sys._L.mb_set_velocity_coupling(ctx, C.byref(vc) if vc is not None else None))  # (Langevin: cleared)
     rng = rng or np.random.default_rng()
     p.rng_ctr1 = int(rng.integers(0, 2 ** 63))
     p.rng_key = int(rng.integers(0, 2 ** 63))
@@ -848,7 +886,10 @@ def simulate(sys: System, sim, n_steps: Optional[int] = None, init_step: int = 0
     plan = _LogPlan(sys, int(n_steps), int(init_step), run_loggers) if sys.loggers and run_loggers is not False else None
     scale = 1.0
     for attempt in range(max_retries + 1):
-        if plan is None:
+        if isinstance(sim, Langevin):
+            rc = sys._L.mb_simulate_langevin(ctx, _ptr(sys.coords), _ptr(sys.velocities), C.byref(p),
+                                             C.byref(plan.desc) if plan is not None else None)
+        elif plan is None:
             rc = sys._L.mb_simulate_vv(ctx, _ptr(sys.coords), _ptr(sys.velocities), C.byref(p))
         else:  # a retry overwrites the records of the failed attempt
             rc = sys._L.mb_simulate_vv_log(ctx, _ptr(sys.coords), _ptr(sys.velocities), C.byref(p), C.byref(plan.desc))

@@ -234,5 +234,18 @@ __host__ __device__ inline void philox4x32_10(uint32_t c[4], uint32_t k0, uint32
         k1 += W1;
     }
 }
+// Three N(0, sd^2) draws from one Philox block d by Box-Muller: (sd r1 cos 2 pi u2, sd r1 sin 2 pi u2, sd r2 cos 2 pi u4) with
+// r1, r2 = sqrt(-2 log u1), sqrt(-2 log u3), u1, u3 = (d[0] + 1) / 2^32, (d[2] + 1) / 2^32 in (0, 1] (log stays finite) and
+// u2, u4 = d[1] / 2^32, d[3] / 2^32 in [0, 1). The Langevin integrator's O step; the same transform as the Andersen
+// thermostat's resampling (andersen_apply keeps its own copy of these lines: calling this helper changes its SASS).
+__host__ __device__ __forceinline__ void box_muller3(const uint32_t d[4], double sd, double out[3]) {
+    const double two_pi = 6.283185307179586;
+    const double u1 = ((double)d[0] + 1.0) * (1.0 / 4294967296.0), u2 = (double)d[1] * (1.0 / 4294967296.0);
+    const double u3 = ((double)d[2] + 1.0) * (1.0 / 4294967296.0), u4 = (double)d[3] * (1.0 / 4294967296.0);
+    const double r1 = sqrt(-2.0 * log(u1)), r2 = sqrt(-2.0 * log(u3));
+    out[0] = sd * r1 * cos(two_pi * u2);
+    out[1] = sd * r1 * sin(two_pi * u2);
+    out[2] = sd * r2 * cos(two_pi * u4);
+}
 
 }  // namespace mb

@@ -12,6 +12,7 @@
 #include "cells.cuh"
 #include "common.cuh"
 #include "force.cuh"
+#include "langevin.cuh"
 #include "minimize.cuh"
 #include "pair.cuh"
 #include "pme.cuh"
@@ -321,7 +322,8 @@ class EngineBase {
                                const int32_t* sj) = 0;
     virtual int set_neighbor_policy(double r_list, int rebuild_every) = 0;
     virtual int forces_energy(const void* coords, void* fs, void* pe, void* vir, int64_t step_n, bool with_specific) = 0;
-    virtual int simulate_vv(void* coords, void* vels, const mb_vv_params_t* p, mb_log_t* log) = 0;
+    // lg: the Langevin integrator's parameters, NULL for VelocityVerlet (p then carries the fields both share)
+    virtual int simulate(void* coords, void* vels, const mb_vv_params_t* p, const mb_langevin_params_t* lg, mb_log_t* log) = 0;
     virtual int remove_cm(void* vels) = 0;
     virtual int kinetic_energy(const void* vels, double* out) = 0;
     virtual int rebuild(const void* coords) = 0;
@@ -1685,6 +1687,8 @@ class Engine : public EngineBase {
         bool thermostat;
         int* flag_ptr;
         VCouple vc;       // velocity-rescaling thermostat (kind VC_NONE: none)
+        bool langevin;    // the integrator: Langevin (langevin.cuh) or VelocityVerlet
+        LangevinCoef lc;  // Langevin's c, sqrt(1 - c^2) and kT
     };
     // what one step does beyond the plain VelocityVerlet step
     struct StepOpts {
@@ -1716,17 +1720,26 @@ class Engine : public EngineBase {
             cm_deferred_epoch_ = 0;
         }
         prof_.begin(Prof::VV);
-        const Thermo<T> th = thermo_in_k1(c);
-        const int thk = th.on ? TH_ANDERSEN : (c.vc.kind != VC_NONE ? TH_SCALE : TH_NONE);
-        with_const<TH_NONE, TH_ANDERSEN, TH_SCALE>(thk, [&](auto TH) {
-            // two atoms per thread, one wave (48 registers: 5 CTAs per SM)
-            vv_kick_drift_kernel<T, TH><<<std::max(1, std::min((nb + 1) / 2, 5 * sm_count_)), 256, 0, stream_>>>(
-                s0, n_own, c.dt, c.dt_half, c.skin_half2, cm, d_f4_.as<T4>(), d_xref4_.as<T4>(), d_pos4_.as<T4>(), d_vel4_.as<T4>(),
-                c.flag_ptr, ctl, cap ? cap->handle : 0, cap && path_ == 1 ? 1 : 0, push, ext_map(), th);
-        });
+        if (c.langevin) {
+            // (single GPU: s0 = 0.) At most vvb CTAs, so d_partial_ (max(vvb, 2048) x 8 doubles, prepare) holds their 3 each
+            const int lgb = std::max(1, std::min(nb, 8 * sm_count_));
+            langevin_step_kernel<T><<<lgb, VV_THREADS, 0, stream_>>>(
+                n_own, c.dt, c.dt_half, c.skin_half2, c.lc, o.do_cm, c.inv_mass, cm, d_f4_.as<T4>(), d_xref4_.as<T4>(),
+                d_pos4_.as<T4>(), d_vel4_.as<T4>(), d_orig_.as<int>(), d_mass_.as<T>(), d_partial_.as<double>(), c.flag_ptr, ctl,
+                cap ? cap->handle : 0, cap && path_ == 1 ? 1 : 0, ext_map());
+        } else {
+            const Thermo<T> th = thermo_in_k1(c);
+            const int thk = th.on ? TH_ANDERSEN : (c.vc.kind != VC_NONE ? TH_SCALE : TH_NONE);
+            with_const<TH_NONE, TH_ANDERSEN, TH_SCALE>(thk, [&](auto TH) {
+                // two atoms per thread, one wave (48 registers: 5 CTAs per SM)
+                vv_kick_drift_kernel<T, TH><<<std::max(1, std::min((nb + 1) / 2, 5 * sm_count_)), 256, 0, stream_>>>(
+                    s0, n_own, c.dt, c.dt_half, c.skin_half2, cm, d_f4_.as<T4>(), d_xref4_.as<T4>(), d_pos4_.as<T4>(), d_vel4_.as<T4>(),
+                    c.flag_ptr, ctl, cap ? cap->handle : 0, cap && path_ == 1 ? 1 : 0, push, ext_map(), th);
+            });
+        }
         prof_.end(Prof::VV);
         launches_++;
-        if (o.clear_cm_after_k1) {
+        if (o.clear_cm_after_k1) {  // (VelocityVerlet: the Langevin step clears a consumed v_cm itself)
             clear_cm_kernel<T><<<1, 1, 0, stream_>>>(cm);
             launches_++;
         }
@@ -1770,6 +1783,11 @@ class Engine : public EngineBase {
         const int vvb2 = std::max(1, std::min((n_ownb + 2 * VV_THREADS - 1) / (2 * VV_THREADS), 8 * sm_count_));
         MB_TRY(launch_pairs(false, d_f4_.as<T4>(), dec));
         MB_TRY(launch_bonded(false));
+        if (c.langevin) {  // these forces are the next step's kick: the step ends here
+            if (o.log_mask) MB_TRY(enqueue_log(c, o.log_mask));
+            MB_CUDA(cudaGetLastError());
+            return MB_OK;
+        }
         const bool p2p_sig = dec && p2p_active();  // (after a rebuild: the new ownership's peers)
         PeerSignal sig;
         memset(&sig, 0, sizeof(sig));
@@ -1823,7 +1841,7 @@ class Engine : public EngineBase {
         return MB_OK;
     }
     // single-GPU step loop: the thermostat of step n runs at the top of step n+1's drift kernel; the last step of a call is
-    // closed by the standalone kernel (simulate_vv)
+    // closed by the standalone kernel (simulate)
     Thermo<T> thermo_in_k1(const StepCfg& c) const {
         Thermo<T> th;
         memset(&th, 0, sizeof(th));
@@ -1845,10 +1863,13 @@ class Engine : public EngineBase {
         double dt, kT, prob;
         int64_t n;
         mb_vcoupling_t vc;  // the velocity-rescaling thermostat's kind and parameters (baked into K2's arguments)
+        int langevin;       // the integrator, and Langevin's kT and friction (baked into its step kernel's arguments)
+        double langevin_kT, friction;
         bool operator==(const GraphKey& o) const {
             return path == o.path && do_cm == o.do_cm && thermostat == o.thermostat && geom_version == o.geom_version &&
                    rebuild_every == o.rebuild_every && log_mask == o.log_mask && dt == o.dt && kT == o.kT && prob == o.prob && n == o.n &&
-                   vc.kind == o.vc.kind && vc.n_steps == o.vc.n_steps && vc.kT == o.vc.kT && vc.tau == o.vc.tau;
+                   vc.kind == o.vc.kind && vc.n_steps == o.vc.n_steps && vc.kT == o.vc.kT && vc.tau == o.vc.tau &&
+                   langevin == o.langevin && langevin_kT == o.langevin_kT && friction == o.friction;
         }
     };
     // one executable step graph per log mask; the host loop picks one per step
@@ -1869,7 +1890,8 @@ class Engine : public EngineBase {
         for (int m = 0; m < 8; m++) destroy_graph(m);
         destroy_sd_graph();
     }
-    // Capture one MD step (K1, decide, [IF rebuild], force, K2, [thermostat], [log records]) into an executable graph.
+    // Capture one MD step (K1, [IF rebuild], force, K2, [thermostat], [log records]; Langevin: L, [IF rebuild], force,
+    // [log records]) into an executable graph.
     int build_step_graph(const StepCfg& c, const GraphKey& key) {
         const int mask = key.log_mask;
         destroy_graph(mask);
@@ -1936,7 +1958,7 @@ class Engine : public EngineBase {
         return m;
     }
 
-    // The device-side loggers of one simulate_vv call. Device outputs are written in place; host outputs go through device
+    // The device-side loggers of one simulate call. Device outputs are written in place; host outputs go through device
     // staging: all energy records, copied at the end, and a bounded ring of frames per kind, copied out whenever it is full.
     struct LogRun {
         mb_log_t* log = nullptr;
@@ -2006,17 +2028,26 @@ class Engine : public EngineBase {
             const int64_t rest = lr.ring[k] > 0 ? lr.framed[k] % lr.ring[k] : 0;
             if (rest > 0) MB_TRY(copy_back(lr.out[k + 1], (size_t)rest * lr.frame_bytes, (size_t)(lr.framed[k] - rest) * lr.frame_bytes));
         }
-        // (after MB_ERR_CAPACITY in simulate_vv these records are as invalid as the coordinates)
+        // (after MB_ERR_CAPACITY in simulate these records are as invalid as the coordinates)
         lr.log->n_energies = lr.n[0];
         lr.log->n_coords = lr.framed[0];
         lr.log->n_vels = lr.framed[1];
         return MB_OK;
     }
 
-    int simulate_vv(void* coords, void* vels, const mb_vv_params_t* p, mb_log_t* log) override {
+    // mb_simulate_vv, mb_simulate_vv_log and mb_simulate_langevin: one body, one step loop, one graph builder
+    int simulate(void* coords, void* vels, const mb_vv_params_t* p, const mb_langevin_params_t* lg, mb_log_t* log) override {
         MB_TRY(prepare());
         if (!coords || !vels || !p) return set_error(MB_ERR_INVALID, "null argument");
         if (p->n_steps < 0 || !(p->dt > 0)) return set_error(MB_ERR_INVALID, "n_steps < 0 or dt <= 0");
+        if (lg) {
+            if (!(std::isfinite(lg->kT) && lg->kT >= 0)) return set_error(MB_ERR_INVALID, "mb_simulate_langevin: kT must be finite and >= 0");
+            if (!(std::isfinite(lg->friction) && lg->friction >= 0))
+                return set_error(MB_ERR_INVALID, "mb_simulate_langevin: friction must be finite and >= 0");
+            if (vcoupling.kind != MB_VC_NONE)
+                return set_error(MB_ERR_INVALID, "mb_simulate_langevin: a velocity coupling is set on the context (couplings with Langevin are not supported)");
+            if (decomposed()) return set_error(MB_ERR_INVALID, "mb_simulate_langevin: not available in decomposed (multi-GPU) runs");
+        }
         if (vcoupling.kind != MB_VC_NONE) {
             if (p->andersen_kT > 0 && p->andersen_prob > 0)
                 return set_error(MB_ERR_INVALID, "mb_simulate_vv: at most one thermostat per call (Andersen and a velocity-rescaling thermostat)");
@@ -2043,6 +2074,13 @@ class Engine : public EngineBase {
         c.prob = p->andersen_prob;
         c.do_cm = (p->remove_cm_every == 0) ? 0 : (p->remove_cm_every == 1 ? 1 : -1);
         c.vc = VCouple{vcoupling.kind, vcoupling.n_steps, 3 * (long long)n_ - 3, vcoupling.kT, p->dt, vcoupling.tau, total_mass_};
+        c.langevin = lg != nullptr;
+        c.lc = LangevinCoef{1.0, 0.0, 0.0};
+        if (lg) {  // Langevin(dt, temperature, friction): vel_scale, noise_scale (src/simulators.jl:1092-1097), in double
+            c.lc.vel_scale = exp(-p->dt * lg->friction);
+            c.lc.noise_scale = sqrt(1.0 - c.lc.vel_scale * c.lc.vel_scale);
+            c.lc.kT = lg->kT;
+        }
         if (path_ == 0) {
             init_slots(xb.as<T>());
             // velocities + wrap through ingest with an identity order (geometry only needs L)
@@ -2118,7 +2156,8 @@ class Engine : public EngineBase {
             for (int64_t k = 1; k <= p->n_steps; k++) need[log_mask_at(log, p->init_step + k)] = true;
             for (int m = 0; m < 8 && use_graph; m++) {
                 if (!need[m]) continue;
-                GraphKey key{path_, c.do_cm, c.thermostat ? 1 : 0, geom_version_, rebuild_every_, m, p->dt, p->andersen_kT, p->andersen_prob, n_, vcoupling};
+                GraphKey key{path_, c.do_cm, c.thermostat ? 1 : 0, geom_version_, rebuild_every_, m, p->dt, p->andersen_kT, p->andersen_prob, n_, vcoupling,
+                             c.langevin ? 1 : 0, lg ? lg->kT : 0.0, lg ? lg->friction : 0.0};
                 if (!graphs_[m].exec || !(key == graphs_[m].key)) {
                     if (build_step_graph(c, key) != MB_OK) {
                         graph_failed_ = true;  // stay on the stream path for this context
@@ -2153,7 +2192,7 @@ class Engine : public EngineBase {
                 }
                 StepOpts o;
                 o.do_cm = do_cm;
-                o.clear_cm_after_k1 = clear_after_k1;
+                o.clear_cm_after_k1 = clear_after_k1 && !c.langevin;
                 o.rebuild_hint = hint;
                 o.defer_cm = k < p->n_steps;
                 o.log_mask = log_mask_at(log, step_n);
@@ -2339,7 +2378,7 @@ class Engine : public EngineBase {
         const bool use_graph = graph_enabled_ && !graph_failed_ && !prof_.enabled && !pme_on_ && p->max_steps > 0;
         graph_used_ = false;
         if (use_graph) {
-            const GraphKey key{path_, 0, 0, geom_version_, 0, -1, 0.0, 0.0, 0.0, n_, {MB_VC_NONE, 0, 0.0, 0.0}};
+            const GraphKey key{path_, 0, 0, geom_version_, 0, -1, 0.0, 0.0, 0.0, n_, {MB_VC_NONE, 0, 0.0, 0.0}, 0, 0.0, 0.0};
             if (!sd_graph_.exec || !(key == sd_graph_.key)) {
                 if (build_sd_graph(key) != MB_OK) graph_failed_ = true;  // stay on the stream path for this context
             }
@@ -2683,10 +2722,16 @@ int mb_random_velocities(mb_ctx* ctx, void* vels, double kT, uint64_t rng_ctr1, 
     return ctx->e->random_velocities(vels, kT, rng_ctr1, rng_key);
 }
 int mb_kinetic_energy_tensor(mb_ctx* ctx, const void* vels, double* ke_tensor9_host) { MB_CTX_GUARD(ctx); return ctx->e->kinetic_tensor(vels, ke_tensor9_host); }
-int mb_simulate_vv(mb_ctx* ctx, void* coords, void* vels, const mb_vv_params_t* p) { MB_CTX_GUARD(ctx); return ctx->e->simulate_vv(coords, vels, p, nullptr); }
+int mb_simulate_vv(mb_ctx* ctx, void* coords, void* vels, const mb_vv_params_t* p) { MB_CTX_GUARD(ctx); return ctx->e->simulate(coords, vels, p, nullptr, nullptr); }
 int mb_simulate_vv_log(mb_ctx* ctx, void* coords, void* vels, const mb_vv_params_t* p, mb_log_t* log) {
     MB_CTX_GUARD(ctx);
-    return ctx->e->simulate_vv(coords, vels, p, log);
+    return ctx->e->simulate(coords, vels, p, nullptr, log);
+}
+int mb_simulate_langevin(mb_ctx* ctx, void* coords, void* vels, const mb_langevin_params_t* p, mb_log_t* log) {
+    MB_CTX_GUARD(ctx);
+    if (!p) return mb::set_error(MB_ERR_INVALID, "null argument");
+    const mb_vv_params_t vp = {p->dt, p->n_steps, p->init_step, p->remove_cm_every, 0.0, 0.0, p->rng_ctr1, p->rng_key};
+    return ctx->e->simulate(coords, vels, &vp, p, log);
 }
 int mb_minimize_sd(mb_ctx* ctx, void* coords, mb_sd_params_t* p) { MB_CTX_GUARD(ctx); return ctx->e->minimize_sd(coords, p); }
 int mb_set_velocity_coupling(mb_ctx* ctx, const mb_vcoupling_t* c) {

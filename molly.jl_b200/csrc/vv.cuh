@@ -184,9 +184,19 @@ __device__ __forceinline__ void andersen_apply(typename VT<T>::T4& v, int orig_i
     }
 }
 
-// ---- K1: first half kick + drift + displacement check; the last CTA to finish does the step bookkeeping:
-// advance step_n, apply the fixed-interval neighbour policy (find_neighbors every n_steps, src/neighbors.jl:671) and
-// publish the rebuild decision to the CUDA graph's conditional node (when the step runs as a graph).
+// The step bookkeeping of a drift pass (K1, the Langevin step), done by one thread of the last CTA to finish: advance step_n,
+// apply the fixed-interval neighbour policy (find_neighbors every n_steps, src/neighbors.jl:671) and publish the rebuild
+// decision to the CUDA graph's conditional node (when the step runs as a graph).
+__device__ __forceinline__ void step_advance(Control* __restrict__ ctl, cudaGraphConditionalHandle handle, int use_handle) {
+    __threadfence();
+    const long long step_n = ++ctl->step;
+    const long long kk = step_n - ctl->init_step;
+    int rb = *(volatile int*)&ctl->rebuild;
+    if (ctl->rebuild_every > 0 && kk > 1 && (step_n - 1) % ctl->rebuild_every == 0) { rb = 1; ctl->rebuild = 1; }
+    if (use_handle) cudaGraphSetConditional(handle, rb ? 1u : 0u);
+}
+
+// ---- K1: first half kick + drift + displacement check; the last CTA to finish does the step bookkeeping (step_advance).
 // THERMO: the variants that also apply the previous step's thermostat are separate instantiations so that the plain kernel
 // keeps its register count (one atom per thread, latency-bound: occupancy matters): TH_ANDERSEN resamples (Philox +
 // Box-Muller inlined), TH_SCALE applies the pending velocity-rescaling factor after the pending v_cm.
@@ -301,12 +311,7 @@ __global__ void vv_kick_drift_kernel(int s0, int n, T dt, T dt_half, T skin_half
     }
     __syncthreads();
     if (s_last && threadIdx.x == 0) {
-        __threadfence();
-        const long long step_n = ++ctl->step;
-        const long long kk = step_n - ctl->init_step;
-        int rb = *(volatile int*)&ctl->rebuild;
-        if (ctl->rebuild_every > 0 && kk > 1 && (step_n - 1) % ctl->rebuild_every == 0) { rb = 1; ctl->rebuild = 1; }
-        if (use_handle) cudaGraphSetConditional(handle, rb ? 1u : 0u);
+        step_advance(ctl, handle, use_handle);
         if (push.n_peer > 0) {  // every CTA's peer stores are ordered before its ticket: publish the epoch
             __threadfence_system();
             for (int q = 0; q < push.n_peer; q++) st_release_sys(push.signal_flag[q], push.epoch);
