@@ -284,6 +284,38 @@ typedef struct {
 } mb_langevin_params_t;
 int mb_simulate_langevin(mb_ctx* ctx, void* coords, void* vels, const mb_langevin_params_t* p, mb_log_t* log);
 
+/* simulate!(sys, NoseHoover(dt, temperature, damping; remove_CM_motion), n_steps) (src/simulators.jl:1491-1614; Evans and
+ * Holian 1985). Q = damping, T0 = kT / k, T(v) = sum m|v|^2 / (Nf k) with Nf = 3N - 3 (the df of `temperature`). Prologue
+ * as mb_simulate_vv: wrap, CM removal when init_step == 0 and remove_cm_every != 0, neighbours, F0, loggers at init_step,
+ * and zeta = 0 at the start of every call (the reference keeps zeta as a local of simulate!, so two chunked calls differ
+ * from one long call). Step n, with a = F/m:
+ *   1. v_half = v + (a - v zeta) dt/2
+ *   2. x += v_half dt; wrap
+ *   3. zeta_half = zeta + dt / (2 Q^2) (T(v) / T0 - 1), with the full-step velocities v before step 1
+ *   4. zeta = zeta_half + dt / (2 Q^2) (T(v_half) / T0 - 1)
+ *   5. neighbours; F = forces(x)
+ *   6. v = (v_half + a dt/2) / (1 + zeta dt/2)
+ *   7. CM removal when n % remove_cm_every == 0; loggers (mb_log_t, as for mb_simulate_vv_log; NULL: no logging).
+ * zeta and both kinetic sums are double (sums per CTA, added in index order); the per-atom arithmetic is in the context's
+ * dtype, in the reference's order of operations, with zeta rounded to it. One step is two kernels around the force
+ * evaluation. Where the engine differs from the reference:
+ *  - the neighbour rebuild is triggered by the exact displacement test (as for mb_simulate_vv), not by the finder's
+ *    fixed interval alone;
+ *  - a = F (1/m) with the context's 1/m (massless atoms: no kick; they still feel the friction term).
+ * MB_ERR_INVALID before any work for dt <= 0, n_steps < 0, kT not finite or <= 0 (T0 = 0 makes T / T0 infinite), damping
+ * not finite or <= 0, fewer than 2 atoms (Nf <= 0), a velocity coupling set on the context (mb_set_velocity_coupling;
+ * couplings with NoseHoover take the stock path), a decomposed (multi-GPU) context, and the logging errors of
+ * mb_simulate_vv_log. MB_ERR_CAPACITY as in mb_simulate_vv. */
+typedef struct {
+    double dt;
+    int64_t n_steps;
+    int64_t init_step;
+    int32_t remove_cm_every;  /* NoseHoover.remove_CM_motion (default 1; 0 = never) */
+    double kT;                /* k * temperature in kJ/mol */
+    double damping;           /* ps (reference default 100 dt) */
+} mb_nosehoover_params_t;
+int mb_simulate_nose_hoover(mb_ctx* ctx, void* coords, void* vels, const mb_nosehoover_params_t* p, mb_log_t* log);
+
 /* simulate!(sys, SteepestDescentMinimizer(step_size, max_steps, tol)) (src/simulators.jl:183-274) on the device: wrap the
  * coordinates, E = potential energy; then for step n = init_step+1 .. init_step+max_steps: F = forces, m = max |F_i|,
  * x <- wrap(x + h F / m), E_trial = potential energy; E_trial < E accepts (h <- 6h/5, E <- E_trial), otherwise x is restored

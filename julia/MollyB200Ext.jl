@@ -10,6 +10,7 @@
 #   Molly.simulate!(sys, sim::VelocityVerlet, n_steps; ...)                                                 simulators.jl:547
 #   Molly.simulate!(sys, sim::SteepestDescentMinimizer; ...)                                                simulators.jl:183
 #   Molly.simulate!(sys, sim::Langevin, n_steps; ...) with coupling === nothing                              simulators.jl:1101
+#   Molly.simulate!(sys, sim::NoseHoover, n_steps; ...) with coupling === nothing                            simulators.jl:1534
 # (Molly.remove_CM_motion! for CuArray Systems is NOT redefined: the stock extension owns that exact signature)
 # and falls through to the stock methods (invoke) for anything it does not recognise: non-cubic boundaries,
 # constraints, virtual sites, couplings other than one AndersenThermostat, ImmediateThermostat, BerendsenThermostat or
@@ -63,6 +64,16 @@ struct MBLangevinParams
     friction::Float64
     rng_ctr1::UInt64
     rng_key::UInt64
+end
+
+# mb_nosehoover_params_t (mb_simulate_nose_hoover)
+struct MBNoseHooverParams
+    dt::Float64
+    n_steps::Int64
+    init_step::Int64
+    remove_cm_every::Int32
+    kT::Float64
+    damping::Float64
 end
 
 # mb_vcoupling_t (mb_set_velocity_coupling)
@@ -395,6 +406,38 @@ function Molly.simulate!(sys::System{3, <:CuArray, T}, sim::Langevin, n_steps::I
         end
     end
     check(ccall((:mb_simulate_langevin, LIB), Cint, (Ptr{Cvoid}, CuPtr{Cvoid}, CuPtr{Cvoid}, Ref{MBLangevinParams}, Ptr{MBLog}),
+                ctx.handle, pointer(sys.coords), pointer(sys.velocities), Ref(p), C_NULL))
+    return sys
+end
+
+# ---- simulate!(sys, ::NoseHoover, n) (src/simulators.jl:1534-1614) ---------------------------------------------------------
+# Taken over under the conditions of the Langevin method above: one mb_simulate_nose_hoover call, which starts zeta at 0 as
+# the stock method does on every call. Units are stripped (dt and damping in ps, k T in kJ/mol). Anything else runs the stock
+# method.
+function Molly.simulate!(sys::System{3, <:CuArray, T}, sim::NoseHoover, n_steps::Integer;
+                         init_step=0, rng=Random.default_rng(), run_loggers=true, kwargs...) where T
+    descs = engine_eligible(sys, sys.pairwise_inters)
+    device_logs = run_loggers == false || isempty(sys.loggers) ||
+                  all(l -> !isnothing(device_log_kind(l)), values(sys.loggers))
+    if isnothing(descs) || !isnothing(sim.coupling) || !device_logs ||
+            !all(gi -> gi isa Molly.LJDispersionCorrection, sys.general_inters) ||
+            !all(!isnothing, map(specific_desc, sys.specific_inter_lists))
+        # stock: simulate!(sys, sim::NoseHoover, n_steps_or_time; ...) src/simulators.jl:1534
+        return invoke(Molly.simulate!, Tuple{Any, NoseHoover, Any}, sys, sim, n_steps;
+                      init_step=init_step, rng=rng, run_loggers=run_loggers, kwargs...)
+    end
+    ctx = context_for(sys, descs)
+    set_specific!(ctx, sys)
+    set_velocity_coupling!(ctx, nothing)
+    p = MBNoseHooverParams(_ps(sim.dt), n_steps, init_step, Int32(sim.remove_CM_motion),
+                           Float64(ustrip(sys.k * sim.temperature)), _ps(sim.damping))
+    if run_loggers != false && !isempty(sys.loggers)
+        return simulate_logged!(sys, ctx, n_steps, init_step, run_loggers) do lg
+            ccall((:mb_simulate_nose_hoover, LIB), Cint, (Ptr{Cvoid}, CuPtr{Cvoid}, CuPtr{Cvoid}, Ref{MBNoseHooverParams}, Ref{MBLog}),
+                  ctx.handle, pointer(sys.coords), pointer(sys.velocities), Ref(p), lg)
+        end
+    end
+    check(ccall((:mb_simulate_nose_hoover, LIB), Cint, (Ptr{Cvoid}, CuPtr{Cvoid}, CuPtr{Cvoid}, Ref{MBNoseHooverParams}, Ptr{MBLog}),
                 ctx.handle, pointer(sys.coords), pointer(sys.velocities), Ref(p), C_NULL))
     return sys
 end

@@ -13,6 +13,7 @@ julia/MollyB200Ext.jl, see INTEGRATION.md):
     VelocityRescaleThermostat                       simulate, see mb_set_velocity_coupling)
     SteepestDescentMinimizer                        src/simulators.jl:183-274 (simulate dispatches on the simulator)
     Langevin                                        src/simulators.jl:1065-1210 (mb_simulate_langevin)
+    NoseHoover                                      src/simulators.jl:1491-1614 (mb_simulate_nose_hoover)
     forces, forces_virial, potential_energy         src/force.jl:678-720, src/energy.jl:202-248
     kinetic_energy, temperature, remove_CM_motion   src/energy.jl:44-175, src/spatial.jl:901-929
     *EnergyLogger, TemperatureLogger, Coordinates-  src/loggers.jl:44-102, :134-278 (recorded on the device inside
@@ -433,6 +434,33 @@ class Langevin:
 
 
 @dataclass
+class NoseHoover:
+    """NoseHoover(dt, temperature, damping=100 dt; coupling=None, remove_CM_motion=1) — src/simulators.jl:1491-1614, the
+    Nose-Hoover thermostat of Evans and Holian 1985, run on the device by mb_simulate_nose_hoover (see include/mollyb200.h
+    for the step and where the engine differs from the reference). dt in ps, temperature in K (> 0: the step divides by
+    it), damping in ps. The thermostat variable zeta starts at 0 in every call, as in the reference. A coupling is not run
+    by the engine: simulate refuses it."""
+    dt: float
+    temperature: float
+    damping: Optional[float] = None
+    coupling: object = None
+    remove_CM_motion: int = 1
+
+    def __post_init__(self):
+        if not (math.isfinite(self.dt) and self.dt > 0):
+            raise ValueError(f"dt must be finite and positive, found {self.dt}")
+        if not (math.isfinite(self.temperature) and self.temperature > 0):
+            raise ValueError(f"temperature must be finite and positive, found {self.temperature}")
+        if self.damping is None:
+            self.damping = 100 * self.dt  # the reference's default
+        if not (math.isfinite(self.damping) and self.damping > 0):
+            raise ValueError(f"damping must be finite and positive, found {self.damping}")
+        self.remove_CM_motion = int(self.remove_CM_motion)  # Int(remove_CM_motion): false -> 0
+        if self.remove_CM_motion < 0:
+            raise ValueError(f"remove_CM_motion must be non-negative, found {self.remove_CM_motion}")
+
+
+@dataclass
 class SteepestDescentMinimizer:
     """SteepestDescentMinimizer(step_size, max_steps, tol, log_stream) — src/simulators.jl:183-274, run on the device by
     mb_minimize_sd (see include/mollyb200.h for where the engine may differ from the reference). step_size in nm, tol in
@@ -836,6 +864,8 @@ def simulate(sys: System, sim, n_steps: Optional[int] = None, init_step: int = 0
     velocities and appends to the histories of sys.loggers (recorded on the device, see _LogPlan).
     Langevin: simulate!(sys, sim, n_steps; run_loggers=true) — src/simulators.jl:1101-1210, the same arguments and loggers
     as VelocityVerlet; the velocities are half a step behind the positions.
+    NoseHoover: simulate!(sys, sim, n_steps; run_loggers=true) — src/simulators.jl:1534-1614, the same arguments and loggers
+    as VelocityVerlet; zeta starts at 0 in every call.
     SteepestDescentMinimizer: simulate!(sys, sim; run_loggers=false) — src/simulators.jl:183-274, see steepest_descent.
     Loggers are not run during a minimisation (run_loggers must be false)."""
     if isinstance(sim, SteepestDescentMinimizer):
@@ -845,7 +875,7 @@ def simulate(sys: System, sim, n_steps: Optional[int] = None, init_step: int = 0
             raise NotImplementedError("loggers are not run during a minimisation on the device (run_loggers must be false)")
         steepest_descent(sys, sim, init_step=init_step, max_retries=max_retries)
         return sys
-    if not isinstance(sim, (VelocityVerlet, Langevin)):
+    if not isinstance(sim, (VelocityVerlet, Langevin, NoseHoover)):
         raise TypeError(f"unsupported simulator {type(sim).__name__}")
     if n_steps is None:
         raise TypeError(f"simulate(sys, ::{type(sim).__name__}, n_steps) needs n_steps")
@@ -860,6 +890,12 @@ def simulate(sys: System, sim, n_steps: Optional[int] = None, init_step: int = 0
         p = capi.MBLangevinParams()
         p.kT = sys.k * sim.temperature
         p.friction = float(sim.friction)
+    elif isinstance(sim, NoseHoover):
+        if couplings:
+            raise TypeError(f"unsupported coupling {couplings[0]!r} with NoseHoover (the stock Molly path handles it)")
+        p = capi.MBNoseHooverParams()
+        p.kT = sys.k * sim.temperature
+        p.damping = float(sim.damping)
     else:
         p = capi.MBVVParams()
         p.andersen_kT = 0.0
@@ -877,10 +913,11 @@ def simulate(sys: System, sim, n_steps: Optional[int] = None, init_step: int = 0
     p.init_step = int(init_step)
     p.remove_cm_every = int(sim.remove_CM_motion)
     ctx = sys.engine()
-    capi.check(sys._L.mb_set_velocity_coupling(ctx, C.byref(vc) if vc is not None else None))  # (Langevin: cleared)
-    rng = rng or np.random.default_rng()
-    p.rng_ctr1 = int(rng.integers(0, 2 ** 63))
-    p.rng_key = int(rng.integers(0, 2 ** 63))
+    capi.check(sys._L.mb_set_velocity_coupling(ctx, C.byref(vc) if vc is not None else None))  # (Langevin, NoseHoover: cleared)
+    if not isinstance(sim, NoseHoover):  # (NoseHoover draws nothing)
+        rng = rng or np.random.default_rng()
+        p.rng_ctr1 = int(rng.integers(0, 2 ** 63))
+        p.rng_key = int(rng.integers(0, 2 ** 63))
     host = not hasattr(sys.coords, "data_ptr")
     backup = (sys.coords.copy(), sys.velocities.copy()) if host else None
     plan = _LogPlan(sys, int(n_steps), int(init_step), run_loggers) if sys.loggers and run_loggers is not False else None
@@ -889,6 +926,9 @@ def simulate(sys: System, sim, n_steps: Optional[int] = None, init_step: int = 0
         if isinstance(sim, Langevin):
             rc = sys._L.mb_simulate_langevin(ctx, _ptr(sys.coords), _ptr(sys.velocities), C.byref(p),
                                              C.byref(plan.desc) if plan is not None else None)
+        elif isinstance(sim, NoseHoover):
+            rc = sys._L.mb_simulate_nose_hoover(ctx, _ptr(sys.coords), _ptr(sys.velocities), C.byref(p),
+                                                C.byref(plan.desc) if plan is not None else None)
         elif plan is None:
             rc = sys._L.mb_simulate_vv(ctx, _ptr(sys.coords), _ptr(sys.velocities), C.byref(p))
         else:  # a retry overwrites the records of the failed attempt

@@ -14,6 +14,7 @@
 #include "force.cuh"
 #include "langevin.cuh"
 #include "minimize.cuh"
+#include "nosehoover.cuh"
 #include "pair.cuh"
 #include "pme.cuh"
 #include "vv.cuh"
@@ -322,8 +323,10 @@ class EngineBase {
                                const int32_t* sj) = 0;
     virtual int set_neighbor_policy(double r_list, int rebuild_every) = 0;
     virtual int forces_energy(const void* coords, void* fs, void* pe, void* vir, int64_t step_n, bool with_specific) = 0;
-    // lg: the Langevin integrator's parameters, NULL for VelocityVerlet (p then carries the fields both share)
-    virtual int simulate(void* coords, void* vels, const mb_vv_params_t* p, const mb_langevin_params_t* lg, mb_log_t* log) = 0;
+    // lg, nh: the Langevin or Nose-Hoover integrator's parameters (at most one), both NULL for VelocityVerlet (p then carries
+    // the fields all three share)
+    virtual int simulate(void* coords, void* vels, const mb_vv_params_t* p, const mb_langevin_params_t* lg,
+                         const mb_nosehoover_params_t* nh, mb_log_t* log) = 0;
     virtual int remove_cm(void* vels) = 0;
     virtual int kinetic_energy(const void* vels, double* out) = 0;
     virtual int rebuild(const void* coords) = 0;
@@ -672,6 +675,7 @@ class Engine : public EngineBase {
         MB_CUDA(cudaMemsetAsync(d_ctl_.p, 0, sizeof(Control), stream_));
         MB_CUDA(d_cm_.ensure(sizeof(CmState<T>)));
         MB_CUDA(cudaMemsetAsync(d_cm_.p, 0, sizeof(CmState<T>), stream_));
+        MB_CUDA(d_nh_.ensure(sizeof(NhState)));
         MB_CUDA(d_stage_a_.ensure(3 * np * sizeof(T)));
         MB_CUDA(d_stage_b_.ensure(3 * np * sizeof(T)));
         MB_CUDA(d_stage_c_.ensure(3 * np * sizeof(T)));
@@ -1687,9 +1691,11 @@ class Engine : public EngineBase {
         bool thermostat;
         int* flag_ptr;
         VCouple vc;       // velocity-rescaling thermostat (kind VC_NONE: none)
-        bool langevin;    // the integrator: Langevin (langevin.cuh) or VelocityVerlet
+        int integrator;   // INTEG_*: VelocityVerlet (vv.cuh), Langevin (langevin.cuh) or Nose-Hoover (nosehoover.cuh)
         LangevinCoef lc;  // Langevin's c, sqrt(1 - c^2) and kT
+        NhCoef nc;        // Nose-Hoover's dt / (2 Q^2) and Nf k T0
     };
+    enum { INTEG_VV = 0, INTEG_LANGEVIN = 1, INTEG_NH = 2 };
     // what one step does beyond the plain VelocityVerlet step
     struct StepOpts {
         int do_cm = 0;                   // remove_CM_motion after this step's kick
@@ -1720,12 +1726,19 @@ class Engine : public EngineBase {
             cm_deferred_epoch_ = 0;
         }
         prof_.begin(Prof::VV);
-        if (c.langevin) {
+        if (c.integrator == INTEG_LANGEVIN) {
             // (single GPU: s0 = 0.) At most vvb CTAs, so d_partial_ (max(vvb, 2048) x 8 doubles, prepare) holds their 3 each
             const int lgb = std::max(1, std::min(nb, 8 * sm_count_));
             langevin_step_kernel<T><<<lgb, VV_THREADS, 0, stream_>>>(
                 n_own, c.dt, c.dt_half, c.skin_half2, c.lc, o.do_cm, c.inv_mass, cm, d_f4_.as<T4>(), d_xref4_.as<T4>(),
                 d_pos4_.as<T4>(), d_vel4_.as<T4>(), d_orig_.as<int>(), d_mass_.as<T>(), d_partial_.as<double>(), c.flag_ptr, ctl,
+                cap ? cap->handle : 0, cap && path_ == 1 ? 1 : 0, ext_map());
+        } else if (c.integrator == INTEG_NH) {
+            // (single GPU: s0 = 0.) At most vvb CTAs, so d_partial_ holds their 2 each
+            const int nhb = std::max(1, std::min(nb, 8 * sm_count_));
+            nh_kick_drift_kernel<T><<<nhb, VV_THREADS, 0, stream_>>>(
+                n_own, c.dt, c.dt_half, c.skin_half2, c.nc, d_nh_.as<NhState>(), cm, d_f4_.as<T4>(), d_xref4_.as<T4>(),
+                d_pos4_.as<T4>(), d_vel4_.as<T4>(), d_mass_.as<T>(), d_partial_.as<double>(), c.flag_ptr, ctl,
                 cap ? cap->handle : 0, cap && path_ == 1 ? 1 : 0, ext_map());
         } else {
             const Thermo<T> th = thermo_in_k1(c);
@@ -1739,7 +1752,7 @@ class Engine : public EngineBase {
         }
         prof_.end(Prof::VV);
         launches_++;
-        if (o.clear_cm_after_k1) {  // (VelocityVerlet: the Langevin step clears a consumed v_cm itself)
+        if (o.clear_cm_after_k1) {  // (VelocityVerlet: the Langevin step and NH2 clear a consumed v_cm themselves)
             clear_cm_kernel<T><<<1, 1, 0, stream_>>>(cm);
             launches_++;
         }
@@ -1783,7 +1796,19 @@ class Engine : public EngineBase {
         const int vvb2 = std::max(1, std::min((n_ownb + 2 * VV_THREADS - 1) / (2 * VV_THREADS), 8 * sm_count_));
         MB_TRY(launch_pairs(false, d_f4_.as<T4>(), dec));
         MB_TRY(launch_bonded(false));
-        if (c.langevin) {  // these forces are the next step's kick: the step ends here
+        if (c.integrator == INTEG_LANGEVIN) {  // these forces are the next step's kick: the step ends here
+            if (o.log_mask) MB_TRY(enqueue_log(c, o.log_mask));
+            MB_CUDA(cudaGetLastError());
+            return MB_OK;
+        }
+        if (c.integrator == INTEG_NH) {
+            const int nhb2 = std::max(1, std::min(nb2, 8 * sm_count_));
+            prof_.begin(Prof::VV);
+            nh_kick2_kernel<T><<<nhb2, VV_THREADS, 0, stream_>>>(n_ownb, c.dt_half, o.do_cm, c.inv_mass, d_nh_.as<NhState>(),
+                                                                 d_f4_.as<T4>(), d_mass_.as<T>(), d_vel4_.as<T4>(),
+                                                                 d_partial_.as<double>(), ctl, cm);
+            prof_.end(Prof::VV);
+            launches_++;
             if (o.log_mask) MB_TRY(enqueue_log(c, o.log_mask));
             MB_CUDA(cudaGetLastError());
             return MB_OK;
@@ -1863,13 +1888,13 @@ class Engine : public EngineBase {
         double dt, kT, prob;
         int64_t n;
         mb_vcoupling_t vc;  // the velocity-rescaling thermostat's kind and parameters (baked into K2's arguments)
-        int langevin;       // the integrator, and Langevin's kT and friction (baked into its step kernel's arguments)
-        double langevin_kT, friction;
+        int integrator;     // INTEG_*, and Langevin's kT and friction or Nose-Hoover's kT and damping (baked into the
+        double integ_kT, friction, damping;  // step kernels' arguments)
         bool operator==(const GraphKey& o) const {
             return path == o.path && do_cm == o.do_cm && thermostat == o.thermostat && geom_version == o.geom_version &&
                    rebuild_every == o.rebuild_every && log_mask == o.log_mask && dt == o.dt && kT == o.kT && prob == o.prob && n == o.n &&
                    vc.kind == o.vc.kind && vc.n_steps == o.vc.n_steps && vc.kT == o.vc.kT && vc.tau == o.vc.tau &&
-                   langevin == o.langevin && langevin_kT == o.langevin_kT && friction == o.friction;
+                   integrator == o.integrator && integ_kT == o.integ_kT && friction == o.friction && damping == o.damping;
         }
     };
     // one executable step graph per log mask; the host loop picks one per step
@@ -1891,7 +1916,7 @@ class Engine : public EngineBase {
         destroy_sd_graph();
     }
     // Capture one MD step (K1, [IF rebuild], force, K2, [thermostat], [log records]; Langevin: L, [IF rebuild], force,
-    // [log records]) into an executable graph.
+    // [log records]; Nose-Hoover: NH1, [IF rebuild], force, NH2, [log records]) into an executable graph.
     int build_step_graph(const StepCfg& c, const GraphKey& key) {
         const int mask = key.log_mask;
         destroy_graph(mask);
@@ -2035,8 +2060,10 @@ class Engine : public EngineBase {
         return MB_OK;
     }
 
-    // mb_simulate_vv, mb_simulate_vv_log and mb_simulate_langevin: one body, one step loop, one graph builder
-    int simulate(void* coords, void* vels, const mb_vv_params_t* p, const mb_langevin_params_t* lg, mb_log_t* log) override {
+    // mb_simulate_vv, mb_simulate_vv_log, mb_simulate_langevin and mb_simulate_nose_hoover: one body, one step loop, one
+    // graph builder
+    int simulate(void* coords, void* vels, const mb_vv_params_t* p, const mb_langevin_params_t* lg, const mb_nosehoover_params_t* nh,
+                 mb_log_t* log) override {
         MB_TRY(prepare());
         if (!coords || !vels || !p) return set_error(MB_ERR_INVALID, "null argument");
         if (p->n_steps < 0 || !(p->dt > 0)) return set_error(MB_ERR_INVALID, "n_steps < 0 or dt <= 0");
@@ -2047,6 +2074,16 @@ class Engine : public EngineBase {
             if (vcoupling.kind != MB_VC_NONE)
                 return set_error(MB_ERR_INVALID, "mb_simulate_langevin: a velocity coupling is set on the context (couplings with Langevin are not supported)");
             if (decomposed()) return set_error(MB_ERR_INVALID, "mb_simulate_langevin: not available in decomposed (multi-GPU) runs");
+        }
+        if (nh) {
+            // (kT = 0 would make T / T0 infinite)
+            if (!(std::isfinite(nh->kT) && nh->kT > 0)) return set_error(MB_ERR_INVALID, "mb_simulate_nose_hoover: kT must be finite and > 0");
+            if (!(std::isfinite(nh->damping) && nh->damping > 0))
+                return set_error(MB_ERR_INVALID, "mb_simulate_nose_hoover: damping must be finite and > 0");
+            if (n_ < 2) return set_error(MB_ERR_INVALID, "mb_simulate_nose_hoover: needs at least 2 atoms (Nf = 3N - 3 > 0)");
+            if (vcoupling.kind != MB_VC_NONE)
+                return set_error(MB_ERR_INVALID, "mb_simulate_nose_hoover: a velocity coupling is set on the context (couplings with Nose-Hoover are not supported)");
+            if (decomposed()) return set_error(MB_ERR_INVALID, "mb_simulate_nose_hoover: not available in decomposed (multi-GPU) runs");
         }
         if (vcoupling.kind != MB_VC_NONE) {
             if (p->andersen_kT > 0 && p->andersen_prob > 0)
@@ -2065,6 +2102,7 @@ class Engine : public EngineBase {
         CmState<T>* cm = d_cm_.as<CmState<T>>();
         clear_cm_kernel<T><<<1, 1, 0, stream_>>>(cm);
         launches_++;
+        if (nh) MB_CUDA(cudaMemsetAsync(d_nh_.p, 0, sizeof(NhState), stream_));  // zeta = 0 at the start of every call
         StepCfg c;
         c.dt = (T)p->dt;
         c.dt_half = (T)p->dt / (T)2;
@@ -2074,8 +2112,13 @@ class Engine : public EngineBase {
         c.prob = p->andersen_prob;
         c.do_cm = (p->remove_cm_every == 0) ? 0 : (p->remove_cm_every == 1 ? 1 : -1);
         c.vc = VCouple{vcoupling.kind, vcoupling.n_steps, 3 * (long long)n_ - 3, vcoupling.kT, p->dt, vcoupling.tau, total_mass_};
-        c.langevin = lg != nullptr;
+        c.integrator = lg ? INTEG_LANGEVIN : (nh ? INTEG_NH : INTEG_VV);
         c.lc = LangevinCoef{1.0, 0.0, 0.0};
+        c.nc = NhCoef{0.0, 1.0};
+        if (nh) {  // NoseHoover(dt, temperature, damping): dt / (2 damping^2) and Nf k T0 (src/simulators.jl:1575-1579), in double
+            c.nc.coef = p->dt / (2.0 * nh->damping * nh->damping);
+            c.nc.nf_kT = (double)(3 * (long long)n_ - 3) * nh->kT;
+        }
         if (lg) {  // Langevin(dt, temperature, friction): vel_scale, noise_scale (src/simulators.jl:1092-1097), in double
             c.lc.vel_scale = exp(-p->dt * lg->friction);
             c.lc.noise_scale = sqrt(1.0 - c.lc.vel_scale * c.lc.vel_scale);
@@ -2157,7 +2200,7 @@ class Engine : public EngineBase {
             for (int m = 0; m < 8 && use_graph; m++) {
                 if (!need[m]) continue;
                 GraphKey key{path_, c.do_cm, c.thermostat ? 1 : 0, geom_version_, rebuild_every_, m, p->dt, p->andersen_kT, p->andersen_prob, n_, vcoupling,
-                             c.langevin ? 1 : 0, lg ? lg->kT : 0.0, lg ? lg->friction : 0.0};
+                             c.integrator, lg ? lg->kT : (nh ? nh->kT : 0.0), lg ? lg->friction : 0.0, nh ? nh->damping : 0.0};
                 if (!graphs_[m].exec || !(key == graphs_[m].key)) {
                     if (build_step_graph(c, key) != MB_OK) {
                         graph_failed_ = true;  // stay on the stream path for this context
@@ -2192,7 +2235,7 @@ class Engine : public EngineBase {
                 }
                 StepOpts o;
                 o.do_cm = do_cm;
-                o.clear_cm_after_k1 = clear_after_k1 && !c.langevin;
+                o.clear_cm_after_k1 = clear_after_k1 && c.integrator == INTEG_VV;
                 o.rebuild_hint = hint;
                 o.defer_cm = k < p->n_steps;
                 o.log_mask = log_mask_at(log, step_n);
@@ -2378,7 +2421,7 @@ class Engine : public EngineBase {
         const bool use_graph = graph_enabled_ && !graph_failed_ && !prof_.enabled && !pme_on_ && p->max_steps > 0;
         graph_used_ = false;
         if (use_graph) {
-            const GraphKey key{path_, 0, 0, geom_version_, 0, -1, 0.0, 0.0, 0.0, n_, {MB_VC_NONE, 0, 0.0, 0.0}, 0, 0.0, 0.0};
+            const GraphKey key{path_, 0, 0, geom_version_, 0, -1, 0.0, 0.0, 0.0, n_, {MB_VC_NONE, 0, 0.0, 0.0}, 0, 0.0, 0.0, 0.0};
             if (!sd_graph_.exec || !(key == sd_graph_.key)) {
                 if (build_sd_graph(key) != MB_OK) graph_failed_ = true;  // stay on the stream path for this context
             }
@@ -2602,6 +2645,7 @@ class Engine : public EngineBase {
     DevBuf d_mass_in_, d_charge_in_, d_ljp_in_;
     DevBuf d_pos4_, d_vel4_, d_f4_, d_xref4_, d_lj2_, d_orig_, d_inv_orig_, d_mass_;
     DevBuf d_pos4_t_, d_vel4_t_, d_lj2_t_, d_orig_t_, d_mass_t_;
+    DevBuf d_nh_;  // NhState of the Nose-Hoover integrator (fixed address: the step graphs bake it in)
     DevBuf d_ctl_, d_cm_, d_stage_a_, d_stage_b_, d_stage_c_, d_scalars_;
     DevBuf d_ex_ptr_, d_ex_idx_, d_sp_ptr_, d_sp_idx_;
     DevBuf d_cid_, d_perm_, d_cell_count_, d_cell_start_, d_cell_fill_;
@@ -2722,16 +2766,22 @@ int mb_random_velocities(mb_ctx* ctx, void* vels, double kT, uint64_t rng_ctr1, 
     return ctx->e->random_velocities(vels, kT, rng_ctr1, rng_key);
 }
 int mb_kinetic_energy_tensor(mb_ctx* ctx, const void* vels, double* ke_tensor9_host) { MB_CTX_GUARD(ctx); return ctx->e->kinetic_tensor(vels, ke_tensor9_host); }
-int mb_simulate_vv(mb_ctx* ctx, void* coords, void* vels, const mb_vv_params_t* p) { MB_CTX_GUARD(ctx); return ctx->e->simulate(coords, vels, p, nullptr, nullptr); }
+int mb_simulate_vv(mb_ctx* ctx, void* coords, void* vels, const mb_vv_params_t* p) { MB_CTX_GUARD(ctx); return ctx->e->simulate(coords, vels, p, nullptr, nullptr, nullptr); }
 int mb_simulate_vv_log(mb_ctx* ctx, void* coords, void* vels, const mb_vv_params_t* p, mb_log_t* log) {
     MB_CTX_GUARD(ctx);
-    return ctx->e->simulate(coords, vels, p, nullptr, log);
+    return ctx->e->simulate(coords, vels, p, nullptr, nullptr, log);
 }
 int mb_simulate_langevin(mb_ctx* ctx, void* coords, void* vels, const mb_langevin_params_t* p, mb_log_t* log) {
     MB_CTX_GUARD(ctx);
     if (!p) return mb::set_error(MB_ERR_INVALID, "null argument");
     const mb_vv_params_t vp = {p->dt, p->n_steps, p->init_step, p->remove_cm_every, 0.0, 0.0, p->rng_ctr1, p->rng_key};
-    return ctx->e->simulate(coords, vels, &vp, p, log);
+    return ctx->e->simulate(coords, vels, &vp, p, nullptr, log);
+}
+int mb_simulate_nose_hoover(mb_ctx* ctx, void* coords, void* vels, const mb_nosehoover_params_t* p, mb_log_t* log) {
+    MB_CTX_GUARD(ctx);
+    if (!p) return mb::set_error(MB_ERR_INVALID, "null argument");
+    const mb_vv_params_t vp = {p->dt, p->n_steps, p->init_step, p->remove_cm_every, 0.0, 0.0, 0, 0};
+    return ctx->e->simulate(coords, vels, &vp, nullptr, p, log);
 }
 int mb_minimize_sd(mb_ctx* ctx, void* coords, mb_sd_params_t* p) { MB_CTX_GUARD(ctx); return ctx->e->minimize_sd(coords, p); }
 int mb_set_velocity_coupling(mb_ctx* ctx, const mb_vcoupling_t* c) {
