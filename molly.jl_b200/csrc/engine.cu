@@ -5,6 +5,7 @@
 #include <algorithm>
 #include <map>
 #include <memory>
+#include <tuple>
 #include <type_traits>
 
 #include "../../include/mollyb200.h"
@@ -368,7 +369,7 @@ class Engine : public EngineBase {
         graph_enabled_ = !(ng && ng[0] == '1');
     }
     ~Engine() override {
-        destroy_graph();
+        drop_graphs();
         p2p_close();
         if (pme_plan_ >= 0 && g_cufft.Destroy) g_cufft.Destroy(pme_plan_);
         if (own_stream_) cudaStreamDestroy(stream_);
@@ -544,6 +545,7 @@ class Engine : public EngineBase {
     // digest parameters -> kernel constants, allocate per-atom state
     int prepare() {
         if (!dirty_) return MB_OK;
+        drop_graphs();  // they bake in what is digested here (Graph)
         if (n_ <= 0) return set_error(MB_ERR_STATE, "atoms not set");
         if (!(box_[0] > 0)) return set_error(MB_ERR_STATE, "box not set");
         if (n_ > 2000000000LL) return set_error(MB_ERR_INVALID, "too many atoms");
@@ -700,7 +702,6 @@ class Engine : public EngineBase {
         g_ap_.tric = tric_;
         floor_ = CapFloor();
         have_list_ = false;
-        destroy_sd_graph();  // the minimiser's graph bakes the kernel parameters in
         dirty_ = false;
         return MB_OK;
     }
@@ -886,7 +887,7 @@ class Engine : public EngineBase {
         }
         int64_t mx = std::max(sp_n_[0], std::max(sp_n_[1], sp_n_[2]));
         MB_CUDA(d_sp_partial_.ensure((size_t)(3 * ((mx + BONDED_THREADS - 1) / BONDED_THREADS) + 8) * sizeof(double)));
-        destroy_graph();  // the step graph bakes the term counts in
+        drop_graphs();  // the graphs bake the term counts in
         return MB_OK;
     }
     bool has_lists() const { return sp_n_[0] + sp_n_[1] + sp_n_[2] > 0; }
@@ -952,7 +953,7 @@ class Engine : public EngineBase {
         pme_rc_ = r_cut; pme_tol_ = error_tol; pme_epsr_ = eps_r;
         pme_on_ = true;
         pme_ready_ = false;
-        destroy_graph();  // the captured step does not contain the PME launches
+        drop_graphs();  // the captured graphs do not contain the PME launches
         return MB_OK;
     }
     // ---- LJDispersionCorrection (general interaction; lennard_jones.jl:163-275) -----------------------------------
@@ -1399,6 +1400,7 @@ class Engine : public EngineBase {
         MB_CUDA(cudaMemcpyAsync(&d_ctl_.as<Control>()->peak_ghost, zeros, sizeof(zeros), cudaMemcpyHostToDevice, stream_));
         for (;;) {  // ends: every retry makes the brick smaller, and a single cell that does not fit is refused
             MB_TRY(choose_geometry());
+            drop_graphs();  // they bake in the geometry and the list buffers sized for it
             MB_TRY(alloc_brick_tables());
             // pass A: sort + tables with unlimited halo capacity to measure
             g_.halo_cap = 65535;
@@ -1471,7 +1473,6 @@ class Engine : public EngineBase {
             MB_TRY(read_ctl(c));
             if (c.overflow) return set_error(MB_ERR_CAPACITY, "neighbour capacity overflow during first build");
             have_list_ = true;
-            geom_version_++;
             if (decomposed()) {
                 MB_TRY(update_ownership());
                 since_rebuild_ = 0;
@@ -1704,9 +1705,27 @@ class Engine : public EngineBase {
         bool defer_cm = false;           // decomposed: the next step's K1 sums the slabs' momenta itself
         int log_mask = 0;                // LOG_* records after the step
     };
-    // capture mode: the graph being built, the handle of its conditional rebuild node and where that node's body goes
-    struct Capture { cudaGraphConditionalHandle handle; cudaGraph_t graph; cudaGraph_t* body; };
-    int enqueue_step(const StepCfg& c, const StepOpts& o, const Capture* cap = nullptr) {
+    // capture mode (capture_graph): the handles of the conditional rebuild node (cell-list path) and of the WHILE loop (if
+    // any), and the rebuild node's body once splice_rebuild has added it
+    struct Capture { cudaGraphConditionalHandle rebuild = 0, loop = 0; cudaGraph_t body = nullptr; };
+    // a conditional IF node on the rebuild handle in place of the gated rebuild; capture_graph fills its body
+    int splice_rebuild(Capture& cap) {
+        cudaStreamCaptureStatus status;
+        const cudaGraphNode_t* deps = nullptr;
+        size_t ndeps = 0;
+        cudaGraph_t gcap = nullptr;
+        MB_CUDA(cudaStreamGetCaptureInfo_v2(stream_, &status, nullptr, &gcap, &deps, &ndeps));
+        cudaGraphNodeParams cp = {cudaGraphNodeTypeConditional};
+        cp.conditional.handle = cap.rebuild;
+        cp.conditional.type = cudaGraphCondTypeIf;
+        cp.conditional.size = 1;
+        cudaGraphNode_t cnode;
+        MB_CUDA(cudaGraphAddNode(&cnode, gcap, deps, ndeps, &cp));
+        cap.body = cp.conditional.phGraph_out[0];
+        MB_CUDA(cudaStreamUpdateCaptureDependencies(stream_, &cnode, 1, cudaStreamSetCaptureDependencies));
+        return MB_OK;
+    }
+    int enqueue_step(const StepCfg& c, const StepOpts& o, Capture* cap = nullptr) {
         const bool dec = decomposed() && path_ == 1;
         const int s0 = dec ? own_s0_ : 0, n_own = dec ? own_n_ : (int)n_;
         const int nb = std::max(1, (n_own + 255) / 256);
@@ -1732,14 +1751,14 @@ class Engine : public EngineBase {
             langevin_step_kernel<T><<<lgb, VV_THREADS, 0, stream_>>>(
                 n_own, c.dt, c.dt_half, c.skin_half2, c.lc, o.do_cm, c.inv_mass, cm, d_f4_.as<T4>(), d_xref4_.as<T4>(),
                 d_pos4_.as<T4>(), d_vel4_.as<T4>(), d_orig_.as<int>(), d_mass_.as<T>(), d_partial_.as<double>(), c.flag_ptr, ctl,
-                cap ? cap->handle : 0, cap && path_ == 1 ? 1 : 0, ext_map());
+                cap ? cap->rebuild : 0, cap && path_ == 1 ? 1 : 0, ext_map());
         } else if (c.integrator == INTEG_NH) {
             // (single GPU: s0 = 0.) At most vvb CTAs, so d_partial_ holds their 2 each
             const int nhb = std::max(1, std::min(nb, 8 * sm_count_));
             nh_kick_drift_kernel<T><<<nhb, VV_THREADS, 0, stream_>>>(
                 n_own, c.dt, c.dt_half, c.skin_half2, c.nc, d_nh_.as<NhState>(), cm, d_f4_.as<T4>(), d_xref4_.as<T4>(),
                 d_pos4_.as<T4>(), d_vel4_.as<T4>(), d_mass_.as<T>(), d_partial_.as<double>(), c.flag_ptr, ctl,
-                cap ? cap->handle : 0, cap && path_ == 1 ? 1 : 0, ext_map());
+                cap ? cap->rebuild : 0, cap && path_ == 1 ? 1 : 0, ext_map());
         } else {
             const Thermo<T> th = thermo_in_k1(c);
             const int thk = th.on ? TH_ANDERSEN : (c.vc.kind != VC_NONE ? TH_SCALE : TH_NONE);
@@ -1747,7 +1766,7 @@ class Engine : public EngineBase {
                 // two atoms per thread, one wave (48 registers: 5 CTAs per SM)
                 vv_kick_drift_kernel<T, TH><<<std::max(1, std::min((nb + 1) / 2, 5 * sm_count_)), 256, 0, stream_>>>(
                     s0, n_own, c.dt, c.dt_half, c.skin_half2, cm, d_f4_.as<T4>(), d_xref4_.as<T4>(), d_pos4_.as<T4>(), d_vel4_.as<T4>(),
-                    c.flag_ptr, ctl, cap ? cap->handle : 0, cap && path_ == 1 ? 1 : 0, push, ext_map(), th);
+                    c.flag_ptr, ctl, cap ? cap->rebuild : 0, cap && path_ == 1 ? 1 : 0, push, ext_map(), th);
             });
         }
         prof_.end(Prof::VV);
@@ -1760,21 +1779,7 @@ class Engine : public EngineBase {
             wrap_kernel<T><<<nb, 256, 0, stream_>>>((int)n_, geom(), d_pos4_.as<T4>());
             launches_++;
         } else if (cap) {
-            // splice a conditional IF node into the capture; its body is filled in by the caller
-            cudaStreamCaptureStatus status;
-            const cudaGraphNode_t* deps = nullptr;
-            size_t ndeps = 0;
-            cudaGraph_t gcap = nullptr;
-            MB_CUDA(cudaStreamGetCaptureInfo_v2(stream_, &status, nullptr, &gcap, &deps, &ndeps));
-            cudaGraphNodeParams cp = {cudaGraphNodeTypeConditional};
-            cp.type = cudaGraphNodeTypeConditional;
-            cp.conditional.handle = cap->handle;
-            cp.conditional.type = cudaGraphCondTypeIf;
-            cp.conditional.size = 1;
-            cudaGraphNode_t cnode;
-            MB_CUDA(cudaGraphAddNode(&cnode, cap->graph, deps, ndeps, &cp));
-            *cap->body = cp.conditional.phGraph_out[0];
-            MB_CUDA(cudaStreamUpdateCaptureDependencies(stream_, &cnode, 1, cudaStreamSetCaptureDependencies));
+            MB_TRY(splice_rebuild(*cap));
         } else if (dec) {
             if (o.rebuild_hint) {
                 // neighbour rebuild on a decomposed box: replicate positions and velocities, rebuild (identical sort on every
@@ -1881,89 +1886,101 @@ class Engine : public EngineBase {
         return th;
     }
 
-    // log_mask: the LOG_* records the step graph ends with (0: a plain step). The logging kernel's destinations are read from
-    // the device descriptor (d_log_desc_), so they are not part of the key.
+    // What a simulate call chooses that its step graphs bake in: the step options, the thermostat and integrator
+    // parameters (kernel arguments) and the log mask, the LOG_* records the graph ends with (0: a plain step). The logging
+    // kernel's destinations are read from the device descriptor (d_log_desc_), so they are not part of it.
     struct GraphKey {
-        int path, do_cm, thermostat, geom_version, rebuild_every, log_mask;
-        double dt, kT, prob;
-        int64_t n;
-        mb_vcoupling_t vc;  // the velocity-rescaling thermostat's kind and parameters (baked into K2's arguments)
-        int integrator;     // INTEG_*, and Langevin's kT and friction or Nose-Hoover's kT and damping (baked into the
-        double integ_kT, friction, damping;  // step kernels' arguments)
-        bool operator==(const GraphKey& o) const {
-            return path == o.path && do_cm == o.do_cm && thermostat == o.thermostat && geom_version == o.geom_version &&
-                   rebuild_every == o.rebuild_every && log_mask == o.log_mask && dt == o.dt && kT == o.kT && prob == o.prob && n == o.n &&
-                   vc.kind == o.vc.kind && vc.n_steps == o.vc.n_steps && vc.kT == o.vc.kT && vc.tau == o.vc.tau &&
-                   integrator == o.integrator && integ_kT == o.integ_kT && friction == o.friction && damping == o.damping;
+        int do_cm, log_mask, integrator;  // INTEG_*
+        double dt, andersen_kT, andersen_prob;
+        double integ_kT, friction, damping;  // Langevin's kT and friction, or Nose-Hoover's kT and damping
+        mb_vcoupling_t vc;                   // the velocity-rescaling thermostat (K2's arguments)
+        auto fields() const {
+            return std::tie(do_cm, log_mask, integrator, dt, andersen_kT, andersen_prob, integ_kT, friction, damping, vc.kind,
+                            vc.n_steps, vc.kT, vc.tau);
         }
+        bool operator==(const GraphKey& o) const { return fields() == o.fields(); }
     };
-    // one executable step graph per log mask; the host loop picks one per step
-    struct StepGraph {
+    // A captured graph: a step graph (one per log mask; the host loop picks one per step) or the minimiser's loop.
+    // Invalidation rule: captured kernel nodes keep their arguments by value (pair parameters, box, masses, term counts,
+    // geometry, buffer addresses), so every graph is dropped wherever context state they bake in changes: in prepare(),
+    // which every setter of atoms, box, interactions, exceptions, neighbour policy or launch config reaches through dirty_;
+    // in first_build(), which picks the geometry and sizes the list buffers; in set_specific() and set_pme(). The key then
+    // holds only what a simulate call chooses; the minimiser's graph needs none.
+    struct Graph {
         cudaGraph_t graph = nullptr;
         cudaGraphExec_t exec = nullptr;
-        GraphKey key;
-        int64_t launches = 0;  // kernels per step outside the rebuild body
+        int64_t launches = 0;  // kernels per launch outside the rebuild body
+        GraphKey key = {};
+        void drop() {
+            if (exec) cudaGraphExecDestroy(exec);
+            if (graph) cudaGraphDestroy(graph);
+            exec = nullptr;
+            graph = nullptr;
+        }
     };
-    void destroy_graph(int mask) {
-        StepGraph& sg = graphs_[mask];
-        if (sg.exec) cudaGraphExecDestroy(sg.exec);
-        if (sg.graph) cudaGraphDestroy(sg.graph);
-        sg.exec = nullptr;
-        sg.graph = nullptr;
+    void drop_graphs() {
+        for (Graph& g : graphs_) g.drop();
+        sd_graph_.drop();
     }
-    void destroy_graph() {
-        for (int m = 0; m < 8; m++) destroy_graph(m);
-        destroy_sd_graph();
-    }
-    // Capture one MD step (K1, [IF rebuild], force, K2, [thermostat], [log records]; Langevin: L, [IF rebuild], force,
-    // [log records]; Nose-Hoover: NH1, [IF rebuild], force, NH2, [log records]) into an executable graph.
-    int build_step_graph(const StepCfg& c, const GraphKey& key) {
-        const int mask = key.log_mask;
-        destroy_graph(mask);
-        cudaGraph_t& gr = graphs_[mask].graph;
-        cudaGraphExec_t& gx = graphs_[mask].exec;
-        const bool prof_was = prof_.enabled;
-        prof_.enabled = false;
-        const int64_t launches_before = launches_;
-        auto fail = [&](int rc) {
+    // what both graph paths need: graphs enabled, no failed capture, no stage timers, no PME (its cuFFT launches stay
+    // outside the captured graphs)
+    bool graphs_usable() const { return graph_enabled_ && !graph_failed_ && !prof_.enabled && !pme_on_; }
+    // Capture enqueue(cap) into g. On the cell-list path enqueue splices the conditional rebuild node (splice_rebuild) and
+    // the rebuild pipeline is captured into its body. loop: enqueue is captured as the body of a WHILE node on cap.loop.
+    // launches_ is restored (g.launches counts the captured kernels per launch); a failure ends the capture, clears the
+    // error and restores n_force_evals_ too.
+    template <typename Enqueue>
+    int capture_graph(Graph& g, bool loop, Enqueue enqueue) {
+        g.drop();
+        const int64_t launches_before = launches_, evals_before = n_force_evals_;
+        auto fail = [&]() {
             cudaStreamCaptureStatus st;
             if (cudaStreamIsCapturing(stream_, &st) == cudaSuccess && st != cudaStreamCaptureStatusNone) {
                 cudaGraph_t junk = nullptr;
                 cudaStreamEndCapture(stream_, &junk);
             }
             cudaGetLastError();
-            destroy_graph(mask);
-            prof_.enabled = prof_was;
+            g.drop();
             launches_ = launches_before;
-            return rc;
+            n_force_evals_ = evals_before;
+            return MB_ERR_CUDA;
         };
-        if (cudaGraphCreate(&gr, 0) != cudaSuccess) return fail(MB_ERR_CUDA);
-        cudaGraphConditionalHandle handle = 0;
-        if (path_ == 1 && cudaGraphConditionalHandleCreate(&handle, gr, 0, cudaGraphCondAssignDefault) != cudaSuccess)
-            return fail(MB_ERR_CUDA);
-        if (cudaStreamBeginCaptureToGraph(stream_, gr, nullptr, nullptr, 0, cudaStreamCaptureModeRelaxed) != cudaSuccess)
-            return fail(MB_ERR_CUDA);
-        cudaGraph_t body = nullptr;
+        if (cudaGraphCreate(&g.graph, 0) != cudaSuccess) return fail();
+        Capture cap;
+        cudaGraph_t into = g.graph;
+        if (loop) {
+            if (cudaGraphConditionalHandleCreate(&cap.loop, g.graph, 1, cudaGraphCondAssignDefault) != cudaSuccess) return fail();
+            cudaGraphNodeParams cp = {cudaGraphNodeTypeConditional};
+            cp.conditional.handle = cap.loop;
+            cp.conditional.type = cudaGraphCondTypeWhile;
+            cp.conditional.size = 1;
+            cudaGraphNode_t wnode;
+            if (cudaGraphAddNode(&wnode, g.graph, nullptr, 0, &cp) != cudaSuccess) return fail();
+            into = cp.conditional.phGraph_out[0];
+        }
+        if (path_ == 1 && cudaGraphConditionalHandleCreate(&cap.rebuild, g.graph, 0, cudaGraphCondAssignDefault) != cudaSuccess)
+            return fail();
+        auto capture_into = [&](cudaGraph_t graph, auto body) {
+            cudaGraph_t out = nullptr;
+            return cudaStreamBeginCaptureToGraph(stream_, graph, nullptr, nullptr, 0, cudaStreamCaptureModeRelaxed) == cudaSuccess &&
+                   body() == MB_OK && cudaStreamEndCapture(stream_, &out) == cudaSuccess;
+        };
+        if (!capture_into(into, [&] { return enqueue(cap); })) return fail();
+        g.launches = launches_ - launches_before;
+        if (path_ == 1 && !(cap.body && capture_into(cap.body, [&] { return enqueue_rebuild(true, false); }))) return fail();
+        if (cudaGraphInstantiate(&g.exec, g.graph, 0) != cudaSuccess) return fail();
+        launches_ = launches_before;
+        return MB_OK;
+    }
+    // One MD step (K1, [IF rebuild], force, K2, [thermostat], [log records]; Langevin: L, [IF rebuild], force,
+    // [log records]; Nose-Hoover: NH1, [IF rebuild], force, NH2, [log records]) as an executable graph.
+    int build_step_graph(const StepCfg& c, const GraphKey& key) {
         StepOpts o;
         o.do_cm = c.do_cm;
-        o.log_mask = mask;
-        const Capture cap = {handle, gr, &body};
-        if (enqueue_step(c, o, &cap) != MB_OK) return fail(MB_ERR_CUDA);
-        cudaGraph_t out = nullptr;
-        if (cudaStreamEndCapture(stream_, &out) != cudaSuccess) return fail(MB_ERR_CUDA);
-        const int64_t step_nodes = launches_ - launches_before;
-        if (path_ == 1) {
-            if (!body) return fail(MB_ERR_CUDA);
-            if (cudaStreamBeginCaptureToGraph(stream_, body, nullptr, nullptr, 0, cudaStreamCaptureModeRelaxed) != cudaSuccess)
-                return fail(MB_ERR_CUDA);
-            if (enqueue_rebuild(true, false) != MB_OK) return fail(MB_ERR_CUDA);
-            if (cudaStreamEndCapture(stream_, &out) != cudaSuccess) return fail(MB_ERR_CUDA);
-        }
-        if (cudaGraphInstantiate(&gx, gr, 0) != cudaSuccess) return fail(MB_ERR_CUDA);
-        prof_.enabled = prof_was;
-        launches_ = launches_before;
-        graphs_[mask].launches = step_nodes;
-        graphs_[mask].key = key;
+        o.log_mask = key.log_mask;
+        Graph& g = graphs_[key.log_mask];
+        MB_TRY(capture_graph(g, false, [&](Capture& cap) { return enqueue_step(c, o, &cap); }));
+        g.key = key;
         return MB_OK;
     }
 
@@ -2189,18 +2206,18 @@ class Engine : public EngineBase {
             }
         }
 
-        // CUDA-graph path: static per-step sequence (remove_CM_motion in {0,1}, no stage timers requested)
-        bool use_graph = graph_enabled_ && !graph_failed_ && !prof_.enabled && c.do_cm >= 0 && p->n_steps >= 4 &&
-                         !(cm_pending && c.do_cm == 0) && !dec &&  // the decomposed step issues NCCL calls with per-rebuild sizes
-                         !pme_on_;                                  // cuFFT launches stay outside the captured step for now
+        // CUDA-graph path: static per-step sequence (remove_CM_motion in {0,1})
+        bool use_graph = graphs_usable() && c.do_cm >= 0 && p->n_steps >= 4 && !(cm_pending && c.do_cm == 0) &&
+                         !dec;  // the decomposed step issues NCCL calls with per-rebuild sizes
         if (use_graph) {
             // one executable per log mask this call uses (the plain step and the log steps)
             bool need[8] = {false, false, false, false, false, false, false, false};
             for (int64_t k = 1; k <= p->n_steps; k++) need[log_mask_at(log, p->init_step + k)] = true;
+            GraphKey key{c.do_cm, 0, c.integrator, p->dt, p->andersen_kT, p->andersen_prob, lg ? lg->kT : (nh ? nh->kT : 0.0),
+                         lg ? lg->friction : 0.0, nh ? nh->damping : 0.0, vcoupling};
             for (int m = 0; m < 8 && use_graph; m++) {
                 if (!need[m]) continue;
-                GraphKey key{path_, c.do_cm, c.thermostat ? 1 : 0, geom_version_, rebuild_every_, m, p->dt, p->andersen_kT, p->andersen_prob, n_, vcoupling,
-                             c.integrator, lg ? lg->kT : (nh ? nh->kT : 0.0), lg ? lg->friction : 0.0, nh ? nh->damping : 0.0};
+                key.log_mask = m;
                 if (!graphs_[m].exec || !(key == graphs_[m].key)) {
                     if (build_step_graph(c, key) != MB_OK) {
                         graph_failed_ = true;  // stay on the stream path for this context
@@ -2272,13 +2289,13 @@ class Engine : public EngineBase {
     // Steepest-descent minimisation (minimize.cuh). The kept forces and saved positions are in original order: d_sd_f_,
     // d_sd_x_; the trial's forces go to d_f4_ (slot order), so the context's force state is not preserved.
     // The evaluation of the current positions, the decision and the accept pass (init: the starting coordinates)
-    int enqueue_sd_eval(bool init, const Capture* cap_while) {
+    int enqueue_sd_eval(bool init, const Capture* cap = nullptr) {
         Partials parts;
         MB_TRY(launch_pairs(true, d_f4_.as<T4>(), false, &parts));
         MB_TRY(launch_bonded(true));
         sd_decide_kernel<<<1, SD_THREADS, 0, stream_>>>(d_sd_st_.as<SdState>(), parts.pe, parts.n,
                                                         has_specific() ? d_sp_energy_.as<double>() : nullptr, init ? 1 : 0,
-                                                        cap_while ? cap_while->handle : 0, cap_while ? 1 : 0);
+                                                        cap ? cap->loop : 0, cap ? 1 : 0);
         const int nb = std::max(1, std::min((int)((n_ + SD_THREADS - 1) / SD_THREADS), 4 * sm_count_));
         sd_accept_kernel<T><<<nb, SD_THREADS, 0, stream_>>>((int)n_, path_ == 1 ? d_orig_.as<int>() : nullptr, d_f4_.as<T4>(),
                                                             d_sd_f_.as<T4>(), d_sd_x_.as<T4>(), d_pos4_.as<T4>(), ext_map(),
@@ -2287,94 +2304,31 @@ class Engine : public EngineBase {
         MB_CUDA(cudaGetLastError());
         return MB_OK;
     }
-    // One iteration: trial, [rebuild], evaluation, decision, accept/restore. cap_if: capture mode, where the rebuild becomes a
-    // conditional IF node (its body is captured by the caller into *cap_if->body); otherwise the gated pipeline is enqueued.
-    int enqueue_sd_iter(const Capture* cap_if, const Capture* cap_while) {
+    // One iteration: trial, [rebuild], evaluation, decision, accept/restore. cap: capture mode, where the rebuild becomes a
+    // conditional IF node (splice_rebuild); otherwise the gated pipeline is enqueued.
+    int enqueue_sd_iter(Capture* cap = nullptr) {
         const int nb = std::max(1, std::min((int)((n_ + SD_THREADS - 1) / SD_THREADS), 4 * sm_count_));
         sd_trial_kernel<T><<<nb, SD_THREADS, 0, stream_>>>((int)n_, path_ == 1 ? d_orig_.as<int>() : nullptr, d_sd_f_.as<T4>(),
                                                            d_pos4_.as<T4>(), d_sd_x_.as<T4>(), d_xref4_.as<T4>(),
                                                            path_ == 1 ? g_.skin_half2 : (T)0, ext_map(), d_ctl_.as<Control>(),
-                                                           d_sd_st_.as<SdState>(), cap_if ? cap_if->handle : 0, cap_if ? 1 : 0);
+                                                           d_sd_st_.as<SdState>(), cap ? cap->rebuild : 0, cap && path_ == 1 ? 1 : 0);
         launches_++;
         if (path_ == 0) {
             wrap_kernel<T><<<(int)((n_ + 255) / 256), 256, 0, stream_>>>((int)n_, g_ap_, d_pos4_.as<T4>());
             launches_++;
-        } else if (cap_if) {
-            cudaStreamCaptureStatus status;
-            const cudaGraphNode_t* deps = nullptr;
-            size_t ndeps = 0;
-            cudaGraph_t gcap = nullptr;
-            MB_CUDA(cudaStreamGetCaptureInfo_v2(stream_, &status, nullptr, &gcap, &deps, &ndeps));
-            cudaGraphNodeParams cp = {cudaGraphNodeTypeConditional};
-            cp.type = cudaGraphNodeTypeConditional;
-            cp.conditional.handle = cap_if->handle;
-            cp.conditional.type = cudaGraphCondTypeIf;
-            cp.conditional.size = 1;
-            cudaGraphNode_t cnode;
-            MB_CUDA(cudaGraphAddNode(&cnode, gcap, deps, ndeps, &cp));
-            *cap_if->body = cp.conditional.phGraph_out[0];
-            MB_CUDA(cudaStreamUpdateCaptureDependencies(stream_, &cnode, 1, cudaStreamSetCaptureDependencies));
+        } else if (cap) {
+            MB_TRY(splice_rebuild(*cap));
         } else {
             MB_TRY(enqueue_rebuild(true, false));
         }
-        return enqueue_sd_eval(false, cap_while);
+        return enqueue_sd_eval(false, cap);
     }
-    void destroy_sd_graph() {
-        if (sd_graph_.exec) cudaGraphExecDestroy(sd_graph_.exec);
-        if (sd_graph_.graph) cudaGraphDestroy(sd_graph_.graph);
-        sd_graph_.exec = nullptr;
-        sd_graph_.graph = nullptr;
-    }
-    // Capture the iteration loop: a conditional WHILE node (continue flag set by the decide kernel) whose body is one
-    // iteration, with the rebuild as a nested conditional IF node on the cell-list path.
-    int build_sd_graph(const GraphKey& key) {
-        destroy_sd_graph();
-        cudaGraph_t& gr = sd_graph_.graph;
-        const int64_t launches_before = launches_, evals_before = n_force_evals_;
-        auto fail = [&](int rc) {
-            cudaStreamCaptureStatus st;
-            if (cudaStreamIsCapturing(stream_, &st) == cudaSuccess && st != cudaStreamCaptureStatusNone) {
-                cudaGraph_t junk = nullptr;
-                cudaStreamEndCapture(stream_, &junk);
-            }
-            cudaGetLastError();
-            destroy_sd_graph();
-            launches_ = launches_before;
-            n_force_evals_ = evals_before;
-            return rc;
-        };
-        if (cudaGraphCreate(&gr, 0) != cudaSuccess) return fail(MB_ERR_CUDA);
-        cudaGraphConditionalHandle h_while = 0, h_if = 0;
-        if (cudaGraphConditionalHandleCreate(&h_while, gr, 1, cudaGraphCondAssignDefault) != cudaSuccess) return fail(MB_ERR_CUDA);
-        if (path_ == 1 && cudaGraphConditionalHandleCreate(&h_if, gr, 0, cudaGraphCondAssignDefault) != cudaSuccess)
-            return fail(MB_ERR_CUDA);
-        cudaGraphNodeParams cp = {cudaGraphNodeTypeConditional};
-        cp.type = cudaGraphNodeTypeConditional;
-        cp.conditional.handle = h_while;
-        cp.conditional.type = cudaGraphCondTypeWhile;
-        cp.conditional.size = 1;
-        cudaGraphNode_t wnode;
-        if (cudaGraphAddNode(&wnode, gr, nullptr, 0, &cp) != cudaSuccess) return fail(MB_ERR_CUDA);
-        cudaGraph_t loop_body = cp.conditional.phGraph_out[0], rebuild_body = nullptr;
-        if (cudaStreamBeginCaptureToGraph(stream_, loop_body, nullptr, nullptr, 0, cudaStreamCaptureModeRelaxed) != cudaSuccess)
-            return fail(MB_ERR_CUDA);
-        const Capture cap_if = {h_if, loop_body, &rebuild_body}, cap_while = {h_while, gr, nullptr};
-        if (enqueue_sd_iter(path_ == 1 ? &cap_if : nullptr, &cap_while) != MB_OK) return fail(MB_ERR_CUDA);
-        cudaGraph_t out = nullptr;
-        if (cudaStreamEndCapture(stream_, &out) != cudaSuccess) return fail(MB_ERR_CUDA);
-        const int64_t iter_launches = launches_ - launches_before;
-        if (path_ == 1) {
-            if (!rebuild_body) return fail(MB_ERR_CUDA);
-            if (cudaStreamBeginCaptureToGraph(stream_, rebuild_body, nullptr, nullptr, 0, cudaStreamCaptureModeRelaxed) != cudaSuccess)
-                return fail(MB_ERR_CUDA);
-            if (enqueue_rebuild(true, false) != MB_OK) return fail(MB_ERR_CUDA);
-            if (cudaStreamEndCapture(stream_, &out) != cudaSuccess) return fail(MB_ERR_CUDA);
-        }
-        if (cudaGraphInstantiate(&sd_graph_.exec, gr, 0) != cudaSuccess) return fail(MB_ERR_CUDA);
-        launches_ = launches_before;
+    // The iteration loop: a conditional WHILE node (continue flag set by the decide kernel) whose body is one iteration, with
+    // the rebuild as a nested conditional IF node on the cell-list path.
+    int build_sd_graph() {
+        const int64_t evals_before = n_force_evals_;  // minimize_sd counts the iterations the graph runs
+        MB_TRY(capture_graph(sd_graph_, true, [&](Capture& cap) { return enqueue_sd_iter(&cap); }));
         n_force_evals_ = evals_before;
-        sd_graph_.launches = iter_launches;
-        sd_graph_.key = key;
         return MB_OK;
     }
 
@@ -2417,14 +2371,10 @@ class Engine : public EngineBase {
             if (have_list_) MB_TRY(set_flag_rebuild());
             MB_TRY(sync_state_from(xb.as<T>(), nullptr));
         }
-        MB_TRY(enqueue_sd_eval(true, nullptr));
-        const bool use_graph = graph_enabled_ && !graph_failed_ && !prof_.enabled && !pme_on_ && p->max_steps > 0;
+        MB_TRY(enqueue_sd_eval(true));
         graph_used_ = false;
-        if (use_graph) {
-            const GraphKey key{path_, 0, 0, geom_version_, 0, -1, 0.0, 0.0, 0.0, n_, {MB_VC_NONE, 0, 0.0, 0.0}, 0, 0.0, 0.0, 0.0};
-            if (!sd_graph_.exec || !(key == sd_graph_.key)) {
-                if (build_sd_graph(key) != MB_OK) graph_failed_ = true;  // stay on the stream path for this context
-            }
+        if (graphs_usable() && p->max_steps > 0) {
+            if (!sd_graph_.exec && build_sd_graph() != MB_OK) graph_failed_ = true;  // stay on the stream path for this context
             graph_used_ = !graph_failed_;
         }
         SdState out;
@@ -2440,7 +2390,7 @@ class Engine : public EngineBase {
                 MB_CUDA(cudaMemcpyAsync(&cont, &d_sd_st_.as<SdState>()->cont, sizeof(int), cudaMemcpyDeviceToHost, stream_));
                 MB_CUDA(cudaStreamSynchronize(stream_));
                 if (!cont) break;
-                MB_TRY(enqueue_sd_iter(nullptr, nullptr));
+                MB_TRY(enqueue_sd_iter());
             }
             MB_CUDA(cudaMemcpyAsync(&out, d_sd_st_.p, sizeof(out), cudaMemcpyDeviceToHost, stream_));
             MB_CUDA(cudaStreamSynchronize(stream_));
@@ -2606,10 +2556,9 @@ class Engine : public EngineBase {
     Tric<T> tric_ = {};  // TriclinicBoundary (on = 0: cubic / rectangular box)
     int64_t launches_ = 0, n_force_evals_ = 0, n_steps_ = 0;
     Prof prof_;
-    StepGraph graphs_[8];
-    StepGraph sd_graph_;  // the minimiser's iteration loop (key: path, geometry version, n)
+    Graph graphs_[8];  // step graphs by log mask
+    Graph sd_graph_;   // the minimiser's iteration loop
     bool graph_enabled_ = true, graph_failed_ = false, graph_used_ = false, own_stream_ = false;
-    int geom_version_ = 0;
     // spatial decomposition (z-slabs of cell layers; one rank per GPU)
     ncclComm_t comm_ = nullptr;
     int rank_ = 0, nranks_ = 1;
