@@ -13,7 +13,7 @@ import pytest
 import mbhelpers as H
 import mollyb200 as mb
 from oracle import oracle as o
-from test_gpu_parity import _boundary_atoms, _check, _cutoff_force_bound, _etol, _pos_err, _tol
+from test_gpu_parity import _pos_err
 
 pytestmark = pytest.mark.gpu
 
@@ -53,16 +53,16 @@ class _Reference:
 
     def check(self, f, label, e=None, vir=None, st=None):
         per_atom = np.abs(f.astype(F64) - self.f).max(axis=1)
-        allowed = _tol(self.dtype, self.fmax)
+        allowed = H.tol(self.dtype, self.fmax)
         if self.dtype == F32 and per_atom.max() > allowed:
             # pairs sitting on a cutoff within f32 rounding may land on either side: one F(rc) jump each
-            allowed = allowed + _boundary_atoms(self.orc, self.x64, self.o_inters) * _cutoff_force_bound(self.sd, self.o_inters)
+            allowed = allowed + H.boundary_atoms(self.orc, self.x64, self.o_inters) * H.cutoff_force_bound(self.sd, self.o_inters)
         where = "" if st is None else f"path={st['path']} brick={st['brick_dims']} n_cells={st['n_cells']} "
         de = "" if e is None else f" dE={e - self.e:.3e} (E={self.e:.6e})"
         print(f"[{label}] n={self.sd['n']} {self.dtype.name} {where}max|dF|={per_atom.max():.3e} (max|F|={self.fmax:.3e}){de}")
         assert (per_atom <= allowed).all(), label
         if e is not None:
-            assert abs(e - self.e) <= _etol(self.dtype, self.e), label
+            assert abs(e - self.e) <= H.etol(self.dtype, self.e), label
         if vir is not None:
             vtol = (1e-9 if self.dtype == F64 else 1e-4) * max(np.abs(self.vir).max(), 1.0)
             assert np.abs(vir.astype(F64) - self.vir).max() <= vtol, label
@@ -72,7 +72,7 @@ def _evaluate(s):
     f = mb.forces(s)
     e = mb.potential_energy(s)
     f2, vir = mb.forces_virial(s)
-    assert np.abs(f2.astype(F64) - f.astype(F64)).max() <= _tol(s.dtype, np.abs(f).max())
+    assert np.abs(f2.astype(F64) - f.astype(F64)).max() <= H.tol(s.dtype, np.abs(f).max())
     return f, e, vir
 
 
@@ -120,7 +120,7 @@ def test_forced_brick_shapes(kind, dtype):
         if first is None:
             first = f
         # a pair's image depends on the two atoms' cells only, so every shape evaluates the same pairs
-        assert np.abs(f.astype(F64) - first.astype(F64)).max() <= _tol(dtype, ref.fmax)
+        assert np.abs(f.astype(F64) - first.astype(F64)).max() <= H.tol(dtype, ref.fmax)
     print(f"    pairs in the list: {sorted(pairs)}")
     assert len(pairs) == 1
     if dtype == F64:  # full-shell list: every pair within r_list that is not excluded, twice
@@ -311,7 +311,7 @@ def _with_hub(sd, n_excluded, n_special):
 def test_long_and_index_distant_partner_lists(path, dtype):
     sd, rc, rl = _partner_system(path)
     sd = _with_hub(sd, 40, 40)
-    _check(sd, *_molecular_inters(rc), dtype, r_list=rl, expect_path=path, label=f"40 + 40 partners, path {path}")
+    H.check(sd, *_molecular_inters(rc), dtype, r_list=rl, expect_path=path, label=f"40 + 40 partners, path {path}")
 
 
 @pytest.mark.parametrize("dtype", [F64, F32])
@@ -326,7 +326,7 @@ def test_256_special_partners(path, dtype):
             mb.forces(s)
         s.close()
     else:
-        _check(sd, mi, oi, dtype, r_list=rl, expect_path=0, label="256 special partners, no-list path")
+        H.check(sd, mi, oi, dtype, r_list=rl, expect_path=0, label="256 special partners, no-list path")
 
 
 # ---------------------------------------------------------------------------------------------------
@@ -344,7 +344,7 @@ def test_unwrapped_input_coordinates(dtype):
     sd = dict(sd, coords=x.astype(dtype))
     mi, oi = _lj_inters(1.2, shifted_force=True)
     s, f_w, _ = _run(sd, mi, oi, dtype, 1.3, "wrapped input")
-    tol = _tol(dtype, np.abs(f_w).max())
+    tol = H.tol(dtype, np.abs(f_w).max())
     k = np.random.default_rng(0).integers(-2, 3, x.shape)
     at_L, neg_zero = sd["coords"].copy(), sd["coords"].copy()
     for d in range(3):

@@ -9,7 +9,7 @@ import pytest
 
 import mbhelpers as H
 import mollyb200 as mb
-from test_gpu_parity import _etol, _pos_err, _tol
+from test_gpu_parity import _pos_err
 
 pytestmark = pytest.mark.gpu
 
@@ -126,9 +126,9 @@ def test_host_and_device_arrays_agree(name, make, dtype, golden_6mrr):
                 continue
             assert np.array_equal(h[k], d[k]), (mode, k)
         if bonded:
-            ftol = 1e-12 * fmax if dtype == F64 else _tol(F32, fmax)
+            ftol = 1e-12 * fmax if dtype == F64 else H.tol(F32, fmax)
             assert np.abs(h["f_all"] - d["f_all"]).max() <= ftol, mode
-            assert abs(h["pe_all"][0] - d["pe_all"][0]) <= _etol(dtype, h["pe_all"][0]), mode
+            assert abs(h["pe_all"][0] - d["pe_all"][0]) <= H.etol(dtype, h["pe_all"][0]), mode
             ex, ev = _pos_err(h["x_sim"], d["x_sim"], box), np.abs(h["v_sim"] - d["v_sim"]).max()
             print(f"[{name} {mode}] simulate dx={ex:.3e} dv={ev:.3e}")
             assert ex < (1e-9 if dtype == F64 else 1e-4) and ev < (1e-6 if dtype == F64 else 1e-3), mode

@@ -8,7 +8,7 @@ import pytest
 
 import mbhelpers as H
 import mollyb200 as mb
-from test_gpu_parity import _etol, _pos_err
+from test_gpu_parity import _pos_err
 
 pytestmark = pytest.mark.gpu
 
@@ -101,7 +101,7 @@ def test_records_match_unlogged_runs_stopped_at_each_step(name, dtype, r_list, k
         if step in e_steps:
             k = e_steps.index(step)
             pe, ke = mb.potential_energy(r), mb.kinetic_energy(r)
-            bar = (lambda e: 1e-9 * abs(e)) if dtype == F64 else (lambda e: _etol(dtype, e))
+            bar = (lambda e: 1e-9 * abs(e)) if dtype == F64 else (lambda e: H.etol(dtype, e))
             assert abs(L["pe"].history[k] - pe) <= bar(pe), (step, L["pe"].history[k], pe)
             assert abs(L["ke"].history[k] - ke) <= bar(ke), (step, L["ke"].history[k], ke)
             assert abs(L["tot"].history[k] - (pe + ke)) <= bar(pe) + bar(ke)

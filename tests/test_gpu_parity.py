@@ -19,97 +19,11 @@ from oracle import oracle as o
 pytestmark = pytest.mark.gpu
 
 
-def _tol(dtype, fmax):
-    return (1e-9 * fmax + 1e-9) if np.dtype(dtype) == np.float64 else (5e-5 * fmax + 2e-3)
-
-
-def _etol(dtype, e):
-    return (1e-11 if np.dtype(dtype) == np.float64 else 2e-6) * max(abs(e), 1.0)
-
-
-def _boundary_atoms(orc, x64, o_inters, delta=3e-6):
-    """Atoms that own a pair sitting on a cutoff within f32 rounding of r^2, where a DistanceCutoff /
-    reaction-field force is discontinuous (it jumps by F(rc) ~ 1-2 kJ/mol/nm for CRF with water charges), and
-    a bound on that jump. The reference has the same sensitivity between its f32 and f64 paths."""
-    n = len(x64)
-    count = np.zeros(n)
-    for rc in sorted({it.r_cut for it in o_inters if it.r_cut > 0}):
-        hi = orc.neighbor_list(x64, rc * (1 + delta))
-        lo = orc.neighbor_list(x64, rc * (1 - delta))
-        key = lambda a: set(map(tuple, a[:, :2].tolist()))
-        for i, j in key(hi) - key(lo):
-            count[i] += 1
-            count[j] += 1
-    return count
-
-
-def _cutoff_force_bound(sysd, o_inters):
-    """max |F(rc)| of a single pair over the interaction tuple."""
-    b = 0.0
-    qmax = np.abs(sysd["charge"]).max()
-    for it in o_inters:
-        rc = it.r_cut
-        if rc <= 0:
-            continue
-        if it.kind == o.LJ and it.cutoff_kind == o.CUT_DISTANCE:
-            sig, eps = sysd["sigma"].max(), sysd["eps"].max()
-            s6 = (sig / rc) ** 6
-            b += abs(24 * eps / rc * (2 * s6 * s6 - s6))
-        elif it.kind == o.CRF:
-            e = it.solvent_dielectric
-            krf = (1 / rc ** 3) * (e - 1) / (2 * e + 1)
-            b += it.coulomb_const * qmax * qmax * abs(1 / rc ** 2 - 2 * krf * rc)
-        elif it.kind in (o.COULOMB, o.EWALD_REAL) and it.cutoff_kind == o.CUT_DISTANCE:
-            b += it.coulomb_const * qmax * qmax / rc ** 2
-    return b
-
-
 def _pairwise_forces(s):
     """pairwise_forces_loop_gpu! seam only (mb_forces), whatever else the System carries."""
     fs = np.zeros((s.n, 3), s.dtype)
     mb.capi.check(s._L.mb_forces(s.engine(), s.coords.ctypes.data, fs.ctypes.data, None, 0))
     return fs
-
-
-def _check(sysd, mb_inters, o_inters, dtype, r_list=0.0, expect_path=None, label=""):
-    xin = sysd["coords"].astype(dtype)
-    sd = dict(sysd, coords=xin)
-    s = H.make_system(sd, mb_inters, dtype, r_list=r_list)
-    orc = H.make_oracle(sd, o_inters, dtype=np.float64)
-    f_ref, e_ref, vir_ref = orc.forces_allpairs(xin.astype(np.float64), virial=True)
-    f = mb.forces(s)
-    e = mb.potential_energy(s)
-    f2, vir = mb.forces_virial(s)
-    st = s.stats()
-    if expect_path is not None:
-        assert st["path"] == expect_path, st
-    fmax = np.abs(f_ref).max()
-    err = np.abs(f.astype(np.float64) - f_ref).max()
-    print(f"[{label}] n={sysd['n']} dtype={np.dtype(dtype).name} path={st['path']} bricks={st['n_bricks']} "
-          f"brick={st['brick_dims']} stride={st['list_stride']} maxnb={st['max_neighbors']} halo={st['max_halo']} "
-          f"max|dF|={err:.3e} (max|F|={fmax:.3e}) dE={e - e_ref:.3e} (E={e_ref:.6e})")
-    vtol = (1e-9 if np.dtype(dtype) == np.float64 else 1e-4) * max(np.abs(vir_ref).max(), 1.0)
-    verr = np.abs(vir.astype(np.float64) - vir_ref).max()
-    ferr2 = np.abs(f2.astype(np.float64) - f.astype(np.float64)).max()
-    print(f"    virial err={verr:.3e} (tol {vtol:.3e}) |f(force-only) - f(force+virial)|={ferr2:.3e} repeat-equal={np.array_equal(f, mb.forces(s))}")
-    if np.dtype(dtype) == np.float32 and err > _tol(dtype, fmax):
-        # pairs sitting on the cutoff within f32 rounding may land on either side: allow one F(rc) jump each
-        nb_pairs = _boundary_atoms(orc, xin.astype(np.float64), o_inters)
-        fc = _cutoff_force_bound(sysd, o_inters)
-        per_atom = np.abs(f.astype(np.float64) - f_ref).max(axis=1)
-        allowed = _tol(dtype, fmax) + nb_pairs * fc
-        print(f"    cutoff-boundary atoms: {int((nb_pairs > 0).sum())}; atoms over the plain tolerance: "
-              f"{int((per_atom > _tol(dtype, fmax)).sum())}; F(rc) bound {fc:.3f}; "
-              f"max err off-boundary={per_atom[nb_pairs == 0].max():.3e}")
-        assert (per_atom <= allowed).all()
-    else:
-        assert err <= _tol(dtype, fmax)
-    assert abs(e - e_ref) <= _etol(dtype, e_ref)
-    assert np.array_equal(f, mb.forces(s))  # deterministic: same kernel, no atomics
-    assert ferr2 <= _tol(dtype, fmax)       # the energy/virial variant may contract FMAs differently
-    assert verr <= vtol
-    s.close()
-    return f, e
 
 
 # ---------------------------------------------------------------------------------------------------
@@ -134,80 +48,14 @@ def test_pair_known_answers_through_abi():
     assert f == 0.0 and e == 0.0
 
 
-@pytest.mark.parametrize("dtype", [np.float64, np.float32])
-def test_readme_system_allpairs(dtype):
-    sd = H.readme_system(100, 2.0, seed=1)
-    _check(sd, (mb.LennardJones(),), [o.Inter(o.LJ)], dtype, expect_path=0, label="C1 readme")
-
-
-@pytest.mark.parametrize("dtype", [np.float64, np.float32])
-@pytest.mark.parametrize("cut", ["distance", "shifted_potential", "shifted_force"])
-def test_molecular_allpairs_exceptions(dtype, cut):
-    # box smaller than 2.5 r_list -> the all-pairs kernel serves neighbour-list interactions (exclusions apply)
-    sd = H.molecular_system(150, [3.0, 3.2, 3.4], seed=11)
-    mcut = {"distance": mb.DistanceCutoff, "shifted_potential": mb.ShiftedPotentialCutoff,
-            "shifted_force": mb.ShiftedForceCutoff}[cut](1.2)
-    ocut = {"distance": o.CUT_DISTANCE, "shifted_potential": o.CUT_SHIFTED_POTENTIAL,
-            "shifted_force": o.CUT_SHIFTED_FORCE}[cut]
-    _check(sd, (mb.LennardJones(cutoff=mcut, weight_special=0.5, use_neighbors=True),
-                mb.Coulomb(cutoff=mcut, weight_special=0.8333, use_neighbors=True)),
-           [o.Inter(o.LJ, ocut, 1.2, weight_special=0.5, use_neighbors=True),
-            o.Inter(o.COULOMB, ocut, 1.2, weight_special=0.8333, use_neighbors=True)],
-           dtype, r_list=1.3, expect_path=0, label=f"molecular all-pairs {cut}")
-
-
-@pytest.mark.parametrize("dtype", [np.float64, np.float32])
-def test_mixed_nl_and_nonl_interactions(dtype):
-    """use_neighbors=false interactions ignore the exclusion / special masks (src/force.jl:828-855):
-    LJ through the list (with exclusions), Coulomb over all pairs (without)."""
-    sd = H.molecular_system(150, [3.0, 3.2, 3.4], seed=13)
-    sd = dict(sd, charge=sd["charge"] * 0.1)
-    _check(sd, (mb.LennardJones(cutoff=mb.DistanceCutoff(1.2), weight_special=0.5, use_neighbors=True),
-                mb.Coulomb(cutoff=mb.DistanceCutoff(1.2), weight_special=0.8333, use_neighbors=False)),
-           [o.Inter(o.LJ, o.CUT_DISTANCE, 1.2, weight_special=0.5, use_neighbors=True),
-            o.Inter(o.COULOMB, o.CUT_DISTANCE, 1.2, weight_special=0.8333, use_neighbors=False)],
-           dtype, r_list=1.3, expect_path=0, label="mixed nl/non-nl")
-
-
 # ---------------------------------------------------------------------------------------------------
 # brick / neighbour-list path
 # ---------------------------------------------------------------------------------------------------
 @pytest.mark.parametrize("dtype", [np.float64, np.float32])
-@pytest.mark.parametrize("cells", [6, 9])
-def test_lj_fluid_brick_path(dtype, cells):
-    sd = H.lj_fluid(cells, seed=42, dtype=np.float64)  # 864 / 2916 atoms at the C2 density, rc 1.2 nm
-    rc = 1.2 if cells >= 9 else 0.9
-    _check(sd, (mb.LennardJones(cutoff=mb.DistanceCutoff(rc), use_neighbors=True),),
-           [o.Inter(o.LJ, o.CUT_DISTANCE, rc, use_neighbors=True)], dtype, r_list=rc + 0.1, expect_path=1,
-           label=f"LJ fluid {cells}")
-
-
-@pytest.mark.parametrize("dtype", [np.float64, np.float32])
 def test_lj_fluid_16k(dtype):
     sd = H.lj_fluid(16, seed=42, dtype=np.float64)  # 16384 atoms, box 9.19 nm
-    _check(sd, (mb.LennardJones(cutoff=mb.DistanceCutoff(1.2), use_neighbors=True),),
-           [o.Inter(o.LJ, o.CUT_DISTANCE, 1.2, use_neighbors=True)], dtype, r_list=1.3, expect_path=1, label="LJ 16k")
-
-
-@pytest.mark.parametrize("dtype", [np.float64, np.float32])
-@pytest.mark.parametrize("coul", ["crf", "coulomb_sf", "ewald", "ewald_approx"])
-def test_molecular_brick_path(dtype, coul):
-    sd = H.molecular_system(1000, [5.1, 5.4, 5.8], seed=5)  # 4000 atoms, orthorhombic, mixed types, charges
-    lj_m = mb.LennardJones(cutoff=mb.DistanceCutoff(1.0), use_neighbors=True, weight_special=0.5)
-    lj_o = o.Inter(o.LJ, o.CUT_DISTANCE, 1.0, weight_special=0.5, use_neighbors=True)
-    if coul == "crf":
-        c_m = mb.CoulombReactionField(dist_cutoff=1.0, use_neighbors=True, weight_special=0.8333)
-        c_o = o.Inter(o.CRF, o.CUT_DISTANCE, 1.0, weight_special=0.8333, use_neighbors=True)
-    elif coul == "coulomb_sf":
-        c_m = mb.Coulomb(cutoff=mb.ShiftedForceCutoff(1.0), use_neighbors=True, weight_special=0.8333)
-        c_o = o.Inter(o.COULOMB, o.CUT_SHIFTED_FORCE, 1.0, weight_special=0.8333, use_neighbors=True)
-    else:
-        approx = coul == "ewald_approx"  # approximate_erfc=true is the reference's default (coulomb.jl:1331)
-        c_m = mb.CoulombEwald(dist_cutoff=1.0, use_neighbors=True, weight_special=0.8333, approximate_erfc=approx)
-        alpha = float(np.sqrt(-np.log(2 * 5e-4)) / 1.0)
-        c_o = o.Inter(o.EWALD_REAL, o.CUT_DISTANCE, 1.0, weight_special=0.8333, ewald_alpha=alpha, use_neighbors=True,
-                      approx_erfc=approx)
-    _check(sd, (lj_m, c_m), [lj_o, c_o], dtype, r_list=1.1, expect_path=1, label=f"molecular brick {coul}")
+    H.check(sd, (mb.LennardJones(cutoff=mb.DistanceCutoff(1.2), use_neighbors=True),),
+             [o.Inter(o.LJ, o.CUT_DISTANCE, 1.2, use_neighbors=True)], dtype, r_list=1.3, expect_path=1, label="LJ 16k")
 
 
 @pytest.mark.parametrize("name", ["lj_only", "coul_only"])
@@ -251,11 +99,11 @@ def test_6mrr_f32_vs_oracle(golden_6mrr):
     x = (g["coords"] - np.floor(g["coords"] / box) * box).astype(np.float32)
     sd = dict(n=len(x), box=box, coords=x, velocities=g["velocities_300K"], mass=g["mass"], charge=g["charge"],
               sigma=g["sigma"], eps=g["eps"], excluded=g["excluded"], special=g["special"])
-    _check(sd, (mb.LennardJones(cutoff=mb.DistanceCutoff(1.0), use_neighbors=True, weight_special=0.5),
-                mb.CoulombReactionField(dist_cutoff=1.0, use_neighbors=True, weight_special=float(g["coulomb14scale"]))),
-           [o.Inter(o.LJ, o.CUT_DISTANCE, 1.0, weight_special=0.5, use_neighbors=True),
-            o.Inter(o.CRF, o.CUT_DISTANCE, 1.0, weight_special=float(g["coulomb14scale"]), use_neighbors=True)],
-           np.float32, r_list=1.15, expect_path=1, label="6mrr LJ+CRF f32")
+    H.check(sd, (mb.LennardJones(cutoff=mb.DistanceCutoff(1.0), use_neighbors=True, weight_special=0.5),
+                 mb.CoulombReactionField(dist_cutoff=1.0, use_neighbors=True, weight_special=float(g["coulomb14scale"]))),
+            [o.Inter(o.LJ, o.CUT_DISTANCE, 1.0, weight_special=0.5, use_neighbors=True),
+             o.Inter(o.CRF, o.CUT_DISTANCE, 1.0, weight_special=float(g["coulomb14scale"]), use_neighbors=True)],
+            np.float32, r_list=1.15, expect_path=1, label="6mrr LJ+CRF f32")
 
 
 def test_forces_track_moving_coordinates_and_rebuild():
@@ -561,12 +409,12 @@ def _full_size_vs_oracle(cells, label):
     extra = nl[~np.isin(key(nl), key(lo))]
     np.add.at(on_cut, extra[:, 0], 1)
     np.add.at(on_cut, extra[:, 1], 1)
-    fc = _cutoff_force_bound(sd, o_inters)
+    fc = H.cutoff_force_bound(sd, o_inters)
     print(f"[{label}] n={sd['n']} bricks={st['n_bricks']} brick={st['brick_dims']} in-cutoff pairs={len(lo)} "
           f"max|dF|={per_atom.max():.3e} (max|F|={fmax:.3e}) pairs on the cutoff={len(extra)} F(rc)={fc:.3e} "
           f"dE/E={(e - e_ref) / abs(e_ref):.3e}")
-    assert (per_atom <= _tol(np.float32, fmax) + on_cut * fc).all()
-    assert abs(e - e_ref) <= _etol(np.float32, e_ref)
+    assert (per_atom <= H.tol(np.float32, fmax) + on_cut * fc).all()
+    assert abs(e - e_ref) <= H.etol(np.float32, e_ref)
     assert np.array_equal(f, mb.forces(s))
     return sd, s, orc
 
@@ -660,26 +508,6 @@ def test_two_point_cutoff_literals_through_abi():
             assert abs(f + f0) < 50 * tol and abs(e - e0) < 50 * tol
     with pytest.raises(ValueError):
         mb.CubicSplineCutoff(0.8, 0.6)
-
-
-@pytest.mark.parametrize("dtype", [np.float64, np.float32])
-@pytest.mark.parametrize("cut", ["cubic_spline", "polynomial"])
-def test_two_point_cutoffs_brick_and_allpairs(dtype, cut):
-    """CubicSpline / Polynomial cutoffs on LJ + Coulomb through both kernels vs the oracle
-    (exercised by the reference in test/simulation.jl:565-572, test/energy_conservation.jl:21-26)."""
-    mcut = {"cubic_spline": mb.CubicSplineCutoff, "polynomial": mb.PolynomialCutoff}[cut](0.8, 1.0)
-    ocut = {"cubic_spline": o.CUT_CUBIC_SPLINE, "polynomial": o.CUT_POLYNOMIAL}[cut]
-    mi = (mb.LennardJones(cutoff=mcut, weight_special=0.5, use_neighbors=True),
-          mb.Coulomb(cutoff=mcut, weight_special=0.8333, use_neighbors=True))
-    oi = [o.Inter(o.LJ, ocut, 1.0, r_act=0.8, weight_special=0.5, use_neighbors=True),
-          o.Inter(o.COULOMB, ocut, 1.0, r_act=0.8, weight_special=0.8333, use_neighbors=True)]
-    sd = H.molecular_system(1000, [5.1, 5.4, 5.8], seed=5)
-    _check(sd, mi, oi, dtype, r_list=1.1, expect_path=1, label=f"molecular brick {cut}")
-    sd = H.molecular_system(150, [3.0, 3.2, 3.4], seed=11)
-    _check(sd, mi, oi, dtype, r_list=1.25, expect_path=0, label=f"molecular all-pairs {cut}")  # 3.0 nm < 2.5 r_list: no-list kernel
-    sd = H.lj_fluid(9, seed=42, dtype=np.float64)
-    _check(sd, (mb.LennardJones(cutoff=mcut, use_neighbors=True),), [o.Inter(o.LJ, ocut, 1.0, r_act=0.8, use_neighbors=True)],
-           dtype, r_list=1.1, expect_path=1, label=f"LJ fluid {cut} (uniform)")
 
 
 # ---------------------------------------------------------------------------------------------------

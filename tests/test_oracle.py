@@ -54,6 +54,14 @@ def test_mixing_rules():
     x = np.array([[1.0, 1, 1], [1.0 + 0.25 * 2 ** (1 / 6), 1, 1]])  # minimum: E = -eps_mixed
     _, pe, _ = s.forces_allpairs(x, n_threads=1)
     assert abs(pe + 0.14142135623730953) < 1e-12
+    # geometric sigma of (0.2, 0.3) = sqrt(0.06) = 0.2449489742783178 (test/interactions.jl:17)
+    s = o.OracleSystem(box=[5.0] * 3, mass=[1, 1], charge=[0, 0], sigma=[0.2, 0.3], eps=[0.1, 0.2],
+                       inters=[o.Inter(o.LJ, sigma_mix=o.MIX_GEOMETRIC)])
+    sig = 0.2449489742783178
+    _, pe, _ = s.forces_allpairs(np.array([[1.0, 1, 1], [1.0 + sig, 1, 1]]), n_threads=1)
+    assert abs(pe) < 1e-12
+    f, pe, _ = s.forces_allpairs(np.array([[1.0, 1, 1], [1.0 + sig * 2 ** (1 / 6), 1, 1]]), n_threads=1)
+    assert abs(pe + 0.14142135623730953) < 1e-12 and np.abs(f).max() < 1e-9
 
 
 def test_crf_behaviour():
