@@ -194,10 +194,9 @@ __global__ void __launch_bounds__(BONDED_THREADS)
 
 // pe_partial[0..n) summed in index order -> *acc += sum (one CTA of SUM_THREADS)
 __global__ void sum_partials_kernel(int n, const double* __restrict__ partial, double* acc) {
-    double v = 0;
-    for (int i = threadIdx.x; i < n; i += blockDim.x) v += partial[i];
-    v = block_sum<SUM_THREADS>(v);
-    if (threadIdx.x == 0) *acc += v;
+    double v[1];
+    sum_partials<SUM_THREADS, 1>(partial, n, v);
+    if (threadIdx.x == 0) *acc += v[0];
 }
 
 template <typename T>

@@ -50,15 +50,25 @@ struct Control {
     unsigned int call_max_disp2_bits;  // largest value any rebuild interval of the current call reached
 };
 
-// centre-of-mass velocity waiting to be subtracted by the next reader of the velocities (vv.cuh; written by K2's last CTA
-// or by the force kernel's fused second kick), and the velocity-rescaling thermostat's factor: the next reader applies
-// v <- lam (v - v_cm), each part when its flag is set
+// centre-of-mass velocity waiting to be subtracted by the next reader of the velocities (vv.cuh; published by the last CTA
+// of K2, the Langevin step or NH2, or by the decomposed runs' v_cm kernels), and the velocity-rescaling thermostat's factor:
+// the next reader applies v <- lam (v - v_cm), each part when its flag is set
 template <typename T>
 struct CmState {
     T v[3];
     int valid;
     T lam;
     int scaled;
+    // v_cm = s / M from the momentum sum s = sum(m v) and inv_mass = 1 / M
+    __device__ __forceinline__ void publish(const double s[3], double inv_mass) {
+        for (int k = 0; k < 3; k++) v[k] = (T)(s[k] * inv_mass);
+        valid = 1;
+    }
+    // the pending state applied to one velocity
+    __device__ __forceinline__ void apply(typename VT<T>::T4& u) const {
+        if (valid) { u.x -= v[0]; u.y -= v[1]; u.z -= v[2]; }
+        if (scaled) { u.x *= lam; u.y *= lam; u.z *= lam; }
+    }
 };
 
 struct BrickHdr {

@@ -201,10 +201,12 @@ __device__ __forceinline__ double block_sum(double v) {
 }
 
 // True in every thread of the CTA that takes the last of gridDim.x tickets (atomicInc wraps *ticket back to 0 for the next
-// launch). Thread 0 fences before it takes the ticket: its own global stores, and those that a barrier ordered before it, are
-// visible to the last CTA, which fences again before it reads them.
+// launch). It opens with a CTA barrier, so every thread of the CTA has finished its loads and stores before the CTA takes its
+// ticket: the last CTA may overwrite what the other CTAs read (v_cm, the step counter, zeta), and the global stores of every
+// thread are ordered before thread 0's fence, hence visible to the last CTA, which fences again before it reads them.
 __device__ __forceinline__ bool last_cta(unsigned int* ticket) {
     __shared__ bool s_last;
+    __syncthreads();
     if (threadIdx.x == 0) {
         __threadfence();
         const unsigned int t = atomicInc(ticket, gridDim.x - 1);
@@ -212,6 +214,34 @@ __device__ __forceinline__ bool last_cta(unsigned int* ticket) {
     }
     __syncthreads();
     return s_last;
+}
+
+// s = partial[0..n) of width W (W doubles per entry, component k at W i + k) summed per component in index order by one CTA
+// of NT threads: thread t adds entries t, t + NT, ... in turn, then block_sum. The result is valid in thread 0 only; block_sum's
+// rule on its scratch applies.
+template <int NT, int W>
+__device__ __forceinline__ void sum_partials(const double* __restrict__ partial, int n, double (&s)[W]) {
+#pragma unroll
+    for (int k = 0; k < W; k++) s[k] = 0;
+    for (int i = threadIdx.x; i < n; i += NT)
+#pragma unroll
+        for (int k = 0; k < W; k++) s[k] += partial[W * (size_t)i + k];
+    block_sum<NT, W>(s);
+}
+
+// v[0..W) of every thread summed over the grid, each component on its own and with the same bits on every run: each CTA's
+// block_sum goes to partial[W blockIdx.x + k] (W gridDim.x doubles), and the CTA that takes the last ticket adds them in
+// index order (sum_partials). Returns true in every thread of that CTA, with the totals in v of thread 0; false elsewhere.
+template <int NT, int W>
+__device__ __forceinline__ bool grid_sum(double (&v)[W], double* __restrict__ partial, unsigned int* ticket) {
+    block_sum<NT, W>(v);
+    if (threadIdx.x == 0)
+#pragma unroll
+        for (int k = 0; k < W; k++) partial[W * (size_t)blockIdx.x + k] = v[k];
+    if (!last_cta(ticket)) return false;
+    __threadfence();
+    sum_partials<NT, W>(partial, gridDim.x, v);  // (last_cta's barriers lie between block_sum's two uses of its scratch)
+    return true;
 }
 
 // ---------------------------------------------------------------------------------------------
@@ -236,8 +266,8 @@ __host__ __device__ inline void philox4x32_10(uint32_t c[4], uint32_t k0, uint32
 }
 // Three N(0, sd^2) draws from one Philox block d by Box-Muller: (sd r1 cos 2 pi u2, sd r1 sin 2 pi u2, sd r2 cos 2 pi u4) with
 // r1, r2 = sqrt(-2 log u1), sqrt(-2 log u3), u1, u3 = (d[0] + 1) / 2^32, (d[2] + 1) / 2^32 in (0, 1] (log stays finite) and
-// u2, u4 = d[1] / 2^32, d[3] / 2^32 in [0, 1). The Langevin integrator's O step; the same transform as the Andersen
-// thermostat's resampling (andersen_apply keeps its own copy of these lines: calling this helper changes its SASS).
+// u2, u4 = d[1] / 2^32, d[3] / 2^32 in [0, 1). The Langevin integrator's O step, the Andersen thermostat's resampling and
+// random_velocities.
 __host__ __device__ __forceinline__ void box_muller3(const uint32_t d[4], double sd, double out[3]) {
     const double two_pi = 6.283185307179586;
     const double u1 = ((double)d[0] + 1.0) * (1.0 / 4294967296.0), u2 = (double)d[1] * (1.0 / 4294967296.0);

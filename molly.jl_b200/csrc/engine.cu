@@ -1725,6 +1725,17 @@ class Engine : public EngineBase {
         MB_CUDA(cudaStreamUpdateCaptureDependencies(stream_, &cnode, 1, cudaStreamSetCaptureDependencies));
         return MB_OK;
     }
+    // The grid of an integration pass (K1, K2, the Langevin step, NH1, NH2) over n atoms: CTAs of VV_THREADS threads with
+    // per_thread atoms each, at most per_sm CTAs per SM. The grid decides how grid_sum groups the sums, so a pass keeps its
+    // grid from one release to the next. Each CTA writes `width` doubles to d_partial_, which is checked to hold them.
+    int integ_grid(int& grid, int n, int per_thread, int per_sm, int width) {
+        const int per_cta = per_thread * VV_THREADS;
+        grid = std::max(1, std::min((n + per_cta - 1) / per_cta, per_sm * sm_count_));
+        if ((size_t)grid * width * sizeof(double) > d_partial_.bytes)
+            return set_error(MB_ERR_STATE, "integration pass of " + std::to_string(grid) + " CTAs x " + std::to_string(width) +
+                                               " doubles overruns the partial-sum buffer");
+        return MB_OK;
+    }
     int enqueue_step(const StepCfg& c, const StepOpts& o, Capture* cap = nullptr) {
         const bool dec = decomposed() && path_ == 1;
         const int s0 = dec ? own_s0_ : 0, n_own = dec ? own_n_ : (int)n_;
@@ -1745,26 +1756,25 @@ class Engine : public EngineBase {
             cm_deferred_epoch_ = 0;
         }
         prof_.begin(Prof::VV);
-        if (c.integrator == INTEG_LANGEVIN) {
-            // (single GPU: s0 = 0.) At most vvb CTAs, so d_partial_ (max(vvb, 2048) x 8 doubles, prepare) holds their 3 each
-            const int lgb = std::max(1, std::min(nb, 8 * sm_count_));
-            langevin_step_kernel<T><<<lgb, VV_THREADS, 0, stream_>>>(
+        int grid;
+        if (c.integrator == INTEG_LANGEVIN) {  // (single GPU: s0 = 0)
+            MB_TRY(integ_grid(grid, n_own, 1, 8, 3));
+            langevin_step_kernel<T><<<grid, VV_THREADS, 0, stream_>>>(
                 n_own, c.dt, c.dt_half, c.skin_half2, c.lc, o.do_cm, c.inv_mass, cm, d_f4_.as<T4>(), d_xref4_.as<T4>(),
                 d_pos4_.as<T4>(), d_vel4_.as<T4>(), d_orig_.as<int>(), d_mass_.as<T>(), d_partial_.as<double>(), c.flag_ptr, ctl,
                 cap ? cap->rebuild : 0, cap && path_ == 1 ? 1 : 0, ext_map());
-        } else if (c.integrator == INTEG_NH) {
-            // (single GPU: s0 = 0.) At most vvb CTAs, so d_partial_ holds their 2 each
-            const int nhb = std::max(1, std::min(nb, 8 * sm_count_));
-            nh_kick_drift_kernel<T><<<nhb, VV_THREADS, 0, stream_>>>(
+        } else if (c.integrator == INTEG_NH) {  // (single GPU: s0 = 0)
+            MB_TRY(integ_grid(grid, n_own, 1, 8, 2));
+            nh_kick_drift_kernel<T><<<grid, VV_THREADS, 0, stream_>>>(
                 n_own, c.dt, c.dt_half, c.skin_half2, c.nc, d_nh_.as<NhState>(), cm, d_f4_.as<T4>(), d_xref4_.as<T4>(),
                 d_pos4_.as<T4>(), d_vel4_.as<T4>(), d_mass_.as<T>(), d_partial_.as<double>(), c.flag_ptr, ctl,
                 cap ? cap->rebuild : 0, cap && path_ == 1 ? 1 : 0, ext_map());
         } else {
             const Thermo<T> th = thermo_in_k1(c);
             const int thk = th.on ? TH_ANDERSEN : (c.vc.kind != VC_NONE ? TH_SCALE : TH_NONE);
+            MB_TRY(integ_grid(grid, n_own, 2, 5, 0));  // two atoms per thread, one wave (48 registers: 5 CTAs per SM)
             with_const<TH_NONE, TH_ANDERSEN, TH_SCALE>(thk, [&](auto TH) {
-                // two atoms per thread, one wave (48 registers: 5 CTAs per SM)
-                vv_kick_drift_kernel<T, TH><<<std::max(1, std::min((nb + 1) / 2, 5 * sm_count_)), 256, 0, stream_>>>(
+                vv_kick_drift_kernel<T, TH><<<grid, VV_THREADS, 0, stream_>>>(
                     s0, n_own, c.dt, c.dt_half, c.skin_half2, cm, d_f4_.as<T4>(), d_xref4_.as<T4>(), d_pos4_.as<T4>(), d_vel4_.as<T4>(),
                     c.flag_ptr, ctl, cap ? cap->rebuild : 0, cap && path_ == 1 ? 1 : 0, push, ext_map(), th);
             });
@@ -1798,7 +1808,6 @@ class Engine : public EngineBase {
         }
         const int s0b = dec ? own_s0_ : 0, n_ownb = dec ? own_n_ : (int)n_;  // ownership may have changed in the rebuild
         const int nb2 = std::max(1, (n_ownb + 255) / 256);
-        const int vvb2 = std::max(1, std::min((n_ownb + 2 * VV_THREADS - 1) / (2 * VV_THREADS), 8 * sm_count_));
         MB_TRY(launch_pairs(false, d_f4_.as<T4>(), dec));
         MB_TRY(launch_bonded(false));
         if (c.integrator == INTEG_LANGEVIN) {  // these forces are the next step's kick: the step ends here
@@ -1807,9 +1816,9 @@ class Engine : public EngineBase {
             return MB_OK;
         }
         if (c.integrator == INTEG_NH) {
-            const int nhb2 = std::max(1, std::min(nb2, 8 * sm_count_));
+            MB_TRY(integ_grid(grid, n_ownb, 1, 8, 3));
             prof_.begin(Prof::VV);
-            nh_kick2_kernel<T><<<nhb2, VV_THREADS, 0, stream_>>>(n_ownb, c.dt_half, o.do_cm, c.inv_mass, d_nh_.as<NhState>(),
+            nh_kick2_kernel<T><<<grid, VV_THREADS, 0, stream_>>>(n_ownb, c.dt_half, o.do_cm, c.inv_mass, d_nh_.as<NhState>(),
                                                                  d_f4_.as<T4>(), d_mass_.as<T>(), d_vel4_.as<T4>(),
                                                                  d_partial_.as<double>(), ctl, cm);
             prof_.end(Prof::VV);
@@ -1822,10 +1831,11 @@ class Engine : public EngineBase {
         PeerSignal sig;
         memset(&sig, 0, sizeof(sig));
         if (p2p_sig) sig = make_signal(epoch, o.do_cm != 0);
+        MB_TRY(integ_grid(grid, n_ownb, 2, 8, c.vc.kind != VC_NONE ? 4 : 3));
         prof_.begin(Prof::VV);
         with_const<true, false>(c.vc.kind != VC_NONE, [&](auto CP) {
-            vv_kick2_kernel<T, CP><<<vvb2, VV_THREADS, 0, stream_>>>(s0b, n_ownb, c.dt_half, o.do_cm, c.inv_mass, d_f4_.as<T4>(),
-                                                                     d_mass_.as<T>(), d_vel4_.as<T4>(), d_partial_.as<double>(), ctl, cm, 0,
+            vv_kick2_kernel<T, CP><<<grid, VV_THREADS, 0, stream_>>>(s0b, n_ownb, c.dt_half, o.do_cm, c.inv_mass, d_f4_.as<T4>(),
+                                                                     d_mass_.as<T>(), d_vel4_.as<T4>(), d_partial_.as<double>(), ctl, cm,
                                                                      dec ? d_mom_.as<double>() : nullptr, sig, c.vc);
         });
         prof_.end(Prof::VV);
@@ -2088,9 +2098,6 @@ class Engine : public EngineBase {
             if (!(std::isfinite(lg->kT) && lg->kT >= 0)) return set_error(MB_ERR_INVALID, "mb_simulate_langevin: kT must be finite and >= 0");
             if (!(std::isfinite(lg->friction) && lg->friction >= 0))
                 return set_error(MB_ERR_INVALID, "mb_simulate_langevin: friction must be finite and >= 0");
-            if (vcoupling.kind != MB_VC_NONE)
-                return set_error(MB_ERR_INVALID, "mb_simulate_langevin: a velocity coupling is set on the context (couplings with Langevin are not supported)");
-            if (decomposed()) return set_error(MB_ERR_INVALID, "mb_simulate_langevin: not available in decomposed (multi-GPU) runs");
         }
         if (nh) {
             // (kT = 0 would make T / T0 infinite)
@@ -2098,9 +2105,13 @@ class Engine : public EngineBase {
             if (!(std::isfinite(nh->damping) && nh->damping > 0))
                 return set_error(MB_ERR_INVALID, "mb_simulate_nose_hoover: damping must be finite and > 0");
             if (n_ < 2) return set_error(MB_ERR_INVALID, "mb_simulate_nose_hoover: needs at least 2 atoms (Nf = 3N - 3 > 0)");
+        }
+        if (lg || nh) {
+            const std::string who = lg ? "mb_simulate_langevin" : "mb_simulate_nose_hoover";
             if (vcoupling.kind != MB_VC_NONE)
-                return set_error(MB_ERR_INVALID, "mb_simulate_nose_hoover: a velocity coupling is set on the context (couplings with Nose-Hoover are not supported)");
-            if (decomposed()) return set_error(MB_ERR_INVALID, "mb_simulate_nose_hoover: not available in decomposed (multi-GPU) runs");
+                return set_error(MB_ERR_INVALID, who + ": a velocity coupling is set on the context (couplings with " +
+                                                     (lg ? "Langevin" : "Nose-Hoover") + " are not supported)");
+            if (decomposed()) return set_error(MB_ERR_INVALID, who + ": not available in decomposed (multi-GPU) runs");
         }
         if (vcoupling.kind != MB_VC_NONE) {
             if (p->andersen_kT > 0 && p->andersen_prob > 0)
@@ -2114,7 +2125,6 @@ class Engine : public EngineBase {
         MB_TRY(caller_xyz(coords, d_stage_a_, true, xb));
         MB_TRY(caller_xyz(vels, d_stage_c_, true, vb));
         const int nb = (int)((n_ + 255) / 256);
-        const int vvb = std::min((int)((n_ + VV_THREADS - 1) / VV_THREADS), 8 * sm_count_);
         Control* ctl = d_ctl_.as<Control>();
         CmState<T>* cm = d_cm_.as<CmState<T>>();
         clear_cm_kernel<T><<<1, 1, 0, stream_>>>(cm);
@@ -2175,9 +2185,11 @@ class Engine : public EngineBase {
         bool cm_pending = false;  // host mirror of cm->valid
         if (p->init_step == 0 && p->remove_cm_every != 0) {
             // remove_CM_motion! before the first force evaluation (simulators.jl:563): zero-length kick
-            vv_kick2_kernel<T, false><<<vvb, VV_THREADS, 0, stream_>>>(0, (int)n_, (T)0, 1, c.inv_mass, d_f4_.as<T4>(), d_mass_.as<T>(),
-                                                                       d_vel4_.as<T4>(), d_partial_.as<double>(), ctl, cm, 0, nullptr,
-                                                                       PeerSignal{}, VCouple{});
+            int grid;
+            MB_TRY(integ_grid(grid, (int)n_, 1, 8, 3));
+            vv_kick2_kernel<T, false><<<grid, VV_THREADS, 0, stream_>>>(0, (int)n_, (T)0, 1, c.inv_mass, d_f4_.as<T4>(), d_mass_.as<T>(),
+                                                                        d_vel4_.as<T4>(), d_partial_.as<double>(), ctl, cm, nullptr,
+                                                                        PeerSignal{}, VCouple{});
             launches_++;
             cm_pending = true;
         }
@@ -2207,7 +2219,7 @@ class Engine : public EngineBase {
         }
 
         // CUDA-graph path: static per-step sequence (remove_CM_motion in {0,1})
-        bool use_graph = graphs_usable() && c.do_cm >= 0 && p->n_steps >= 4 && !(cm_pending && c.do_cm == 0) &&
+        bool use_graph = graphs_usable() && c.do_cm >= 0 && p->n_steps >= 4 &&
                          !dec;  // the decomposed step issues NCCL calls with per-rebuild sizes
         if (use_graph) {
             // one executable per log mask this call uses (the plain step and the log steps)

@@ -16,8 +16,9 @@ struct LangevinCoef {
 
 // O step draws: Philox4x32-10 with counter (original atom index + 1, step, ctr1_lo, ctr1_hi) and key (key_lo, key_hi), one
 // block per atom and step, Box-Muller of its four words (box_muller3). A function of (keys, step, atom) only.
-// When do_cm, every CTA writes its partial sum(m v) of the new velocities (K2's layout, 3 doubles per CTA) and the last CTA
-// publishes v_cm = sum(m v) / sum(m) in index order; otherwise it marks v_cm as consumed.
+// When do_cm, sum(m v) of the new velocities goes through grid_sum and the last CTA publishes v_cm = sum(m v) / sum(m);
+// otherwise the last CTA marks v_cm as consumed. The pending v_cm and the step counter read below are overwritten by the last
+// CTA of this same launch (last_cta orders every CTA's reads before its ticket).
 template <typename T>
 __global__ void __launch_bounds__(VV_THREADS)
     langevin_step_kernel(int n, T dt, T dt_half, T skin_half2, LangevinCoef lc, int do_cm, double inv_total_mass,
@@ -25,9 +26,6 @@ __global__ void __launch_bounds__(VV_THREADS)
                          typename VT<T>::T4* __restrict__ pos4, typename VT<T>::T4* __restrict__ vel4, const int* __restrict__ orig,
                          const T* __restrict__ mass, double* __restrict__ partial, int* __restrict__ flag, Control* __restrict__ ctl,
                          cudaGraphConditionalHandle handle, int use_handle, ExtMap<T> ext) {
-    // The pending v_cm and the step counter are read here and overwritten by the last CTA of this same launch. That is safe
-    // without a second kernel: every thread reads them before the CTA barrier ahead of last_cta, the CTA takes its ticket after
-    // that barrier, and the last CTA writes only once it holds the last ticket, i.e. after every CTA has finished reading.
     const bool cmv = cm->valid != 0;
     const T cx = cm->v[0], cy = cm->v[1], cz = cm->v[2];
     const uint32_t step_lo = (uint32_t)(ctl->step + 1);  // the step this launch takes
@@ -64,30 +62,11 @@ __global__ void __launch_bounds__(VV_THREADS)
             mv[0] += (double)(v.x * m); mv[1] += (double)(v.y * m); mv[2] += (double)(v.z * m);
         }
     }
-    if (do_cm) {
-        block_sum<VV_THREADS, 3>(mv);
-        if (threadIdx.x == 0)
-            for (int k = 0; k < 3; k++) partial[3 * (size_t)blockIdx.x + k] = mv[k];
-    }
     if (moved) *flag = 1;
-    __syncthreads();  // every thread of the CTA has read v_cm and the step counter (above) before the CTA takes its ticket
-    if (!last_cta(&ctl->ticket)) return;
-    if (threadIdx.x == 0) step_advance(ctl, handle, use_handle);
-    if (!do_cm) {
-        if (threadIdx.x == 0) cm->valid = 0;
-        return;
-    }
-    __threadfence();
-    double s[3] = {0, 0, 0};
-    for (int i = threadIdx.x; i < (int)gridDim.x; i += VV_THREADS)
-        for (int k = 0; k < 3; k++) s[k] += partial[3 * (size_t)i + k];
-    block_sum<VV_THREADS, 3>(s);  // (barriers lie between this and the first call's reads of the scratch)
-    if (threadIdx.x == 0) {
-        cm->v[0] = (T)(s[0] * inv_total_mass);
-        cm->v[1] = (T)(s[1] * inv_total_mass);
-        cm->v[2] = (T)(s[2] * inv_total_mass);
-        cm->valid = 1;
-    }
+    if (!(do_cm ? grid_sum<VV_THREADS, 3>(mv, partial, &ctl->ticket) : last_cta(&ctl->ticket)) || threadIdx.x != 0) return;
+    if (do_cm) cm->publish(mv, inv_total_mass);
+    else cm->valid = 0;
+    step_advance(ctl, handle, use_handle);  // (last: nothing stays live across its conditional-node call)
 }
 
 }  // namespace mb

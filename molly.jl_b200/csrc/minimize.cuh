@@ -63,7 +63,6 @@ __global__ void __launch_bounds__(SD_THREADS)
         }
     }
     if (moved) ctl->rebuild = 1;
-    __syncthreads();  // every thread's stores before the ticket
     if (last_cta(&ctl->ticket) && threadIdx.x == 0) {
         __threadfence();
         st->move_ok = ok ? 1 : 0;
@@ -71,16 +70,16 @@ __global__ void __launch_bounds__(SD_THREADS)
     }
 }
 
-// Energy of the trial positions (pair partials in index order with block_sum, then the specific terms and the constant),
+// Energy of the trial positions (pair partials in index order with sum_partials, then the specific terms and the constant),
 // the decision, the step-size update, the trace record and the continue flag. One CTA of SD_THREADS. init: the evaluation
 // at the starting coordinates (record 0 = (init_step, E0, NaN, 1)).
 __global__ void __launch_bounds__(SD_THREADS)
     sd_decide_kernel(SdState* __restrict__ st, const double* __restrict__ pe_partial, int n_pe, const double* __restrict__ sp_energy,
                      int init, cudaGraphConditionalHandle handle, int use_handle) {
-    double pe = 0;
-    for (int i = threadIdx.x; i < n_pe; i += SD_THREADS) pe += pe_partial[i];
-    pe = block_sum<SD_THREADS>(pe);
+    double s[1];
+    sum_partials<SD_THREADS, 1>(pe_partial, n_pe, s);
     if (threadIdx.x != 0) return;
+    double pe = s[0];
     if (sp_energy) pe += *sp_energy;
     pe += st->pe_const;
     const double nan = __longlong_as_double(0x7ff8000000000000ll);

@@ -29,9 +29,10 @@ __host__ __device__ inline double nh_zeta_step(double zeta, double mv2_old, doub
     return zeta_half + c.coef * (mv2_half / c.nf_kT - 1.0);
 }
 
-// NH1: one atom per thread (grid-stride). Every CTA writes its partial (sum m|v|^2, sum m|v_half|^2) as 2 doubles; the last
-// CTA adds them in index order, updates zeta and does the step bookkeeping (step_advance). Four CTAs per SM: left to itself,
-// ptxas squeezes the f32 instantiation into 48 registers and spills in the ghost-copy loop.
+// NH1: one atom per thread (grid-stride). (sum m|v|^2, sum m|v_half|^2) go through grid_sum; the last CTA updates zeta and does
+// the step bookkeeping (step_advance). zeta and the step counter read below are overwritten by that CTA (last_cta orders every
+// CTA's reads before its ticket). Four CTAs per SM: left to itself, ptxas squeezes the f32 instantiation into 48 registers and
+// spills in the ghost-copy loop.
 template <typename T>
 __global__ void __launch_bounds__(VV_THREADS, 4)
     nh_kick_drift_kernel(int n, T dt, T dt_half, T skin_half2, NhCoef nc, NhState* __restrict__ nh, const CmState<T>* cm,
@@ -39,9 +40,6 @@ __global__ void __launch_bounds__(VV_THREADS, 4)
                          typename VT<T>::T4* __restrict__ pos4, typename VT<T>::T4* __restrict__ vel4, const T* __restrict__ mass,
                          double* __restrict__ partial, int* __restrict__ flag, Control* __restrict__ ctl,
                          cudaGraphConditionalHandle handle, int use_handle, ExtMap<T> ext) {
-    // zeta and the step counter are read here and overwritten by the last CTA of this same launch. That is safe without a
-    // second kernel: every thread reads them before the CTA barrier ahead of last_cta, the CTA takes its ticket after that
-    // barrier, and the last CTA writes only once it holds the last ticket, i.e. after every CTA has finished reading.
     const double zeta = nh->zeta;
     const T z = (T)zeta;
     const bool cmv = cm->valid != 0;
@@ -69,24 +67,15 @@ __global__ void __launch_bounds__(VV_THREADS, 4)
         const T dx = p.x - r.x, dy = p.y - r.y, dz = p.z - r.z;
         moved |= (dx * dx + dy * dy + dz * dz > skin_half2);
     }
-    block_sum<VV_THREADS, 2>(k2);
-    if (threadIdx.x == 0) { partial[2 * (size_t)blockIdx.x] = k2[0]; partial[2 * (size_t)blockIdx.x + 1] = k2[1]; }
     if (moved) *flag = 1;
-    __syncthreads();  // every thread of the CTA has read zeta, v_cm and the step counter (above) before the CTA takes its ticket
-    if (!last_cta(&ctl->ticket)) return;
-    __threadfence();
-    double s[2] = {0, 0};
-    for (int i = threadIdx.x; i < (int)gridDim.x; i += VV_THREADS) { s[0] += partial[2 * (size_t)i]; s[1] += partial[2 * (size_t)i + 1]; }
-    block_sum<VV_THREADS, 2>(s);  // (barriers lie between this and the first call's reads of the scratch)
-    if (threadIdx.x == 0) {
-        nh->zeta = nh_zeta_step(zeta, s[0], s[1], nc);
-        step_advance(ctl, handle, use_handle);  // (last: nothing stays live across its conditional-node call)
-    }
+    if (!grid_sum<VV_THREADS, 2>(k2, partial, &ctl->ticket) || threadIdx.x != 0) return;
+    nh->zeta = nh_zeta_step(zeta, k2[0], k2[1], nc);
+    step_advance(ctl, handle, use_handle);  // (last: nothing stays live across its conditional-node call)
 }
 
-// NH2: one atom per thread (grid-stride). NH1 consumed the pending v_cm. When do_cm, every CTA writes its partial sum(m v)
-// (K2's layout, 3 doubles per CTA) and the last CTA publishes v_cm = sum(m v) / sum(m) in index order, applied lazily by the
-// next reader of the velocities; otherwise v_cm is marked consumed.
+// NH2: one atom per thread (grid-stride). NH1 consumed the pending v_cm. When do_cm, sum(m v) goes through grid_sum and the last
+// CTA publishes v_cm = sum(m v) / sum(m), applied lazily by the next reader of the velocities; otherwise v_cm is marked
+// consumed.
 template <typename T>
 __global__ void __launch_bounds__(VV_THREADS)
     nh_kick2_kernel(int n, T dt_half, int do_cm, double inv_total_mass, const NhState* __restrict__ nh,
@@ -111,21 +100,7 @@ __global__ void __launch_bounds__(VV_THREADS)
         if (blockIdx.x == 0 && threadIdx.x == 0) cm->valid = 0;
         return;
     }
-    block_sum<VV_THREADS, 3>(mv);
-    if (threadIdx.x == 0)
-        for (int k = 0; k < 3; k++) partial[3 * (size_t)blockIdx.x + k] = mv[k];
-    if (!last_cta(&ctl->ticket)) return;
-    __threadfence();
-    double s[3] = {0, 0, 0};
-    for (int i = threadIdx.x; i < (int)gridDim.x; i += VV_THREADS)
-        for (int k = 0; k < 3; k++) s[k] += partial[3 * (size_t)i + k];
-    block_sum<VV_THREADS, 3>(s);  // (barriers lie between this and the first call's reads of the scratch)
-    if (threadIdx.x == 0) {
-        cm->v[0] = (T)(s[0] * inv_total_mass);
-        cm->v[1] = (T)(s[1] * inv_total_mass);
-        cm->v[2] = (T)(s[2] * inv_total_mass);
-        cm->valid = 1;
-    }
+    if (grid_sum<VV_THREADS, 3>(mv, partial, &ctl->ticket) && threadIdx.x == 0) cm->publish(mv, inv_total_mass);
 }
 
 }  // namespace mb

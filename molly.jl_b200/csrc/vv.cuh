@@ -71,8 +71,7 @@ __global__ void ingest_kernel(int n, Geom<T> g, const T* __restrict__ coords, co
 }
 
 // ---- export: slot order -> original order, wrapped coordinates, pending CM velocity applied ----
-// position p wrapped into the box as export_kernel does it, stored at dst[0..2] (the logger's coordinate frames; export_kernel
-// keeps its own copy of these lines: calling this helper changes its SASS)
+// position p wrapped into the box, stored at dst[0..2] (exported coordinates and the logger's coordinate frames)
 template <typename T>
 __device__ __forceinline__ void store_wrapped(const Geom<T>& g, typename VT<T>::T4 p, T* dst) {
     T x[3] = {p.x, p.y, p.z};
@@ -96,26 +95,10 @@ __global__ void export_kernel(int n, Geom<T> g, const typename VT<T>::T4* __rest
     int s = blockIdx.x * blockDim.x + threadIdx.x;
     if (s >= n) return;
     int o = orig[s];
-    if (coords) {
-        typename VT<T>::T4 p = pos4[s];
-        T x[3] = {p.x, p.y, p.z};
-        if (g.tric.on) {
-            tric_wrap<T>(g.tric, x[0], x[1], x[2]);
-            for (int d = 0; d < 3; d++) coords[3 * (size_t)o + d] = x[d];
-        } else {
-#pragma unroll
-            for (int d = 0; d < 3; d++) {
-                T v = x[d] - ffloor(x[d] * g.invL[d]) * g.L[d];
-                if (v >= g.L[d]) v -= g.L[d];
-                if (v < (T)0) v = (T)0;
-                coords[3 * (size_t)o + d] = v;
-            }
-        }
-    }
+    if (coords) store_wrapped<T>(g, pos4[s], coords + 3 * (size_t)o);
     if (vels) {
         typename VT<T>::T4 v = vel4[s];
-        if (cm && cm->valid) { v.x -= cm->v[0]; v.y -= cm->v[1]; v.z -= cm->v[2]; }
-        if (cm && cm->scaled) { v.x *= cm->lam; v.y *= cm->lam; v.z *= cm->lam; }
+        if (cm) cm->apply(v);
         vels[3 * (size_t)o] = v.x;
         vels[3 * (size_t)o + 1] = v.y;
         vels[3 * (size_t)o + 2] = v.z;
@@ -173,14 +156,11 @@ __device__ __forceinline__ void andersen_apply(typename VT<T>::T4& v, int orig_i
     if (u < prob) {
         uint32_t d[4] = {(uint32_t)(orig_index + 1 + n), step_lo, ctr1_lo, ctr1_hi};
         philox4x32_10(d, key_lo, key_hi);
-        const double two_pi = 6.283185307179586;
-        double u1 = ((double)d[0] + 1.0) * (1.0 / 4294967296.0), u2 = (double)d[1] * (1.0 / 4294967296.0);
-        double u3 = ((double)d[2] + 1.0) * (1.0 / 4294967296.0), u4 = (double)d[3] * (1.0 / 4294967296.0);
-        double r1 = sqrt(-2.0 * log(u1)), r2 = sqrt(-2.0 * log(u3));
-        double sd = (m > (T)0) ? sqrt((double)kT / (double)m) : 0.0;
-        v.x = (T)(sd * r1 * cos(two_pi * u2));
-        v.y = (T)(sd * r1 * sin(two_pi * u2));
-        v.z = (T)(sd * r2 * cos(two_pi * u4));
+        double g[3];
+        box_muller3(d, (m > (T)0) ? sqrt((double)kT / (double)m) : 0.0, g);
+        v.x = (T)g[0];
+        v.y = (T)g[1];
+        v.z = (T)g[2];
     }
 }
 
@@ -320,9 +300,8 @@ __global__ void vv_kick_drift_kernel(int s0, int n, T dt, T dt_half, T skin_half
 }
 
 // ---- K2: second half kick + centre-of-mass momentum -------------------------------------------
-// Every CTA writes its partial sum(m v); the last CTA to finish adds the partials in index order
-// (deterministic) and publishes v_cm = sum(m v) / sum(m) (src/spatial.jl:901-916). The subtraction is
-// applied lazily by the next reader of the velocities (K1, the thermostat or export).
+// sum(m v) over the grid (grid_sum); the last CTA publishes v_cm = sum(m v) / sum(m) (src/spatial.jl:901-916). The
+// subtraction is applied lazily by the next reader of the velocities (K1, the thermostat or export).
 // COUPLE: the variant for the velocity-rescaling thermostats (single GPU) also sums m v.v in double alongside sum(m v); the
 // last CTA takes K after this step's CM removal, K - u.sum(m v) + M |u|^2 / 2 with u the v_cm as stored, and stores the
 // thermostat's factor next to v_cm (vrescale.cuh).
@@ -334,12 +313,18 @@ __device__ __forceinline__ void vcouple_store(CmState<T>* cm, const VCouple& vc,
     cm->lam = (T)vcouple_lambda(vc, ke, ctl->step, rng);
     cm->scaled = 1;
 }
+// k + m |v|^2 with its roundings spelled out: fma(m, fma(z, z, fma(y, y, x x)), k). Left to the compiler, which of the
+// products gets fused depends on the surrounding code, and in f64 that moves the last bits of the thermostat's K.
+template <typename T4>
+__device__ __forceinline__ double add_mvv(double k, double m, const T4& v) {
+    return fma(m, fma((double)v.z, (double)v.z, fma((double)v.y, (double)v.y, (double)v.x * (double)v.x)), k);
+}
 template <typename T, bool COUPLE>
 __global__ void __launch_bounds__(VV_THREADS)
     vv_kick2_kernel(int s0, int n, T dt_half, int do_cm, double inv_total_mass, const typename VT<T>::T4* __restrict__ f4,
                     const T* __restrict__ mass, typename VT<T>::T4* __restrict__ vel4, double* __restrict__ partial,
-                    Control* __restrict__ ctl, CmState<T>* __restrict__ cm, int apply_pending, double* __restrict__ mom_out,
-                    PeerSignal sig, VCouple vc) {
+                    Control* __restrict__ ctl, CmState<T>* __restrict__ cm, double* __restrict__ mom_out, PeerSignal sig,
+                    VCouple vc) {
     constexpr int W = COUPLE ? 4 : 3;
     double px = 0, py = 0, pz = 0, kk = 0;
     const int stride = gridDim.x * blockDim.x;
@@ -349,64 +334,44 @@ __global__ void __launch_bounds__(VV_THREADS)
         typename VT<T>::T4 va = vel4[sa], vb = vel4[okb ? sb : sa];
         const typename VT<T>::T4 fa = f4[sa], fb = f4[okb ? sb : sa];
         const T ma = mass[sa], mb_ = mass[okb ? sb : sa];
-        if (apply_pending && cm->valid) {
-            va.x -= cm->v[0]; va.y -= cm->v[1]; va.z -= cm->v[2];
-            vb.x -= cm->v[0]; vb.y -= cm->v[1]; vb.z -= cm->v[2];
-        }
         const T aa = va.w * dt_half, ab = vb.w * dt_half;
         va.x += fa.x * aa; va.y += fa.y * aa; va.z += fa.z * aa;
         vb.x += fb.x * ab; vb.y += fb.y * ab; vb.z += fb.z * ab;
         vel4[sa] = va;
         px += (double)(va.x * ma); py += (double)(va.y * ma); pz += (double)(va.z * ma);
-        if (COUPLE) kk += (double)ma * ((double)va.x * va.x + (double)va.y * va.y + (double)va.z * va.z);
+        if (COUPLE) kk = add_mvv(kk, ma, va);
         if (okb) {
             vel4[sb] = vb;
             px += (double)(vb.x * mb_); py += (double)(vb.y * mb_); pz += (double)(vb.z * mb_);
-            if (COUPLE) kk += (double)mb_ * ((double)vb.x * vb.x + (double)vb.y * vb.y + (double)vb.z * vb.z);
+            if (COUPLE) kk = add_mvv(kk, mb_, vb);
         }
     }
     if (!COUPLE && !do_cm && sig.n_peer == 0) return;
-    const int tid = threadIdx.x;
-    double p[W] = {px, py, pz};
-    if constexpr (COUPLE) p[W - 1] = kk;
-    block_sum<VV_THREADS, W>(p);
-    if (tid == 0)
-        for (int k = 0; k < W; k++) partial[W * (size_t)blockIdx.x + k] = p[k];
-    if (last_cta(&ctl->ticket)) {
-        __threadfence();
-        double s[W] = {};
-        for (int i = tid; i < (int)gridDim.x; i += VV_THREADS)
-            for (int k = 0; k < W; k++) s[k] += partial[W * (size_t)i + k];
-        __syncthreads();  // block_sum's scratch is reused
-        block_sum<VV_THREADS, W>(s);
-        if (tid == 0) {
-            const double a = s[0], b = s[1], c = s[2];
-            // peer-memory transport: the force kernel in front of this one is done with the halo data ...
-            for (int q = 0; q < sig.n_peer; q++) st_release_sys(sig.read_flag[q], sig.epoch);
-            if (!do_cm) {
-                if constexpr (COUPLE) vcouple_store<T>(cm, vc, 0.5 * s[W - 1], ctl);
-                return;
-            }
-            if (sig.n_mom > 0) {  // ... and sum(m v) goes to every rank (peer_cm_kernel adds them in rank order)
-                for (int r = 0; r < sig.n_mom; r++) {
-                    volatile double* d = sig.mom_dst[r];
-                    d[0] = a; d[1] = b; d[2] = c;
-                }
-                __threadfence_system();
-                for (int r = 0; r < sig.n_mom; r++) st_release_sys(sig.mom_flag[r], sig.epoch);
-            } else if (mom_out) {  // decomposed run over NCCL: the all-reduce and cm_from_sum_kernel finish it
-                mom_out[0] = a; mom_out[1] = b; mom_out[2] = c;
-            } else {
-                cm->v[0] = (T)(a * inv_total_mass);
-                cm->v[1] = (T)(b * inv_total_mass);
-                cm->v[2] = (T)(c * inv_total_mass);
-                cm->valid = 1;
-            }
-            if constexpr (COUPLE) {  // (single GPU: v_cm was stored just above)
-                const double ux = cm->v[0], uy = cm->v[1], uz = cm->v[2];
-                vcouple_store<T>(cm, vc, 0.5 * s[W - 1] + 0.5 * vc.total_mass * (ux * ux + uy * uy + uz * uz) - (ux * a + uy * b + uz * c), ctl);
-            }
+    double s[W] = {px, py, pz};
+    if constexpr (COUPLE) s[W - 1] = kk;
+    if (!grid_sum<VV_THREADS, W>(s, partial, &ctl->ticket) || threadIdx.x != 0) return;
+    const double a = s[0], b = s[1], c = s[2];
+    // peer-memory transport: the force kernel in front of this one is done with the halo data ...
+    for (int q = 0; q < sig.n_peer; q++) st_release_sys(sig.read_flag[q], sig.epoch);
+    if (!do_cm) {
+        if constexpr (COUPLE) vcouple_store<T>(cm, vc, 0.5 * s[W - 1], ctl);
+        return;
+    }
+    if (sig.n_mom > 0) {  // ... and sum(m v) goes to every rank (peer_cm_kernel adds them in rank order)
+        for (int r = 0; r < sig.n_mom; r++) {
+            volatile double* d = sig.mom_dst[r];
+            d[0] = a; d[1] = b; d[2] = c;
         }
+        __threadfence_system();
+        for (int r = 0; r < sig.n_mom; r++) st_release_sys(sig.mom_flag[r], sig.epoch);
+    } else if (mom_out) {  // decomposed run over NCCL: the all-reduce and cm_from_sum_kernel finish it
+        mom_out[0] = a; mom_out[1] = b; mom_out[2] = c;
+    } else {
+        cm->publish(s, inv_total_mass);
+    }
+    if constexpr (COUPLE) {  // (single GPU: v_cm was stored just above)
+        const double ux = cm->v[0], uy = cm->v[1], uz = cm->v[2];
+        vcouple_store<T>(cm, vc, 0.5 * s[W - 1] + 0.5 * vc.total_mass * (ux * ux + uy * uy + uz * uz) - (ux * a + uy * b + uz * c), ctl);
     }
 }
 
@@ -418,10 +383,7 @@ __global__ void max_disp_kernel(const Control* __restrict__ ctl, float* __restri
 
 template <typename T>
 __global__ void cm_from_sum_kernel(const double* __restrict__ mom_sum, double inv_total_mass, CmState<T>* cm) {
-    cm->v[0] = (T)(mom_sum[0] * inv_total_mass);
-    cm->v[1] = (T)(mom_sum[1] * inv_total_mass);
-    cm->v[2] = (T)(mom_sum[2] * inv_total_mass);
-    cm->valid = 1;
+    cm->publish(mom_sum, inv_total_mass);
 }
 
 // v_cm from the nranks partial sums of the peer-memory all-to-all, added in rank order (see peer.cuh)
@@ -432,19 +394,16 @@ __global__ void peer_cm_kernel(const PeerComm* __restrict__ comm, int nranks, un
     if ((int)threadIdx.x < nranks) spin_until(&comm->mom_epoch[par][threadIdx.x], epoch);
     __syncwarp();
     if (threadIdx.x == 0) {
-        double a = 0, b = 0, c = 0;
+        double s[3] = {0, 0, 0};
         for (int r = 0; r < nranks; r++) {
             const volatile double* m = comm->mom[par][r];
-            a += m[0]; b += m[1]; c += m[2];
+            s[0] += m[0]; s[1] += m[1]; s[2] += m[2];
         }
-        cm->v[0] = (T)(a * inv_total_mass);
-        cm->v[1] = (T)(b * inv_total_mass);
-        cm->v[2] = (T)(c * inv_total_mass);
-        cm->valid = 1;
+        cm->publish(s, inv_total_mass);
     }
 }
 
-// stand-alone momentum pass (remove_CM_motion! before the first step): same reduction, no kick
+// no pending v_cm or scale factor: the state at the start of every simulate call
 template <typename T>
 __global__ void clear_cm_kernel(CmState<T>* cm) {
     cm->v[0] = cm->v[1] = cm->v[2] = (T)0;
@@ -467,13 +426,11 @@ __global__ void andersen_kernel(int s0, int n_own, int n, T kT, double prob, con
     const uint32_t step_lo = (uint32_t)ctl->step;
     if (s < s0 + n_own) {
         typename VT<T>::T4 v = vel4[s];
-        if (cm->valid) { v.x -= cm->v[0]; v.y -= cm->v[1]; v.z -= cm->v[2]; }
+        cm->apply(v);
         andersen_apply<T>(v, orig[s], n, mass[s], kT, prob, step_lo, ctr1_lo, ctr1_hi, key_lo, key_hi);
         vel4[s] = v;
     }
-    // last CTA clears the pending CM state (the barrier puts every thread's velocity store before the ticket)
-    __syncthreads();
-    if (last_cta(&ctl->ticket) && threadIdx.x == 0) cm->valid = 0;
+    if (last_cta(&ctl->ticket) && threadIdx.x == 0) cm->valid = 0;  // the last CTA clears the pending v_cm
 }
 
 // ---- device-side loggers (mb_simulate_vv_log) -----------------------------------------------------------------
@@ -490,9 +447,8 @@ struct LogDesc {
 constexpr int LOG_THREADS = 256;
 // A read-only observer of the state after step ctl->step: applies the pending v_cm and scale factor and previews the Andersen draw that the
 // next drift kernel (or the standalone thermostat closing the call) will apply, with the same operations, so the logged
-// velocities are those export_kernel would return after this step. KE = 1/2 sum m v.v in double, per-CTA partials added in
-// index order by the last CTA, which also adds the pair-energy partials of the ENERGY force launch in index order and
-// writes the record.
+// velocities are those export_kernel would return after this step. KE = 1/2 sum m v.v in double (grid_sum); the last CTA
+// also adds the pair-energy partials of the ENERGY force launch in index order (sum_partials) and writes the record.
 template <typename T>
 __global__ void __launch_bounds__(LOG_THREADS)
     log_kernel(int n, int mask, Geom<T> g, const typename VT<T>::T4* __restrict__ pos4, const typename VT<T>::T4* __restrict__ vel4,
@@ -504,8 +460,7 @@ __global__ void __launch_bounds__(LOG_THREADS)
     if (s < n) {
         const int o = orig[s];
         typename VT<T>::T4 v = vel4[s];
-        if (cm->valid) { v.x -= cm->v[0]; v.y -= cm->v[1]; v.z -= cm->v[2]; }
-        if (cm->scaled) { v.x *= cm->lam; v.y *= cm->lam; v.z *= cm->lam; }
+        cm->apply(v);
         if (th.on && ctl->step > ctl->init_step)
             andersen_apply<T>(v, o, th.n, mass[s], th.kT, th.prob, (uint32_t)ctl->step, ctl->rng[0], ctl->rng[1], ctl->rng[2], ctl->rng[3]);
         const double vx = v.x, vy = v.y, vz = v.z;
@@ -517,26 +472,17 @@ __global__ void __launch_bounds__(LOG_THREADS)
             dst[0] = v.x; dst[1] = v.y; dst[2] = v.z;
         }
     }
-    const int tid = threadIdx.x;
-    k = block_sum<LOG_THREADS>(k);
-    if (tid == 0) ke_partial[blockIdx.x] = k;
-    if (!last_cta(&ctl->ticket)) return;
-    __threadfence();
-    double ke = 0, pe = 0;
-    for (int i = tid; i < (int)gridDim.x; i += LOG_THREADS) ke += ke_partial[i];
-    if (mask & LOG_ENERGY)
-        for (int i = tid; i < n_pe; i += LOG_THREADS) pe += pe_partial[i];
-    // KE, then PE: one component each, so that both reuse the scratch of the per-CTA sum above
-    __syncthreads();
-    ke = block_sum<LOG_THREADS>(ke);
-    __syncthreads();
-    pe = block_sum<LOG_THREADS>(pe);
-    if (tid == 0) {
+    double ke[1] = {k};
+    if (!grid_sum<LOG_THREADS, 1>(ke, ke_partial, &ctl->ticket)) return;
+    double pe[1];
+    __syncthreads();  // block_sum's scratch is reused
+    sum_partials<LOG_THREADS, 1>(pe_partial, (mask & LOG_ENERGY) ? n_pe : 0, pe);
+    if (threadIdx.x == 0) {
         if (mask & LOG_ENERGY) {
-            if (sp_energy) pe += *sp_energy;
-            pe += d->pe_const;
+            if (sp_energy) pe[0] += *sp_energy;
+            pe[0] += d->pe_const;
             double* r = d->rec + 3 * (size_t)d->count[0];
-            r[0] = (double)ctl->step; r[1] = pe; r[2] = ke;
+            r[0] = (double)ctl->step; r[1] = pe[0]; r[2] = ke[0];
             d->count[0]++;
         }
         if (mask & LOG_COORDS) d->count[1]++;
@@ -583,15 +529,10 @@ __global__ void random_velocities_kernel(int n, T kT, const T* __restrict__ mass
     if (i >= n) return;
     uint32_t d[4] = {(uint32_t)(i + 1), 0u, ctr1_lo, ctr1_hi};
     philox4x32_10(d, key_lo, key_hi);
-    const double two_pi = 6.283185307179586;
-    const double u1 = ((double)d[0] + 1.0) * (1.0 / 4294967296.0), u2 = (double)d[1] * (1.0 / 4294967296.0);
-    const double u3 = ((double)d[2] + 1.0) * (1.0 / 4294967296.0), u4 = (double)d[3] * (1.0 / 4294967296.0);
-    const double r1 = sqrt(-2.0 * log(u1)), r2 = sqrt(-2.0 * log(u3));
     const T m = mass[i];
-    const double sd = (m > (T)0) ? sqrt((double)kT / (double)m) : 0.0;
-    vels[3 * (size_t)i] = (T)(sd * r1 * cos(two_pi * u2));
-    vels[3 * (size_t)i + 1] = (T)(sd * r1 * sin(two_pi * u2));
-    vels[3 * (size_t)i + 2] = (T)(sd * r2 * cos(two_pi * u4));
+    double g[3];
+    box_muller3(d, (m > (T)0) ? sqrt((double)kT / (double)m) : 0.0, g);
+    for (int k = 0; k < 3; k++) vels[3 * (size_t)i + k] = (T)g[k];
 }
 
 // sum(m v) partials over an original-order velocity array (mb_remove_cm_motion)
