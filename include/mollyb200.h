@@ -145,6 +145,13 @@ int mb_forces_energy(mb_ctx* ctx, const void* coords, void* fs_mat, void* pe, vo
  * n_terms x 2 or 3. Host pointers. They are evaluated inside mb_simulate_vv (specific_forces_gpu!, src/force.jl:1231)
  * and by mb_forces_energy_all; mb_forces / mb_energy stay pairwise-only (the pairwise_*_loop_gpu! seam). */
 int mb_set_specific(mb_ctx* ctx, int kind, int64_t n_terms, const int32_t* atom_idx, const double* params);
+/* The multiple-time-step level of every term of one kind (mb_simulate_mts): level[t] of the t-th term as mb_set_specific
+ * received it, a 0-based index into the integrator's ordered fractions, 0 <= level < MB_MTS_MAX_LEVELS. n_terms must equal
+ * the count mb_set_specific set for that kind, which resets every level to 0. The engine stores each kind's terms grouped by
+ * level (stable within a level), so a level is one contiguous range of the bonded launch. Every other evaluation
+ * (mb_forces_energy_all, mb_simulate_vv and the other integrators, the loggers, the minimiser) sums all levels. Host
+ * pointer. Setting an array equal to the current one changes nothing. */
+int mb_set_specific_levels(mb_ctx* ctx, int kind, int64_t n_terms, const int32_t* level);
 /* forces(sys) / potential_energy(sys) of pairwise + specific + general interactions in one call (ADD semantics). */
 int mb_forces_energy_all(mb_ctx* ctx, const void* coords, void* fs_mat, void* pe, int64_t step_n);
 
@@ -315,6 +322,54 @@ typedef struct {
     double damping;           /* ps (reference default 100 dt) */
 } mb_nosehoover_params_t;
 int mb_simulate_nose_hoover(mb_ctx* ctx, void* coords, void* vels, const mb_nosehoover_params_t* p, mb_log_t* log);
+
+/* simulate!(sys, MTSIntegrator(dt, pi/si/gi_fractions; remove_CM_motion), n_steps) and, with langevin != 0,
+ * simulate!(sys, MTSLangevinIntegrator(dt, temperature, friction, ...), n_steps) (src/simulators.jl:1616-1940; rRESPA,
+ * Tuckerman et al. 1992; BAOAB-RESPA, Lagardère et al. 2019). fractions[0 .. n_levels) are the integrator's
+ * ordered_fractions: fractions[0] = 1, each one larger than and a multiple of the one before. Level 0 holds all pairwise
+ * interactions, PME and the terms of level 0 (mb_set_specific_levels); level l > 0 holds the bonded terms of level l.
+ * Prologue as mb_simulate_vv: wrap, CM removal when init_step == 0 and remove_cm_every != 0, neighbours, F_0 (the forces of
+ * level 0), loggers at init_step. An outer step runs mts_substeps! from level 0; at level l with dt_x = dt / fractions[l],
+ * dt_v = dt_x / 2, repeated fractions[l] / fractions[l - 1] times (once for level 0):
+ *   F_l = forces of level l (level 0: only at the start of a call; levels l > 0: on entry to the level);
+ *   v += F_l / m dt_v;
+ *   innermost level: x += v dt_x (MTSIntegrator) or x += v dt_x/2; v = c v + sigma_i xi; x += v dt_x/2 (langevin), with
+ *   c = exp(-dt friction / fractions[n_levels - 1]) and sigma_i = sqrt(1 - c^2) sqrt(kT / m_i); wrap;
+ *   other levels: the substeps of level l + 1;
+ *   F_l = forces of level l; v += F_l / m dt_v.
+ * Then CM removal when n % remove_cm_every == 0 and the loggers (mb_log_t, as for mb_simulate_vv_log), once per outer step.
+ * n_steps counts outer steps. The pairwise forces are evaluated once per outer step; level l > 0 is evaluated
+ * fractions[l] + fractions[l - 1] times per outer step, as in the reference. With n_levels = 1 and langevin = 0 this is the
+ * VelocityVerlet step, and the call runs it. Where the engine differs from the reference:
+ *  - neighbours: the exact displacement trigger of mb_simulate_vv, tested once per outer step after the last innermost
+ *    drift, so the structure is only rebuilt right before the pair evaluation (the bonded terms need none: they are
+ *    evaluated by minimum image). The all-pairs path wraps at that point too, not after every innermost drift;
+ *  - random numbers (langevin): xi of atom i (1-based original index) at innermost substep k (0-based within outer step n)
+ *    is the Box-Muller transform of one Philox4x32-10 block with counter (i, n, k, low word of ctr1) and key `rng_key`.
+ *    A function of (keys, outer step, substep, atom) only, so a run split into calls with the same keys takes the same
+ *    draws; the reference's draws agree in distribution only (random_velocities! on the host rng);
+ *  - f32 (langevin): c v + sigma xi is formed in double and rounded once;
+ *  - massless atoms (1/m = 0) get no kick and no noise;
+ *  - the substeps are unrolled into the captured step graph, so fractions[n_levels - 1] is limited to 1024.
+ * MB_ERR_INVALID before any work for dt <= 0, n_steps < 0, n_levels outside 1 .. MB_MTS_MAX_LEVELS, fractions that are not
+ * ordered as above, a term whose level is n_levels or more, kT or friction negative or not finite (langevin), a velocity
+ * coupling set on the context, a decomposed (multi-GPU) context, and the logging errors of mb_simulate_vv_log.
+ * MB_ERR_CAPACITY as in mb_simulate_vv. */
+#define MB_MTS_MAX_LEVELS 8
+typedef struct {
+    double dt;                            /* outer time step, ps */
+    int64_t n_steps;                      /* outer steps */
+    int64_t init_step;
+    int32_t remove_cm_every;              /* remove_CM_motion (default 1; 0 = never), in outer steps */
+    int32_t n_levels;                     /* length of ordered_fractions */
+    int32_t fractions[MB_MTS_MAX_LEVELS]; /* ordered_fractions; fractions[0] = 1 */
+    int32_t langevin;                     /* 0: MTSIntegrator, 1: MTSLangevinIntegrator */
+    int32_t reserved_;
+    double kT;                            /* langevin: k * temperature in kJ/mol */
+    double friction;                      /* langevin: ps^-1 */
+    uint64_t rng_ctr1, rng_key;           /* langevin: the draws' keys */
+} mb_mts_params_t;
+int mb_simulate_mts(mb_ctx* ctx, void* coords, void* vels, const mb_mts_params_t* p, mb_log_t* log);
 
 /* simulate!(sys, SteepestDescentMinimizer(step_size, max_steps, tol)) (src/simulators.jl:183-274) on the device: wrap the
  * coordinates, E = potential energy; then for step n = init_step+1 .. init_step+max_steps: F = forces, m = max |F_i|,

@@ -11,6 +11,7 @@
 #   Molly.simulate!(sys, sim::SteepestDescentMinimizer; ...)                                                simulators.jl:183
 #   Molly.simulate!(sys, sim::Langevin, n_steps; ...) with coupling === nothing                              simulators.jl:1101
 #   Molly.simulate!(sys, sim::NoseHoover, n_steps; ...) with coupling === nothing                            simulators.jl:1534
+#   Molly.simulate!(sys, sim::AbstractMTSIntegrator, n_steps; ...) with coupling === nothing                 simulators.jl:1850
 # (Molly.remove_CM_motion! for CuArray Systems is NOT redefined: the stock extension owns that exact signature)
 # and falls through to the stock methods (invoke) for anything it does not recognise: non-cubic boundaries,
 # constraints, virtual sites, couplings other than one AndersenThermostat, ImmediateThermostat, BerendsenThermostat or
@@ -74,6 +75,22 @@ struct MBNoseHooverParams
     remove_cm_every::Int32
     kT::Float64
     damping::Float64
+end
+
+# mb_mts_params_t (mb_simulate_mts)
+struct MBMTSParams
+    dt::Float64
+    n_steps::Int64
+    init_step::Int64
+    remove_cm_every::Int32
+    n_levels::Int32
+    fractions::NTuple{8, Int32}
+    langevin::Int32
+    reserved_::Int32
+    kT::Float64
+    friction::Float64
+    rng_ctr1::UInt64
+    rng_key::UInt64
 end
 
 # mb_vcoupling_t (mb_set_velocity_coupling)
@@ -438,6 +455,58 @@ function Molly.simulate!(sys::System{3, <:CuArray, T}, sim::NoseHoover, n_steps:
         end
     end
     check(ccall((:mb_simulate_nose_hoover, LIB), Cint, (Ptr{Cvoid}, CuPtr{Cvoid}, CuPtr{Cvoid}, Ref{MBNoseHooverParams}, Ptr{MBLog}),
+                ctx.handle, pointer(sys.coords), pointer(sys.velocities), Ref(p), C_NULL))
+    return sys
+end
+
+# ---- simulate!(sys, ::MTSIntegrator / ::MTSLangevinIntegrator, n) (src/simulators.jl:1616-1940) ------------------------------
+# Taken over under the conditions of the Langevin method above, when every pairwise fraction is 1 (the engine evaluates all
+# pairwise interactions in one kernel, once per outer step): one mb_simulate_mts call. The level of every specific term is
+# the index of its list's fraction in ordered_fractions, set for each list right after set_specific! set its terms (same
+# loop order, so the levels follow the list each kind ends up with). Anything else runs the stock method.
+function set_specific_levels!(ctx::Context, sys, sim)
+    for (sil, f) in zip(sys.specific_inter_lists, sim.si_fractions)
+        kind, idx, _ = specific_desc(sil)
+        level = fill(Int32(findfirst(==(f), sim.ordered_fractions) - 1), size(idx, 2))
+        check(ccall((:mb_set_specific_levels, LIB), Cint, (Ptr{Cvoid}, Cint, Int64, Ptr{Int32}),
+                    ctx.handle, kind, length(level), level))
+    end
+end
+
+function Molly.simulate!(sys::System{3, <:CuArray, T}, sim::Molly.AbstractMTSIntegrator, n_steps::Integer;
+                         init_step=0, rng=Random.default_rng(), run_loggers=true, kwargs...) where T
+    descs = engine_eligible(sys, sys.pairwise_inters)
+    device_logs = run_loggers == false || isempty(sys.loggers) ||
+                  all(l -> !isnothing(device_log_kind(l)), values(sys.loggers))
+    if isnothing(descs) || !isnothing(sim.coupling) || !device_logs || !all(==(1), sim.pi_fractions) ||
+            length(sim.pi_fractions) != length(sys.pairwise_inters) ||
+            length(sim.si_fractions) != length(sys.specific_inter_lists) ||
+            length(sim.gi_fractions) != length(sys.general_inters) ||
+            length(sim.ordered_fractions) > 8 || last(sim.ordered_fractions) > 1024 ||
+            !all(gi -> gi isa Molly.LJDispersionCorrection, sys.general_inters) ||
+            !all(!isnothing, map(specific_desc, sys.specific_inter_lists))
+        # stock: simulate!(sys, sim::AbstractMTSIntegrator, n_steps_or_time; ...) src/simulators.jl:1850
+        return invoke(Molly.simulate!, Tuple{Any, Molly.AbstractMTSIntegrator, Any}, sys, sim, n_steps;
+                      init_step=init_step, rng=rng, run_loggers=run_loggers, kwargs...)
+    end
+    ctx = context_for(sys, descs)
+    set_specific!(ctx, sys)
+    set_specific_levels!(ctx, sys, sim)
+    set_velocity_coupling!(ctx, nothing)
+    fr = zeros(Int32, 8)
+    fr[1:length(sim.ordered_fractions)] .= sim.ordered_fractions
+    lang = sim isa MTSLangevinIntegrator
+    kT = lang ? Float64(ustrip(sys.k * sim.temperature)) : 0.0
+    friction = !lang ? 0.0 : sim.friction isa Unitful.Quantity ? Float64(ustrip(u"ps^-1", sim.friction)) : Float64(sim.friction)
+    p = MBMTSParams(_ps(sim.dt), n_steps, init_step, Int32(sim.remove_CM_motion), Int32(length(sim.ordered_fractions)),
+                    NTuple{8, Int32}(fr), Int32(lang), Int32(0), kT, friction, rand(rng, UInt64), rand(rng, UInt64))
+    if run_loggers != false && !isempty(sys.loggers)
+        return simulate_logged!(sys, ctx, n_steps, init_step, run_loggers) do lg
+            ccall((:mb_simulate_mts, LIB), Cint, (Ptr{Cvoid}, CuPtr{Cvoid}, CuPtr{Cvoid}, Ref{MBMTSParams}, Ref{MBLog}),
+                  ctx.handle, pointer(sys.coords), pointer(sys.velocities), Ref(p), lg)
+        end
+    end
+    check(ccall((:mb_simulate_mts, LIB), Cint, (Ptr{Cvoid}, CuPtr{Cvoid}, CuPtr{Cvoid}, Ref{MBMTSParams}, Ptr{MBLog}),
                 ctx.handle, pointer(sys.coords), pointer(sys.velocities), Ref(p), C_NULL))
     return sys
 end

@@ -10,7 +10,8 @@ from .api import (Atom, CubicBoundary, TriclinicBoundary, System, NoCutoff, Dist
                   ShiftedForceCutoff, LennardJones, Coulomb, CoulombReactionField, CoulombEwald, GPUNeighborFinder,
                   DistanceNeighborFinder, CellListMapNeighborFinder, TreeNeighborFinder, AndersenThermostat,
                   ImmediateThermostat, BerendsenThermostat, VelocityRescaleThermostat,
-                  VelocityVerlet, Langevin, NoseHoover, forces, forces_virial, potential_energy, forces_energy, find_neighbors, simulate,
+                  VelocityVerlet, Langevin, NoseHoover, MTSIntegrator, MTSLangevinIntegrator, setup_mts_integrator,
+                  mts_levels, forces, forces_virial, potential_energy, forces_energy, find_neighbors, simulate,
                   kinetic_energy, temperature, remove_CM_motion, random_velocities, wrap_coords, device_count,
                   atoms_from_arrays, atoms_to_array, atom_dtype, MollyB200Error, COULOMB_CONST, BOLTZMANN_K,
                   comm_unique_id, comm_init, decomp_plan, InteractionList2Atoms, InteractionList3Atoms,

@@ -22,8 +22,9 @@ EXPORTED = [
     "mb_comm_init", "mb_decomp_plan", "mb_set_profiling", "mb_set_specific", "mb_forces_energy_all", "mb_set_pme", "mb_pme_plan",
     "mb_set_lj_dispersion_correction", "mb_random_velocities", "mb_kinetic_energy_tensor", "mb_set_box_triclinic",
     "mb_simulate_vv_log", "mb_minimize_sd", "mb_set_velocity_coupling", "mb_simulate_langevin",
-    "mb_simulate_nose_hoover",
+    "mb_simulate_nose_hoover", "mb_set_specific_levels", "mb_simulate_mts",
 ]
+MB_MTS_MAX_LEVELS = 8
 
 
 class MBInter(C.Structure):
@@ -66,6 +67,14 @@ class MBNoseHooverParams(C.Structure):
     _fields_ = [
         ("dt", C.c_double), ("n_steps", C.c_int64), ("init_step", C.c_int64), ("remove_cm_every", C.c_int32),
         ("kT", C.c_double), ("damping", C.c_double),
+    ]
+
+
+class MBMTSParams(C.Structure):
+    _fields_ = [
+        ("dt", C.c_double), ("n_steps", C.c_int64), ("init_step", C.c_int64), ("remove_cm_every", C.c_int32),
+        ("n_levels", C.c_int32), ("fractions", C.c_int32 * MB_MTS_MAX_LEVELS), ("langevin", C.c_int32), ("reserved_", C.c_int32),
+        ("kT", C.c_double), ("friction", C.c_double), ("rng_ctr1", C.c_uint64), ("rng_key", C.c_uint64),
     ]
 
 
@@ -128,6 +137,8 @@ def load():
     L.mb_simulate_vv_log.argtypes = [vp, vp, vp, C.POINTER(MBVVParams), C.POINTER(MBLog)]
     L.mb_simulate_langevin.argtypes = [vp, vp, vp, C.POINTER(MBLangevinParams), C.POINTER(MBLog)]
     L.mb_simulate_nose_hoover.argtypes = [vp, vp, vp, C.POINTER(MBNoseHooverParams), C.POINTER(MBLog)]
+    L.mb_simulate_mts.argtypes = [vp, vp, vp, C.POINTER(MBMTSParams), C.POINTER(MBLog)]
+    L.mb_set_specific_levels.argtypes = [vp, C.c_int, i64, vp]
     L.mb_minimize_sd.argtypes = [vp, vp, C.POINTER(MBSDParams)]
     L.mb_set_velocity_coupling.argtypes = [vp, C.POINTER(MBVCoupling)]
     L.mb_remove_cm_motion.argtypes = [vp, vp]

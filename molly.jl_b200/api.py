@@ -14,6 +14,7 @@ julia/MollyB200Ext.jl, see INTEGRATION.md):
     SteepestDescentMinimizer                        src/simulators.jl:183-274 (simulate dispatches on the simulator)
     Langevin                                        src/simulators.jl:1065-1210 (mb_simulate_langevin)
     NoseHoover                                      src/simulators.jl:1491-1614 (mb_simulate_nose_hoover)
+    MTSIntegrator, MTSLangevinIntegrator            src/simulators.jl:1616-1940 (mb_simulate_mts)
     forces, forces_virial, potential_energy         src/force.jl:678-720, src/energy.jl:202-248
     kinetic_energy, temperature, remove_CM_motion   src/energy.jl:44-175, src/spatial.jl:901-929
     *EnergyLogger, TemperatureLogger, Coordinates-  src/loggers.jl:44-102, :134-278 (recorded on the device inside
@@ -460,6 +461,107 @@ class NoseHoover:
             raise ValueError(f"remove_CM_motion must be non-negative, found {self.remove_CM_motion}")
 
 
+def _is_integer(x) -> bool:
+    return isinstance(x, (int, np.integer))
+
+
+def setup_mts_integrator(pi_fractions, si_fractions, gi_fractions) -> tuple:
+    """setup_mts_integrator (src/simulators.jl:1713-1738): the distinct fractions in increasing order, ordered_fractions =
+    (1, f1, f2, ...). ValueError where the reference raises ArgumentError."""
+    if not (len(pi_fractions) or len(si_fractions) or len(gi_fractions)):
+        raise ValueError("MTSIntegrator requires one of pi_fractions, si_fractions or gi_fractions to be provided")
+    if not all(_is_integer(f) for f in (*pi_fractions, *si_fractions, *gi_fractions)):
+        raise ValueError("MTSIntegrator requires pi_fractions, si_fractions and gi_fractions to consist of integers")
+    ordered = tuple(sorted({int(f) for f in (*pi_fractions, *si_fractions, *gi_fractions)}))
+    if ordered[0] < 1:
+        raise ValueError(f"MTSIntegrator fraction {ordered[0]} cannot be less than 1")
+    if ordered[0] > 1:
+        raise ValueError(f"MTSIntegrator fractions must include 1, lowest fraction is {ordered[0]}")
+    for a, b in zip(ordered, ordered[1:]):
+        if b % a != 0:
+            raise ValueError(f"MTSIntegrator fraction {b} not a multiple of fraction {a}")
+    return ordered
+
+
+@dataclass
+class MTSIntegrator:
+    """MTSIntegrator(dt; pi_fractions, si_fractions, gi_fractions, coupling=None, remove_CM_motion=1) —
+    src/simulators.jl:1616-1654, 1740-1745: rRESPA multiple time stepping (Tuckerman et al. 1992), run on the device by
+    mb_simulate_mts (see include/mollyb200.h). dt is the outer step in ps; an interaction with fraction f is applied f times
+    per outer step; n_steps counts outer steps. The engine evaluates every pairwise interaction and PME once per outer step
+    (fraction 1); each specific interaction list has a level of its own. A coupling is not run: simulate refuses it."""
+    dt: float
+    pi_fractions: tuple = ()
+    si_fractions: tuple = ()
+    gi_fractions: tuple = ()
+    coupling: object = None
+    remove_CM_motion: int = 1
+    ordered_fractions: tuple = field(init=False)
+
+    def __post_init__(self):
+        if not (math.isfinite(self.dt) and self.dt > 0):
+            raise ValueError(f"dt must be finite and positive, found {self.dt}")
+        self.pi_fractions, self.si_fractions, self.gi_fractions = (tuple(self.pi_fractions), tuple(self.si_fractions),
+                                                                   tuple(self.gi_fractions))
+        self.ordered_fractions = setup_mts_integrator(self.pi_fractions, self.si_fractions, self.gi_fractions)
+        self.remove_CM_motion = int(self.remove_CM_motion)  # Int(remove_CM_motion): false -> 0
+        if self.remove_CM_motion < 0:
+            raise ValueError(f"remove_CM_motion must be non-negative, found {self.remove_CM_motion}")
+
+
+@dataclass
+class MTSLangevinIntegrator:
+    """MTSLangevinIntegrator(dt, temperature, friction; pi_fractions, si_fractions, gi_fractions, coupling=None,
+    remove_CM_motion=1) — src/simulators.jl:1656-1711, 1747-1757: BAOAB-RESPA (Lagardère et al. 2019), run on the device by
+    mb_simulate_mts. The O step runs at every innermost substep with vel_scale = exp(-dt friction / last(ordered_fractions))
+    and noise_scale = sqrt(1 - vel_scale^2), as the reference's constructor computes them. Temperature in K, friction in
+    ps^-1; the rest as MTSIntegrator."""
+    dt: float
+    temperature: float
+    friction: float
+    pi_fractions: tuple = ()
+    si_fractions: tuple = ()
+    gi_fractions: tuple = ()
+    coupling: object = None
+    remove_CM_motion: int = 1
+    ordered_fractions: tuple = field(init=False)
+    vel_scale: float = field(init=False)
+    noise_scale: float = field(init=False)
+
+    def __post_init__(self):
+        MTSIntegrator.__post_init__(self)
+        _check_temperature(self.temperature)
+        if not (math.isfinite(self.friction) and self.friction >= 0):
+            raise ValueError(f"friction must be finite and non-negative, found {self.friction}")
+        self.vel_scale = math.exp(-self.dt * self.friction / self.ordered_fractions[-1])
+        self.noise_scale = math.sqrt(1 - self.vel_scale ** 2)
+
+
+def mts_levels(sys, sim) -> dict:
+    """The level of every specific term for mb_set_specific_levels: {kind: int32 array}, in the order System._configure
+    concatenates the lists of one kind (e.g. propers then impropers). Checks the fractions against the System as
+    mts_interaction_groups does (ValueError), and refuses what the engine does not split (TypeError): a pairwise
+    interaction or PME at a fraction other than 1 (LJDispersionCorrection exerts no force: any fraction)."""
+    for name, fr, inters in (("pairwise", sim.pi_fractions, sys.pairwise_inters),
+                             ("specific", sim.si_fractions, sys.specific_inter_lists),
+                             ("general", sim.gi_fractions, sys.general_inters)):
+        if len(fr) != len(inters):
+            raise ValueError(f"the system has {len(inters)} {name} interactions but there are {len(fr)} in the "
+                             f"{type(sim).__name__}")
+    if any(f != 1 for f in sim.pi_fractions):
+        raise TypeError(f"{type(sim).__name__}: pairwise interactions at a fraction other than 1 are not supported "
+                        "(the engine evaluates them in one kernel once per outer step; the stock Molly path handles it)")
+    for gi, f in zip(sys.general_inters, sim.gi_fractions):
+        if isinstance(gi, PME) and f != 1:
+            raise TypeError(f"{type(sim).__name__}: PME at a fraction other than 1 is not supported (the stock Molly "
+                            "path handles it)")
+    parts = {}
+    for sil, f in zip(sys.specific_inter_lists, sim.si_fractions):
+        n = len(sil.arrays()[0])
+        parts.setdefault(sil.kind, []).append(np.full(n, sim.ordered_fractions.index(int(f)), np.int32))
+    return {kind: np.ascontiguousarray(np.concatenate(p)) for kind, p in parts.items()}
+
+
 @dataclass
 class SteepestDescentMinimizer:
     """SteepestDescentMinimizer(step_size, max_steps, tol, log_stream) — src/simulators.jl:183-274, run on the device by
@@ -866,6 +968,9 @@ def simulate(sys: System, sim, n_steps: Optional[int] = None, init_step: int = 0
     as VelocityVerlet; the velocities are half a step behind the positions.
     NoseHoover: simulate!(sys, sim, n_steps; run_loggers=true) — src/simulators.jl:1534-1614, the same arguments and loggers
     as VelocityVerlet; zeta starts at 0 in every call.
+    MTSIntegrator, MTSLangevinIntegrator: simulate!(sys, sim, n_steps; run_loggers=true) — src/simulators.jl:1783-1940,
+    n_steps outer steps; the same arguments and loggers (once per outer step) as VelocityVerlet. The level of every specific
+    term is set on the context (mb_set_specific_levels) before the call.
     SteepestDescentMinimizer: simulate!(sys, sim; run_loggers=false) — src/simulators.jl:183-274, see steepest_descent.
     Loggers are not run during a minimisation (run_loggers must be false)."""
     if isinstance(sim, SteepestDescentMinimizer):
@@ -875,7 +980,8 @@ def simulate(sys: System, sim, n_steps: Optional[int] = None, init_step: int = 0
             raise NotImplementedError("loggers are not run during a minimisation on the device (run_loggers must be false)")
         steepest_descent(sys, sim, init_step=init_step, max_retries=max_retries)
         return sys
-    if not isinstance(sim, (VelocityVerlet, Langevin, NoseHoover)):
+    mts = isinstance(sim, (MTSIntegrator, MTSLangevinIntegrator))
+    if not (mts or isinstance(sim, (VelocityVerlet, Langevin, NoseHoover))):
         raise TypeError(f"unsupported simulator {type(sim).__name__}")
     if n_steps is None:
         raise TypeError(f"simulate(sys, ::{type(sim).__name__}, n_steps) needs n_steps")
@@ -884,7 +990,18 @@ def simulate(sys: System, sim, n_steps: Optional[int] = None, init_step: int = 0
     _check_run_loggers(run_loggers)
     couplings = sim.coupling if isinstance(sim.coupling, (tuple, list)) else ((sim.coupling,) if sim.coupling else ())
     vc = None
-    if isinstance(sim, Langevin):
+    if mts:
+        if couplings:
+            raise TypeError(f"unsupported coupling {couplings[0]!r} with {type(sim).__name__} (the stock Molly path handles it)")
+        levels = mts_levels(sys, sim)
+        p = capi.MBMTSParams()
+        p.n_levels = len(sim.ordered_fractions)
+        p.fractions[:p.n_levels] = sim.ordered_fractions
+        if isinstance(sim, MTSLangevinIntegrator):
+            p.langevin = 1
+            p.kT = sys.k * sim.temperature
+            p.friction = float(sim.friction)
+    elif isinstance(sim, Langevin):
         if couplings:
             raise TypeError(f"unsupported coupling {couplings[0]!r} with Langevin (the stock Molly path handles it)")
         p = capi.MBLangevinParams()
@@ -914,6 +1031,9 @@ def simulate(sys: System, sim, n_steps: Optional[int] = None, init_step: int = 0
     p.remove_cm_every = int(sim.remove_CM_motion)
     ctx = sys.engine()
     capi.check(sys._L.mb_set_velocity_coupling(ctx, C.byref(vc) if vc is not None else None))  # (Langevin, NoseHoover: cleared)
+    if mts:  # (an unchanged level array leaves the context as it is)
+        for kind, lv in levels.items():
+            capi.check(sys._L.mb_set_specific_levels(ctx, kind, len(lv), lv.ctypes.data))
     if not isinstance(sim, NoseHoover):  # (NoseHoover draws nothing)
         rng = rng or np.random.default_rng()
         p.rng_ctr1 = int(rng.integers(0, 2 ** 63))
@@ -929,6 +1049,9 @@ def simulate(sys: System, sim, n_steps: Optional[int] = None, init_step: int = 0
         elif isinstance(sim, NoseHoover):
             rc = sys._L.mb_simulate_nose_hoover(ctx, _ptr(sys.coords), _ptr(sys.velocities), C.byref(p),
                                                 C.byref(plan.desc) if plan is not None else None)
+        elif mts:
+            rc = sys._L.mb_simulate_mts(ctx, _ptr(sys.coords), _ptr(sys.velocities), C.byref(p),
+                                        C.byref(plan.desc) if plan is not None else None)
         elif plan is None:
             rc = sys._L.mb_simulate_vv(ctx, _ptr(sys.coords), _ptr(sys.velocities), C.byref(p))
         else:  # a retry overwrites the records of the failed attempt

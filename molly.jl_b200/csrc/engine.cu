@@ -3,6 +3,7 @@
 //
 // There is deliberately no CPU code path: every entry point needs a CUDA device.
 #include <algorithm>
+#include <array>
 #include <map>
 #include <memory>
 #include <tuple>
@@ -15,10 +16,12 @@
 #include "force.cuh"
 #include "langevin.cuh"
 #include "minimize.cuh"
+#include "mts.cuh"
 #include "nosehoover.cuh"
 #include "pair.cuh"
 #include "pme.cuh"
 #include "vv.cuh"
+static_assert(mb::MTS_MAX_LEVELS == MB_MTS_MAX_LEVELS, "mts.cuh levels = MB_MTS_MAX_LEVELS");
 static_assert((int)mb::VC_NONE == (int)MB_VC_NONE && (int)mb::VC_IMMEDIATE == (int)MB_VC_IMMEDIATE &&
                   (int)mb::VC_BERENDSEN == (int)MB_VC_BERENDSEN && (int)mb::VC_VRESCALE == (int)MB_VC_VRESCALE,
               "vrescale.cuh kinds = MB_VC_*");
@@ -324,10 +327,10 @@ class EngineBase {
                                const int32_t* sj) = 0;
     virtual int set_neighbor_policy(double r_list, int rebuild_every) = 0;
     virtual int forces_energy(const void* coords, void* fs, void* pe, void* vir, int64_t step_n, bool with_specific) = 0;
-    // lg, nh: the Langevin or Nose-Hoover integrator's parameters (at most one), both NULL for VelocityVerlet (p then carries
-    // the fields all three share)
+    // lg, nh, mts: the Langevin, Nose-Hoover or multiple-time-step integrator's parameters (at most one), all NULL for
+    // VelocityVerlet (p then carries the fields they share)
     virtual int simulate(void* coords, void* vels, const mb_vv_params_t* p, const mb_langevin_params_t* lg,
-                         const mb_nosehoover_params_t* nh, mb_log_t* log) = 0;
+                         const mb_nosehoover_params_t* nh, const mb_mts_params_t* mts, mb_log_t* log) = 0;
     virtual int remove_cm(void* vels) = 0;
     virtual int kinetic_energy(const void* vels, double* out) = 0;
     virtual int rebuild(const void* coords) = 0;
@@ -338,6 +341,7 @@ class EngineBase {
     virtual int set_profiling(int enable) = 0;
     virtual int comm_init(const void* uid, int rank, int nranks) = 0;
     virtual int set_specific(int kind, int64_t n, const int32_t* idx, const double* par) = 0;
+    virtual int set_specific_levels(int kind, int64_t n, const int32_t* level) = 0;
     virtual int set_pme(double r_cut, double error_tol, int order, double eps_r, int64_t n_pairs, const int32_t* pi, const int32_t* pj) = 0;
     virtual int set_dispersion(double r_cut) = 0;
     virtual int random_velocities(void* vels, double kT, uint64_t ctr1, uint64_t key) = 0;
@@ -885,20 +889,61 @@ class Engine : public EngineBase {
             MB_CUDA(cudaMemcpy(d_sp_idx_k_[kind].p, hidx.data(), hidx.size() * sizeof(int), cudaMemcpyHostToDevice));
             MB_CUDA(cudaMemcpy(d_sp_par_k_[kind].p, hpar.data(), hpar.size() * sizeof(T), cudaMemcpyHostToDevice));
         }
+        h_sp_idx_[kind] = std::move(hidx);  // (kept in the caller's order: mb_set_specific_levels regroups them)
+        h_sp_par_[kind] = std::move(hpar);
+        h_sp_level_[kind].assign(n, 0);
+        for (int l = 0; l <= MTS_MAX_LEVELS; l++) sp_lvl_off_[kind][l] = (l == 0) ? 0 : n;
         int64_t mx = std::max(sp_n_[0], std::max(sp_n_[1], sp_n_[2]));
         MB_CUDA(d_sp_partial_.ensure((size_t)(3 * ((mx + BONDED_THREADS - 1) / BONDED_THREADS) + 8) * sizeof(double)));
         drop_graphs();  // the graphs bake the term counts in
         return MB_OK;
+    }
+    // multiple-time-step levels: the device arrays of a kind hold its terms grouped by level (stable), level l in
+    // [sp_lvl_off_[kind][l], sp_lvl_off_[kind][l + 1])
+    int set_specific_levels(int kind, int64_t n, const int32_t* level) override {
+        if (kind < 0 || kind > 2 || n < 0 || (n > 0 && !level)) return set_error(MB_ERR_INVALID, "mb_set_specific_levels: bad arguments");
+        if (n != sp_n_[kind])
+            return set_error(MB_ERR_INVALID, "mb_set_specific_levels: " + std::to_string(n) + " levels for " + std::to_string(sp_n_[kind]) +
+                                                 " terms of kind " + std::to_string(kind) + " (mb_set_specific)");
+        for (int64_t t = 0; t < n; t++)
+            if (level[t] < 0 || level[t] >= MTS_MAX_LEVELS)
+                return set_error(MB_ERR_INVALID, "mb_set_specific_levels: a level outside 0 .. MB_MTS_MAX_LEVELS - 1");
+        if (std::equal(level, level + n, h_sp_level_[kind].begin())) return MB_OK;  // (the captured graphs stay valid)
+        const int na = kind + 2, np_ = (kind == 2) ? 3 : 2;
+        std::vector<int64_t> order(n);
+        for (int64_t t = 0; t < n; t++) order[t] = t;
+        std::stable_sort(order.begin(), order.end(), [&](int64_t a, int64_t b) { return level[a] < level[b]; });
+        std::vector<int> hidx((size_t)n * na);
+        std::vector<T> hpar((size_t)n * np_);
+        for (int64_t k = 0; k < n; k++) {
+            std::copy_n(&h_sp_idx_[kind][(size_t)order[k] * na], na, &hidx[(size_t)k * na]);
+            std::copy_n(&h_sp_par_[kind][(size_t)order[k] * np_], np_, &hpar[(size_t)k * np_]);
+        }
+        MB_CUDA(cudaMemcpy(d_sp_idx_k_[kind].p, hidx.data(), hidx.size() * sizeof(int), cudaMemcpyHostToDevice));
+        MB_CUDA(cudaMemcpy(d_sp_par_k_[kind].p, hpar.data(), hpar.size() * sizeof(T), cudaMemcpyHostToDevice));
+        h_sp_level_[kind].assign(level, level + n);
+        for (int l = 0; l <= MTS_MAX_LEVELS; l++)
+            sp_lvl_off_[kind][l] = std::count_if(level, level + n, [l](int32_t v) { return v < l; });
+        drop_graphs();  // the graphs bake the level ranges in
+        return MB_OK;
+    }
+    // the deepest level any term sits at
+    int max_specific_level() const {
+        int m = 0;
+        for (int kind = 0; kind < 3; kind++)
+            for (int32_t v : h_sp_level_[kind]) m = std::max(m, (int)v);
+        return m;
     }
     bool has_lists() const { return sp_n_[0] + sp_n_[1] + sp_n_[2] > 0; }
     bool has_specific() const { return has_lists() || pme_on_; }  // everything that is added after the pair kernel
     // the slot of every atom for kernels that index atoms in original order (null: the all-pairs path keeps that order)
     const int* slot_of() const { return path_ == 1 ? d_inv_orig_.as<int>() : nullptr; }
     // add the bonded forces to f4 (slot order on the brick path, original order on the all-pairs path; default d_f4_);
-    // with energy: per-kernel partials are summed into d_sp_energy_ (double, device)
-    int launch_bonded(bool energy, T4* f4 = nullptr) {
+    // with energy: per-kernel partials are summed into d_sp_energy_ (double, device). level: the terms of one
+    // multiple-time-step level (PME belongs to level 0), or -1 for all of them
+    int launch_bonded(bool energy, T4* f4 = nullptr, int level = -1) {
         if (!f4) f4 = d_f4_.as<T4>();
-        if (!has_specific()) return MB_OK;
+        if (!has_specific() || (level > 0 && !has_lists())) return MB_OK;
         MB_CUDA(d_sp_partial_.ensure(64 * sizeof(double)));  // (set_specific sizes it for the lists; PME alone needs it to exist)
         BoxT bx;
         for (int d = 0; d < 3; d++) bx.L[d] = box_[d];
@@ -910,10 +955,11 @@ class Engine : public EngineBase {
         BondedLists L;
         int total_blk = 0;
         for (int kind = 0; kind < 3; kind++) {
-            L.n[kind] = (int)sp_n_[kind];
+            const int64_t lo = level < 0 ? 0 : sp_lvl_off_[kind][level], hi = level < 0 ? sp_n_[kind] : sp_lvl_off_[kind][level + 1];
+            L.n[kind] = (int)(hi - lo);
             L.nblk[kind] = (L.n[kind] + BONDED_THREADS - 1) / BONDED_THREADS;
-            L.idx[kind] = d_sp_idx_k_[kind].as<int>();
-            L.par[kind] = d_sp_par_k_[kind].p;
+            L.idx[kind] = d_sp_idx_k_[kind].as<int>() + lo * (kind + 2);
+            L.par[kind] = d_sp_par_k_[kind].as<T>() + lo * (kind == 2 ? 3 : 2);
             total_blk += L.nblk[kind];
         }
         if (total_blk > 0) {
@@ -931,7 +977,7 @@ class Engine : public EngineBase {
             }
         }
         MB_CUDA(cudaGetLastError());
-        if (pme_on_) MB_TRY(launch_pme(energy, f4));
+        if (pme_on_ && level <= 0) MB_TRY(launch_pme(energy, f4));
         return MB_OK;
     }
 
@@ -1692,11 +1738,15 @@ class Engine : public EngineBase {
         bool thermostat;
         int* flag_ptr;
         VCouple vc;       // velocity-rescaling thermostat (kind VC_NONE: none)
-        int integrator;   // INTEG_*: VelocityVerlet (vv.cuh), Langevin (langevin.cuh) or Nose-Hoover (nosehoover.cuh)
-        LangevinCoef lc;  // Langevin's c, sqrt(1 - c^2) and kT
+        int integrator;   // INTEG_*: VelocityVerlet (vv.cuh), Langevin (langevin.cuh), Nose-Hoover (nosehoover.cuh) or the
+                          // multiple-time-step integrators (mts.cuh)
+        LangevinCoef lc;  // Langevin's (or MTSLangevinIntegrator's) c, sqrt(1 - c^2) and kT
         NhCoef nc;        // Nose-Hoover's dt / (2 Q^2) and Nf k T0
+        int n_levels;     // multiple-time-step integrators: the ordered fractions
+        std::array<int, MTS_MAX_LEVELS> fractions;
     };
-    enum { INTEG_VV = 0, INTEG_LANGEVIN = 1, INTEG_NH = 2 };
+    enum { INTEG_VV = 0, INTEG_LANGEVIN = 1, INTEG_NH = 2, INTEG_MTS = 3, INTEG_MTS_LANGEVIN = 4 };
+    static bool is_mts(int integrator) { return integrator == INTEG_MTS || integrator == INTEG_MTS_LANGEVIN; }
     // what one step does beyond the plain VelocityVerlet step
     struct StepOpts {
         int do_cm = 0;                   // remove_CM_motion after this step's kick
@@ -1737,6 +1787,7 @@ class Engine : public EngineBase {
         return MB_OK;
     }
     int enqueue_step(const StepCfg& c, const StepOpts& o, Capture* cap = nullptr) {
+        if (is_mts(c.integrator)) return enqueue_mts_step(c, o, cap);
         const bool dec = decomposed() && path_ == 1;
         const int s0 = dec ? own_s0_ : 0, n_own = dec ? own_n_ : (int)n_;
         const int nb = std::max(1, (n_own + 255) / 256);
@@ -1860,6 +1911,101 @@ class Engine : public EngineBase {
         MB_CUDA(cudaGetLastError());
         return MB_OK;
     }
+    // One outer step of the multiple-time-step integrators (mts.cuh): mts_substeps! from level 0, unrolled on the host.
+    // Level 0's forces stay in d_f4_ from one outer step to the next (pairs, its bonded ranges and PME); the inner levels
+    // share d_f4_mts_, which a level recomputes on entry and after each of its substeps, as the reference's one force
+    // buffer. The neighbour rebuild (cell-list path) or the wrap (all-pairs path) follows the last innermost drift, so the
+    // slot order only changes in front of a pair evaluation.
+    struct MtsWalk {
+        int substep = 0;        // innermost substeps issued in this outer step
+        bool cm_taken = false;  // the first kick (which applies the pending v_cm) has been issued
+    };
+    // F of one level: level 0 into d_f4_ (pairs, its bonded terms, PME), level l > 0 into d_f4_mts_ (its bonded terms)
+    int mts_forces(int level) {
+        if (level == 0) {
+            MB_TRY(launch_pairs(false, d_f4_.as<T4>()));
+            return launch_bonded(false, nullptr, 0);
+        }
+        MB_CUDA(cudaMemsetAsync(d_f4_mts_.p, 0, (size_t)n_ * sizeof(T4), stream_));
+        return launch_bonded(false, d_f4_mts_.as<T4>(), level);
+    }
+    int enqueue_mts_level(const StepCfg& c, const StepOpts& o, Capture* cap, int l, bool recompute, MtsWalk& w) {
+        const int n = (int)n_, n_inner = c.fractions[c.n_levels - 1];
+        const double dt_x = (double)c.dt / c.fractions[l];
+        const T dt_v = (T)(dt_x / 2);
+        T4* f = (l == 0) ? d_f4_.as<T4>() : d_f4_mts_.as<T4>();
+        Control* ctl = d_ctl_.as<Control>();
+        CmState<T>* cm = d_cm_.as<CmState<T>>();
+        int grid;
+        MB_TRY(integ_grid(grid, n, 1, 8, 0));
+        // after the first kick of the outer step, which applied the pending v_cm: clear it where nothing overwrites it
+        auto first_kick_done = [&]() {
+            if (w.cm_taken) return;
+            w.cm_taken = true;
+            if (o.clear_cm_after_k1) {
+                clear_cm_kernel<T><<<1, 1, 0, stream_>>>(cm);
+                launches_++;
+            }
+        };
+        const int reps = c.fractions[l] / (l == 0 ? 1 : c.fractions[l - 1]);
+        for (int r = 0; r < reps; r++) {
+            if (recompute) MB_TRY(mts_forces(l));
+            const int apply_cm = w.cm_taken ? 0 : 1;
+            if (l == c.n_levels - 1) {
+                const int last = (w.substep == n_inner - 1) ? 1 : 0;
+                prof_.begin(Prof::VV);
+                with_const<true, false>(c.integrator == INTEG_MTS_LANGEVIN, [&](auto LG) {
+                    mts_kick_drift_kernel<T, LG><<<grid, VV_THREADS, 0, stream_>>>(
+                        n, dt_v, (T)dt_x, (T)(dt_x / 2), c.skin_half2, c.lc, w.substep, apply_cm, last, cm, f, d_xref4_.as<T4>(),
+                        d_pos4_.as<T4>(), d_vel4_.as<T4>(), d_orig_.as<int>(), c.flag_ptr, ctl, cap ? cap->rebuild : 0,
+                        cap && path_ == 1 ? 1 : 0, ext_map());
+                });
+                prof_.end(Prof::VV);
+                launches_++;
+                first_kick_done();
+                w.substep++;
+                if (last) {
+                    if (path_ == 0) {
+                        wrap_kernel<T><<<(n + 255) / 256, 256, 0, stream_>>>(n, geom(), d_pos4_.as<T4>());
+                        launches_++;
+                    } else if (cap) {
+                        MB_TRY(splice_rebuild(*cap));
+                    } else if (rebuild_every_ == 0 || o.rebuild_hint) {
+                        MB_TRY(enqueue_rebuild(true, false));
+                    }
+                }
+            } else {
+                prof_.begin(Prof::VV);
+                mts_kick_kernel<T><<<grid, VV_THREADS, 0, stream_>>>(n, dt_v, apply_cm, cm, f, d_vel4_.as<T4>());
+                prof_.end(Prof::VV);
+                launches_++;
+                first_kick_done();
+                MB_TRY(enqueue_mts_level(c, o, cap, l + 1, true, w));
+            }
+            MB_TRY(mts_forces(l));
+            prof_.begin(Prof::VV);
+            if (l == 0) {  // K2: the closing kick of the outer step, with sum(m v) and v_cm
+                MB_TRY(integ_grid(grid, n, 2, 8, 3));
+                vv_kick2_kernel<T, false><<<grid, VV_THREADS, 0, stream_>>>(0, n, dt_v, o.do_cm, c.inv_mass, d_f4_.as<T4>(), d_mass_.as<T>(),
+                                                                            d_vel4_.as<T4>(), d_partial_.as<double>(), ctl, cm, nullptr,
+                                                                            PeerSignal{}, VCouple{});
+            } else {
+                mts_kick_kernel<T><<<grid, VV_THREADS, 0, stream_>>>(n, dt_v, 0, cm, f, d_vel4_.as<T4>());
+            }
+            prof_.end(Prof::VV);
+            launches_++;
+            recompute = false;
+        }
+        MB_CUDA(cudaGetLastError());
+        return MB_OK;
+    }
+    int enqueue_mts_step(const StepCfg& c, const StepOpts& o, Capture* cap) {
+        MtsWalk w;
+        MB_TRY(enqueue_mts_level(c, o, cap, 0, false, w));
+        if (o.log_mask) MB_TRY(enqueue_log(c, o.log_mask));
+        MB_CUDA(cudaGetLastError());
+        return MB_OK;
+    }
     // Record the state after the current step (LOG_* mask; single-GPU runs). The energy is a second evaluation at the same
     // positions by the ENERGY variants into a scratch force buffer: the trajectory keeps the forces of the plain kernels,
     // so logging does not change it.
@@ -1902,11 +2048,13 @@ class Engine : public EngineBase {
     struct GraphKey {
         int do_cm, log_mask, integrator;  // INTEG_*
         double dt, andersen_kT, andersen_prob;
-        double integ_kT, friction, damping;  // Langevin's kT and friction, or Nose-Hoover's kT and damping
+        double integ_kT, friction, damping;  // Langevin's (MTSLangevinIntegrator's) kT and friction, or Nose-Hoover's kT and damping
         mb_vcoupling_t vc;                   // the velocity-rescaling thermostat (K2's arguments)
+        int n_levels;                        // the multiple-time-step integrators' ordered fractions (0 levels: none)
+        std::array<int, MTS_MAX_LEVELS> fractions;
         auto fields() const {
             return std::tie(do_cm, log_mask, integrator, dt, andersen_kT, andersen_prob, integ_kT, friction, damping, vc.kind,
-                            vc.n_steps, vc.kT, vc.tau);
+                            vc.n_steps, vc.kT, vc.tau, n_levels, fractions);
         }
         bool operator==(const GraphKey& o) const { return fields() == o.fields(); }
     };
@@ -1983,7 +2131,8 @@ class Engine : public EngineBase {
         return MB_OK;
     }
     // One MD step (K1, [IF rebuild], force, K2, [thermostat], [log records]; Langevin: L, [IF rebuild], force,
-    // [log records]; Nose-Hoover: NH1, [IF rebuild], force, NH2, [log records]) as an executable graph.
+    // [log records]; Nose-Hoover: NH1, [IF rebuild], force, NH2, [log records]; multiple time steps: the unrolled substeps
+    // of enqueue_mts_step, [log records]) as an executable graph.
     int build_step_graph(const StepCfg& c, const GraphKey& key) {
         StepOpts o;
         o.do_cm = c.do_cm;
@@ -2087,10 +2236,10 @@ class Engine : public EngineBase {
         return MB_OK;
     }
 
-    // mb_simulate_vv, mb_simulate_vv_log, mb_simulate_langevin and mb_simulate_nose_hoover: one body, one step loop, one
-    // graph builder
+    // mb_simulate_vv, mb_simulate_vv_log, mb_simulate_langevin, mb_simulate_nose_hoover and mb_simulate_mts: one body, one
+    // step loop, one graph builder
     int simulate(void* coords, void* vels, const mb_vv_params_t* p, const mb_langevin_params_t* lg, const mb_nosehoover_params_t* nh,
-                 mb_log_t* log) override {
+                 const mb_mts_params_t* mts, mb_log_t* log) override {
         MB_TRY(prepare());
         if (!coords || !vels || !p) return set_error(MB_ERR_INVALID, "null argument");
         if (p->n_steps < 0 || !(p->dt > 0)) return set_error(MB_ERR_INVALID, "n_steps < 0 or dt <= 0");
@@ -2106,11 +2255,31 @@ class Engine : public EngineBase {
                 return set_error(MB_ERR_INVALID, "mb_simulate_nose_hoover: damping must be finite and > 0");
             if (n_ < 2) return set_error(MB_ERR_INVALID, "mb_simulate_nose_hoover: needs at least 2 atoms (Nf = 3N - 3 > 0)");
         }
-        if (lg || nh) {
-            const std::string who = lg ? "mb_simulate_langevin" : "mb_simulate_nose_hoover";
+        if (mts) {
+            if (mts->n_levels < 1 || mts->n_levels > MB_MTS_MAX_LEVELS)
+                return set_error(MB_ERR_INVALID, "mb_simulate_mts: n_levels must be in 1 .. MB_MTS_MAX_LEVELS");
+            if (mts->fractions[0] != 1) return set_error(MB_ERR_INVALID, "mb_simulate_mts: the first ordered fraction must be 1");
+            for (int l = 1; l < mts->n_levels; l++)
+                if (!(mts->fractions[l] > mts->fractions[l - 1] && mts->fractions[l] % mts->fractions[l - 1] == 0))
+                    return set_error(MB_ERR_INVALID, "mb_simulate_mts: fraction " + std::to_string(mts->fractions[l]) +
+                                                         " is not a larger multiple of fraction " + std::to_string(mts->fractions[l - 1]));
+            if (mts->fractions[mts->n_levels - 1] > 1024)
+                return set_error(MB_ERR_INVALID, "mb_simulate_mts: more than 1024 innermost substeps per outer step");
+            if (max_specific_level() >= mts->n_levels)
+                return set_error(MB_ERR_INVALID, "mb_simulate_mts: a specific interaction sits at level " + std::to_string(max_specific_level()) +
+                                                     " of " + std::to_string(mts->n_levels) + " (mb_set_specific_levels)");
+            if (mts->langevin) {
+                if (!(std::isfinite(mts->kT) && mts->kT >= 0)) return set_error(MB_ERR_INVALID, "mb_simulate_mts: kT must be finite and >= 0");
+                if (!(std::isfinite(mts->friction) && mts->friction >= 0))
+                    return set_error(MB_ERR_INVALID, "mb_simulate_mts: friction must be finite and >= 0");
+            }
+        }
+        if (lg || nh || mts) {
+            const std::string who = lg ? "mb_simulate_langevin" : (nh ? "mb_simulate_nose_hoover" : "mb_simulate_mts");
             if (vcoupling.kind != MB_VC_NONE)
                 return set_error(MB_ERR_INVALID, who + ": a velocity coupling is set on the context (couplings with " +
-                                                     (lg ? "Langevin" : "Nose-Hoover") + " are not supported)");
+                                                     (lg ? "Langevin" : (nh ? "Nose-Hoover" : "the multiple-time-step integrators")) +
+                                                     " are not supported)");
             if (decomposed()) return set_error(MB_ERR_INVALID, who + ": not available in decomposed (multi-GPU) runs");
         }
         if (vcoupling.kind != MB_VC_NONE) {
@@ -2142,6 +2311,20 @@ class Engine : public EngineBase {
         c.integrator = lg ? INTEG_LANGEVIN : (nh ? INTEG_NH : INTEG_VV);
         c.lc = LangevinCoef{1.0, 0.0, 0.0};
         c.nc = NhCoef{0.0, 1.0};
+        c.n_levels = 0;
+        c.fractions.fill(0);
+        // one level without noise is the VelocityVerlet step: it runs as one
+        if (mts && (mts->langevin || mts->n_levels > 1)) {
+            c.integrator = mts->langevin ? INTEG_MTS_LANGEVIN : INTEG_MTS;
+            c.n_levels = mts->n_levels;
+            std::copy_n(mts->fractions, mts->n_levels, c.fractions.begin());
+            if (mts->langevin) {  // MTSLangevinIntegrator: vel_scale, noise_scale (src/simulators.jl:1736-1738), in double
+                c.lc.vel_scale = exp(-p->dt * mts->friction / mts->fractions[mts->n_levels - 1]);
+                c.lc.noise_scale = sqrt(1.0 - c.lc.vel_scale * c.lc.vel_scale);
+                c.lc.kT = mts->kT;
+            }
+            if (c.n_levels > 1) MB_CUDA(d_f4_mts_.ensure(((size_t)n_ + 16) * sizeof(T4)));
+        }
         if (nh) {  // NoseHoover(dt, temperature, damping): dt / (2 damping^2) and Nf k T0 (src/simulators.jl:1575-1579), in double
             c.nc.coef = p->dt / (2.0 * nh->damping * nh->damping);
             c.nc.nf_kT = (double)(3 * (long long)n_ - 3) * nh->kT;
@@ -2202,7 +2385,7 @@ class Engine : public EngineBase {
             MB_TRY(p2p_setup());  // collective; falls back to the NCCL transport on every rank if any mapping fails
         }
         MB_TRY(launch_pairs(false, d_f4_.as<T4>(), dec));
-        MB_TRY(launch_bonded(false));
+        MB_TRY(launch_bonded(false, nullptr, is_mts(c.integrator) ? 0 : -1));  // (multiple time steps: F_0 of level 0)
         if (dec) {
             const unsigned long long e0 = ++epoch_;  // this force evaluation read the replicated state: tell the pushers
             if (p2p_active()) {
@@ -2225,8 +2408,10 @@ class Engine : public EngineBase {
             // one executable per log mask this call uses (the plain step and the log steps)
             bool need[8] = {false, false, false, false, false, false, false, false};
             for (int64_t k = 1; k <= p->n_steps; k++) need[log_mask_at(log, p->init_step + k)] = true;
-            GraphKey key{c.do_cm, 0, c.integrator, p->dt, p->andersen_kT, p->andersen_prob, lg ? lg->kT : (nh ? nh->kT : 0.0),
-                         lg ? lg->friction : 0.0, nh ? nh->damping : 0.0, vcoupling};
+            GraphKey key{c.do_cm, 0, c.integrator, p->dt, p->andersen_kT, p->andersen_prob,
+                         lg ? lg->kT : (nh ? nh->kT : (c.integrator == INTEG_MTS_LANGEVIN ? mts->kT : 0.0)),
+                         lg ? lg->friction : (c.integrator == INTEG_MTS_LANGEVIN ? mts->friction : 0.0), nh ? nh->damping : 0.0,
+                         vcoupling, c.n_levels, c.fractions};
             for (int m = 0; m < 8 && use_graph; m++) {
                 if (!need[m]) continue;
                 key.log_mask = m;
@@ -2264,7 +2449,7 @@ class Engine : public EngineBase {
                 }
                 StepOpts o;
                 o.do_cm = do_cm;
-                o.clear_cm_after_k1 = clear_after_k1 && c.integrator == INTEG_VV;
+                o.clear_cm_after_k1 = clear_after_k1 && (c.integrator == INTEG_VV || is_mts(c.integrator));
                 o.rebuild_hint = hint;
                 o.defer_cm = k < p->n_steps;
                 o.log_mask = log_mask_at(log, step_n);
@@ -2596,6 +2781,12 @@ class Engine : public EngineBase {
     int plan_key_[3] = {-1, -1, -1};
     int64_t sp_n_[3] = {0, 0, 0};
     DevBuf d_sp_idx_k_[3], d_sp_par_k_[3], d_sp_partial_, d_sp_energy_;
+    // the terms as mb_set_specific received them, their multiple-time-step levels, and the level ranges of the device arrays
+    std::vector<int> h_sp_idx_[3];
+    std::vector<T> h_sp_par_[3];
+    std::vector<int32_t> h_sp_level_[3];
+    int64_t sp_lvl_off_[3][MTS_MAX_LEVELS + 1] = {};
+    DevBuf d_f4_mts_;  // forces of the inner multiple-time-step levels (slot order; fixed address: the step graphs bake it in)
     // PME (pme.cuh)
     bool pme_on_ = false, pme_ready_ = false;
     double pme_rc_ = 0, pme_tol_ = 0, pme_epsr_ = 1, pme_alpha_ = 0, pme_self_e_ = 0, pme_ke_ = 138.93545764;
@@ -2717,6 +2908,10 @@ int mb_set_specific(mb_ctx* ctx, int kind, int64_t n_terms, const int32_t* atom_
     MB_CTX_GUARD(ctx);
     return ctx->e->set_specific(kind, n_terms, atom_idx, params);
 }
+int mb_set_specific_levels(mb_ctx* ctx, int kind, int64_t n_terms, const int32_t* level) {
+    MB_CTX_GUARD(ctx);
+    return ctx->e->set_specific_levels(kind, n_terms, level);
+}
 int mb_set_pme(mb_ctx* ctx, double r_cut, double error_tol, int order, double eps_r, int64_t n_pairs, const int32_t* pi, const int32_t* pj) {
     MB_CTX_GUARD(ctx);
     return ctx->e->set_pme(r_cut, error_tol, order, eps_r, n_pairs, pi, pj);
@@ -2727,22 +2922,31 @@ int mb_random_velocities(mb_ctx* ctx, void* vels, double kT, uint64_t rng_ctr1, 
     return ctx->e->random_velocities(vels, kT, rng_ctr1, rng_key);
 }
 int mb_kinetic_energy_tensor(mb_ctx* ctx, const void* vels, double* ke_tensor9_host) { MB_CTX_GUARD(ctx); return ctx->e->kinetic_tensor(vels, ke_tensor9_host); }
-int mb_simulate_vv(mb_ctx* ctx, void* coords, void* vels, const mb_vv_params_t* p) { MB_CTX_GUARD(ctx); return ctx->e->simulate(coords, vels, p, nullptr, nullptr, nullptr); }
+int mb_simulate_vv(mb_ctx* ctx, void* coords, void* vels, const mb_vv_params_t* p) {
+    MB_CTX_GUARD(ctx);
+    return ctx->e->simulate(coords, vels, p, nullptr, nullptr, nullptr, nullptr);
+}
 int mb_simulate_vv_log(mb_ctx* ctx, void* coords, void* vels, const mb_vv_params_t* p, mb_log_t* log) {
     MB_CTX_GUARD(ctx);
-    return ctx->e->simulate(coords, vels, p, nullptr, nullptr, log);
+    return ctx->e->simulate(coords, vels, p, nullptr, nullptr, nullptr, log);
 }
 int mb_simulate_langevin(mb_ctx* ctx, void* coords, void* vels, const mb_langevin_params_t* p, mb_log_t* log) {
     MB_CTX_GUARD(ctx);
     if (!p) return mb::set_error(MB_ERR_INVALID, "null argument");
     const mb_vv_params_t vp = {p->dt, p->n_steps, p->init_step, p->remove_cm_every, 0.0, 0.0, p->rng_ctr1, p->rng_key};
-    return ctx->e->simulate(coords, vels, &vp, p, nullptr, log);
+    return ctx->e->simulate(coords, vels, &vp, p, nullptr, nullptr, log);
 }
 int mb_simulate_nose_hoover(mb_ctx* ctx, void* coords, void* vels, const mb_nosehoover_params_t* p, mb_log_t* log) {
     MB_CTX_GUARD(ctx);
     if (!p) return mb::set_error(MB_ERR_INVALID, "null argument");
     const mb_vv_params_t vp = {p->dt, p->n_steps, p->init_step, p->remove_cm_every, 0.0, 0.0, 0, 0};
-    return ctx->e->simulate(coords, vels, &vp, nullptr, p, log);
+    return ctx->e->simulate(coords, vels, &vp, nullptr, p, nullptr, log);
+}
+int mb_simulate_mts(mb_ctx* ctx, void* coords, void* vels, const mb_mts_params_t* p, mb_log_t* log) {
+    MB_CTX_GUARD(ctx);
+    if (!p) return mb::set_error(MB_ERR_INVALID, "null argument");
+    const mb_vv_params_t vp = {p->dt, p->n_steps, p->init_step, p->remove_cm_every, 0.0, 0.0, p->rng_ctr1, p->rng_key};
+    return ctx->e->simulate(coords, vels, &vp, nullptr, nullptr, p, log);
 }
 int mb_minimize_sd(mb_ctx* ctx, void* coords, mb_sd_params_t* p) { MB_CTX_GUARD(ctx); return ctx->e->minimize_sd(coords, p); }
 int mb_set_velocity_coupling(mb_ctx* ctx, const mb_vcoupling_t* c) {
