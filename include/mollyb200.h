@@ -179,6 +179,37 @@ int mb_set_pme(mb_ctx* ctx, double r_cut, double error_tol, int order, double ep
 int mb_pme_plan(const double box[3], double r_cut, double error_tol, int order, double* alpha_out, int32_t mesh_out[3],
                 double* moduli_out, int capacity);
 
+/* Generalized-Born implicit solvent: the ImplicitSolventOBC and ImplicitSolventGBN2 general interactions
+ * (src/interactions/implicit_solvent.jl). One path for OBC1, OBC2 and GBN2: they differ only in their data. The caller
+ * passes what the reference's structs hold (radii derived from elements stay outside the library):
+ *   offset_radii, scaled_offset_radii, alpha, beta, gamma: n doubles each, original atom order (OBC broadcasts its three
+ *     scalars); scaled radii may be negative (GBN2's sulphur screen);
+ *   neck_class: n int32 in [0, n_neck_classes) (NULL when n_neck_classes == 0); d0, m0: row-major n_neck_classes^2 doubles,
+ *     entry [c_i * n_neck_classes + c_j] = the reference's d0s[i, j] / m0s[i, j] for atoms i, j of classes c_i, c_j (the
+ *     tables are not symmetric). Host pointers; the arrays are copied.
+ * Charges come from the atoms. Three all-pairs passes over every ordered pair (O(N^2), no neighbour list; dist_cutoff > 0
+ * drops pairs beyond it and shifts the pair energy by -1/dist_cutoff as the reference does), deterministic (no atomics).
+ * Once set, mb_forces_energy_all, every integrator's step (inside the captured step graphs), the loggers' energies, the
+ * minimiser and level 0 of mb_simulate_mts add the GB forces and energy after the bonded terms; mb_forces / mb_energy stay
+ * pairwise-only. Setting it drops the captured graphs. p == NULL switches it off.
+ * MB_ERR_STATE: atoms not set. MB_ERR_INVALID: non-finite values, an offset radius <= 0, a negative offset or cutoff, a
+ * neck class out of range, n_neck_classes outside 0 .. MB_GB_MAX_NECK_CLASSES, a decomposed (multi-GPU) context. Changing
+ * the atom count afterwards makes the next evaluation fail until this is called again. There is no GB virial ("Not
+ * currently compatible with virial calculation" in the reference): the virial entry points are pairwise-only. */
+#define MB_GB_MAX_NECK_CLASSES 32
+typedef struct {
+    double dist_cutoff;                   /* inter.dist_cutoff in nm; 0 = none (what setup.jl builds) */
+    double offset, probe_radius, sa_factor;
+    double factor_solute, factor_solvent; /* as the structs hold them (-k / eps_solute, k / eps_solvent) */
+    double kappa;                         /* nm^-1 */
+    double neck_scale, neck_cut;          /* used only when n_neck_classes > 0 */
+    int32_t use_ace;
+    int32_t n_neck_classes;               /* 0: OBC (no neck term); > 0: GBN2 */
+} mb_gbsa_t;
+int mb_set_implicit_solvent(mb_ctx* ctx, const mb_gbsa_t* p, const double* offset_radii, const double* scaled_offset_radii,
+                            const double* alpha, const double* beta, const double* gamma, const int32_t* neck_class,
+                            const double* d0, const double* m0);
+
 /* simulate!(sys, VelocityVerlet(dt, coupling, remove_CM_motion), n_steps) hot loop
  * (src/simulators.jl:547-668): wrap, [CM removal when init_step==0], neighbours, F0, then n_steps of
  * kick / drift / wrap / forces / kick / CM removal (every remove_cm_every steps; 0 = never) /

@@ -16,7 +16,10 @@
 # and falls through to the stock methods (invoke) for anything it does not recognise: non-cubic boundaries,
 # constraints, virtual sites, couplings other than one AndersenThermostat, ImmediateThermostat, BerendsenThermostat or
 # VelocityRescaleThermostat, interactions outside
-# {LennardJones, Coulomb, CoulombReactionField, CoulombEwald} or unsupported cutoffs / mixing rules.
+# {LennardJones, Coulomb, CoulombReactionField, CoulombEwald} or unsupported cutoffs / mixing rules, general interactions
+# other than LJDispersionCorrection and one ImplicitSolventOBC / ImplicitSolventGBN2 (implicit solvent runs in the engine).
+# forces(sys) / potential_energy(sys) keep Molly's own evaluation of general interactions, implicit solvent included: the
+# seam this file overrides there is the pairwise loop.
 
 module MollyB200Ext
 
@@ -92,6 +95,22 @@ struct MBMTSParams
     rng_ctr1::UInt64
     rng_key::UInt64
 end
+
+# mb_gbsa_t (mb_set_implicit_solvent)
+struct MBGbsa
+    dist_cutoff::Float64
+    offset::Float64
+    probe_radius::Float64
+    sa_factor::Float64
+    factor_solute::Float64
+    factor_solvent::Float64
+    kappa::Float64
+    neck_scale::Float64
+    neck_cut::Float64
+    use_ace::Int32
+    n_neck_classes::Int32
+end
+const MB_GB_MAX_NECK_CLASSES = 32
 
 # mb_vcoupling_t (mb_set_velocity_coupling)
 struct MBVCoupling
@@ -301,6 +320,65 @@ function set_specific!(ctx::Context, sys)
     return true
 end
 
+# ---- implicit solvent: ImplicitSolventOBC / ImplicitSolventGBN2 -> mb_set_implicit_solvent ----------------------------
+# The engine adds the GB forces and energy in every integrator's step, the loggers' energies, the minimiser and MTS level 0.
+# It takes what the structs hold (src/interactions/implicit_solvent.jl:337-583), with units stripped in the System's units.
+# GBN2's n x n d0s / m0s tables become neck classes: atoms of equal radius (offset_radii .+ offset) share a class, and the
+# class pair (c_i, c_j) reads d0s[i, j] of one representative pair (the tables are filled by radius, lookup_table :290-320).
+is_gb(gi) = gi isa Molly.ImplicitSolventOBC || gi isa Molly.ImplicitSolventGBN2
+# the general interactions a takeover accepts: LJDispersionCorrection (no force) and at most one GB term
+general_ok(sys) = all(gi -> gi isa Molly.LJDispersionCorrection || is_gb(gi), sys.general_inters) &&
+                  count(is_gb, sys.general_inters) <= 1
+_f64(x) = Float64(ustrip(x))
+_vec(a) = Float64.(ustrip.(Array(a)))
+
+# (MBGbsa, per-atom arrays (offset radii, scaled offset radii, alpha, beta, gamma), neck (classes, d0, m0) or nothing),
+# or nothing when the term has more neck classes than the engine takes
+function gb_desc(inter)
+    or_, sr = _vec(inter.offset_radii), _vec(inter.scaled_offset_radii)
+    n = length(or_)
+    p = (_f64(inter.dist_cutoff), _f64(inter.offset), _f64(inter.probe_radius), _f64(inter.sa_factor),
+         _f64(inter.factor_solute), _f64(inter.factor_solvent), _f64(inter.kappa))
+    if inter isa Molly.ImplicitSolventOBC
+        abg = [fill(_f64(v), n) for v in (inter.α, inter.β, inter.γ)]
+        return MBGbsa(p..., 0.0, 0.0, Int32(inter.use_ACE), Int32(0)), (or_, sr, abg...), nothing
+    end
+    radii = or_ .+ _f64(inter.offset)
+    distinct = sort(unique(radii))
+    nc = length(distinct)
+    nc <= MB_GB_MAX_NECK_CLASSES || return nothing
+    cls = Int32[searchsortedfirst(distinct, r) - 1 for r in radii]
+    reps = [findfirst(==(c), cls) for c in Int32(0):Int32(nc - 1)]
+    d0 = _vec(inter.d0s[reps, reps])                    # nc x nc gather on the device, then to the host
+    m0 = _vec(inter.m0s[reps, reps])
+    abg = (_vec(inter.αs), _vec(inter.βs), _vec(inter.γs))
+    # row-major for C: entry [c_i * nc + c_j] = d0s[i, j]
+    return MBGbsa(p..., Float64(inter.neck_scale), _f64(inter.neck_cut), Int32(inter.use_ACE), Int32(nc)),
+           (or_, sr, abg...), (cls, vec(permutedims(d0)), vec(permutedims(m0)))
+end
+# a GB term the engine cannot take sends the run to the stock path
+gb_ok(sys) = all(gi -> !is_gb(gi) || !isnothing(gb_desc(gi)), sys.general_inters)
+
+# set the System's GB term on the context, or clear it when there is none (done on every taken-over call, like
+# set_specific!); callers have checked gb_ok
+function set_implicit_solvent!(ctx::Context, sys)
+    i = findfirst(is_gb, sys.general_inters)
+    if isnothing(i)
+        check(ccall((:mb_set_implicit_solvent, LIB), Cint,
+                    (Ptr{Cvoid}, Ptr{MBGbsa}, Ptr{Float64}, Ptr{Float64}, Ptr{Float64}, Ptr{Float64}, Ptr{Float64},
+                     Ptr{Int32}, Ptr{Float64}, Ptr{Float64}),
+                    ctx.handle, C_NULL, C_NULL, C_NULL, C_NULL, C_NULL, C_NULL, C_NULL, C_NULL, C_NULL))
+        return nothing
+    end
+    p, (or_, sr, a, b, g), neck = gb_desc(sys.general_inters[i])
+    cls, d0, m0 = isnothing(neck) ? (Int32[0], Float64[0.0], Float64[0.0]) : neck   # (unread when n_neck_classes == 0)
+    check(ccall((:mb_set_implicit_solvent, LIB), Cint,
+                (Ptr{Cvoid}, Ref{MBGbsa}, Ptr{Float64}, Ptr{Float64}, Ptr{Float64}, Ptr{Float64}, Ptr{Float64},
+                 Ptr{Int32}, Ptr{Float64}, Ptr{Float64}),
+                ctx.handle, Ref(p), or_, sr, a, b, g, cls, d0, m0))
+    return nothing
+end
+
 # ---- multi-GPU: one Julia process per GPU (MPI.jl / Distributed); the reference has nothing here -----------
 # rank 0: id = comm_unique_id(); broadcast the 128 bytes; every rank: comm_init!(sys, id, rank, nranks).
 function comm_unique_id()
@@ -322,8 +400,9 @@ end
 # and the records are pushed into the loggers' histories afterwards; otherwise loggers fire between chunks of
 # gcd(logger n_steps) steps (SURVEY.md Appendix A.11). Like the rest of this file, this has only been checked by reading.
 function takeover_params(sys, sim::VelocityVerlet, n_steps, init_step, rng)
-    # LJDispersionCorrection adds no force (lennard_jones.jl:252-275); anything else (PME, implicit solvent) -> stock path
-    all(gi -> gi isa Molly.LJDispersionCorrection, sys.general_inters) || return nothing
+    # LJDispersionCorrection adds no force (lennard_jones.jl:252-275), implicit solvent runs in the engine
+    # (set_implicit_solvent!); anything else (PME) -> stock path
+    general_ok(sys) && gb_ok(sys) || return nothing
     all(!isnothing, map(specific_desc, sys.specific_inter_lists)) || return nothing
     kT, prob = 0.0, 0.0
     vc = nothing
@@ -373,6 +452,7 @@ function Molly.simulate!(sys::System{3, <:CuArray, T}, sim::VelocityVerlet, n_st
     p, vc = tp
     ctx = context_for(sys, descs)
     set_specific!(ctx, sys)
+    set_implicit_solvent!(ctx, sys)
     set_velocity_coupling!(ctx, vc)
     if run_loggers != false && !isempty(sys.loggers) && all(l -> !isnothing(device_log_kind(l)), values(sys.loggers))
         return simulate_logged!(sys, ctx, p, n_steps, init_step, run_loggers)
@@ -403,7 +483,7 @@ function Molly.simulate!(sys::System{3, <:CuArray, T}, sim::Langevin, n_steps::I
     device_logs = run_loggers == false || isempty(sys.loggers) ||
                   all(l -> !isnothing(device_log_kind(l)), values(sys.loggers))
     if isnothing(descs) || !isnothing(sim.coupling) || !device_logs ||
-            !all(gi -> gi isa Molly.LJDispersionCorrection, sys.general_inters) ||
+            !general_ok(sys) || !gb_ok(sys) ||
             !all(!isnothing, map(specific_desc, sys.specific_inter_lists))
         # stock: simulate!(sys, sim::Langevin, n_steps_or_time; ...) src/simulators.jl:1101
         return invoke(Molly.simulate!, Tuple{Any, Langevin, Any}, sys, sim, n_steps;
@@ -411,6 +491,7 @@ function Molly.simulate!(sys::System{3, <:CuArray, T}, sim::Langevin, n_steps::I
     end
     ctx = context_for(sys, descs)
     set_specific!(ctx, sys)
+    set_implicit_solvent!(ctx, sys)
     set_velocity_coupling!(ctx, nothing)
     friction = sim.friction isa Unitful.Quantity ? Float64(ustrip(u"ps^-1", sim.friction)) : Float64(sim.friction)
     p = MBLangevinParams(_ps(sim.dt), n_steps, init_step, Int32(sim.remove_CM_motion),
@@ -437,7 +518,7 @@ function Molly.simulate!(sys::System{3, <:CuArray, T}, sim::NoseHoover, n_steps:
     device_logs = run_loggers == false || isempty(sys.loggers) ||
                   all(l -> !isnothing(device_log_kind(l)), values(sys.loggers))
     if isnothing(descs) || !isnothing(sim.coupling) || !device_logs ||
-            !all(gi -> gi isa Molly.LJDispersionCorrection, sys.general_inters) ||
+            !general_ok(sys) || !gb_ok(sys) ||
             !all(!isnothing, map(specific_desc, sys.specific_inter_lists))
         # stock: simulate!(sys, sim::NoseHoover, n_steps_or_time; ...) src/simulators.jl:1534
         return invoke(Molly.simulate!, Tuple{Any, NoseHoover, Any}, sys, sim, n_steps;
@@ -445,6 +526,7 @@ function Molly.simulate!(sys::System{3, <:CuArray, T}, sim::NoseHoover, n_steps:
     end
     ctx = context_for(sys, descs)
     set_specific!(ctx, sys)
+    set_implicit_solvent!(ctx, sys)
     set_velocity_coupling!(ctx, nothing)
     p = MBNoseHooverParams(_ps(sim.dt), n_steps, init_step, Int32(sim.remove_CM_motion),
                            Float64(ustrip(sys.k * sim.temperature)), _ps(sim.damping))
@@ -483,7 +565,8 @@ function Molly.simulate!(sys::System{3, <:CuArray, T}, sim::Molly.AbstractMTSInt
             length(sim.si_fractions) != length(sys.specific_inter_lists) ||
             length(sim.gi_fractions) != length(sys.general_inters) ||
             length(sim.ordered_fractions) > 8 || last(sim.ordered_fractions) > 1024 ||
-            !all(gi -> gi isa Molly.LJDispersionCorrection, sys.general_inters) ||
+            !general_ok(sys) || !gb_ok(sys) ||
+            any(((gi, f),) -> is_gb(gi) && f != 1, zip(sys.general_inters, sim.gi_fractions)) ||   # GB at level 0 only
             !all(!isnothing, map(specific_desc, sys.specific_inter_lists))
         # stock: simulate!(sys, sim::AbstractMTSIntegrator, n_steps_or_time; ...) src/simulators.jl:1850
         return invoke(Molly.simulate!, Tuple{Any, Molly.AbstractMTSIntegrator, Any}, sys, sim, n_steps;
@@ -492,6 +575,7 @@ function Molly.simulate!(sys::System{3, <:CuArray, T}, sim::Molly.AbstractMTSInt
     ctx = context_for(sys, descs)
     set_specific!(ctx, sys)
     set_specific_levels!(ctx, sys, sim)
+    set_implicit_solvent!(ctx, sys)
     set_velocity_coupling!(ctx, nothing)
     fr = zeros(Int32, 8)
     fr[1:length(sim.ordered_fractions)] .= sim.ordered_fractions
@@ -512,8 +596,8 @@ function Molly.simulate!(sys::System{3, <:CuArray, T}, sim::Molly.AbstractMTSInt
 end
 
 # ---- simulate!(sys, ::SteepestDescentMinimizer) (src/simulators.jl:183-274) ------------------------------------------------
-# Taken over when the System is engine-eligible, has no constraints, no general interactions (the engine would need their
-# energies for the log lines) and run_loggers is false: the whole minimisation is one mb_minimize_sd call, and the
+# Taken over when the System is engine-eligible, has no constraints, no general interactions other than one implicit
+# solvent term (the engine computes its energy; any other it would need for the log lines) and run_loggers is false: the whole minimisation is one mb_minimize_sd call, and the
 # reference's log lines are printed from the trace afterwards. Anything else runs the stock method.
 struct MBSDParams
     step_size::Float64
@@ -533,13 +617,14 @@ end
 function Molly.simulate!(sys::System{3, <:CuArray, T}, sim::SteepestDescentMinimizer; init_step=0, run_loggers=false,
                          kwargs...) where T
     descs = engine_eligible(sys, sys.pairwise_inters)
-    if isnothing(descs) || run_loggers != false || !isempty(sys.general_inters) ||
-            !all(!isnothing, map(specific_desc, sys.specific_inter_lists))
+    if isnothing(descs) || run_loggers != false || !all(is_gb, sys.general_inters) || length(sys.general_inters) > 1 ||
+            !gb_ok(sys) || !all(!isnothing, map(specific_desc, sys.specific_inter_lists))
         return invoke(Molly.simulate!, Tuple{Any, SteepestDescentMinimizer}, sys, sim;
                       init_step=init_step, run_loggers=run_loggers, kwargs...)
     end
     ctx = context_for(sys, descs)
     set_specific!(ctx, sys)
+    set_implicit_solvent!(ctx, sys)
     trace = zeros(Float64, 4, sim.max_steps + 1)   # (step, E or E_trial, max force, accepted) per column
     p = Ref(MBSDParams(Float64(ustrip(sim.step_size)), sim.max_steps, Float64(ustrip(sim.tol)), init_step,
                        pointer(trace), sim.max_steps + 1, 0, 0.0, 0.0, 0.0, Int32(0), Int32(0)))

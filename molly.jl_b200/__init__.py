@@ -17,4 +17,4 @@ from .api import (Atom, CubicBoundary, TriclinicBoundary, System, NoCutoff, Dist
                   comm_unique_id, comm_init, decomp_plan, InteractionList2Atoms, InteractionList3Atoms,
                   InteractionList4Atoms, PotentialEnergyLogger, KineticEnergyLogger, TotalEnergyLogger, TemperatureLogger,
                   CoordinatesLogger, VelocitiesLogger, values, record_steps, SteepestDescentMinimizer, steepest_descent,
-                  sd_log_lines)
+                  sd_log_lines, ImplicitSolventOBC, ImplicitSolventGBN2)

@@ -22,8 +22,9 @@ EXPORTED = [
     "mb_comm_init", "mb_decomp_plan", "mb_set_profiling", "mb_set_specific", "mb_forces_energy_all", "mb_set_pme", "mb_pme_plan",
     "mb_set_lj_dispersion_correction", "mb_random_velocities", "mb_kinetic_energy_tensor", "mb_set_box_triclinic",
     "mb_simulate_vv_log", "mb_minimize_sd", "mb_set_velocity_coupling", "mb_simulate_langevin",
-    "mb_simulate_nose_hoover", "mb_set_specific_levels", "mb_simulate_mts",
+    "mb_simulate_nose_hoover", "mb_set_specific_levels", "mb_simulate_mts", "mb_set_implicit_solvent",
 ]
+MB_GB_MAX_NECK_CLASSES = 32
 MB_MTS_MAX_LEVELS = 8
 
 
@@ -33,6 +34,14 @@ class MBInter(C.Structure):
         ("weight_special", C.c_double), ("coulomb_const", C.c_double), ("solvent_dielectric", C.c_double),
         ("ewald_alpha", C.c_double), ("sigma_mix", C.c_int32), ("eps_mix", C.c_int32), ("approx_erfc", C.c_int32),
         ("use_neighbors", C.c_int32),
+    ]
+
+
+class MBGbsa(C.Structure):
+    _fields_ = [
+        ("dist_cutoff", C.c_double), ("offset", C.c_double), ("probe_radius", C.c_double), ("sa_factor", C.c_double),
+        ("factor_solute", C.c_double), ("factor_solvent", C.c_double), ("kappa", C.c_double), ("neck_scale", C.c_double),
+        ("neck_cut", C.c_double), ("use_ace", C.c_int32), ("n_neck_classes", C.c_int32),
     ]
 
 
@@ -155,6 +164,7 @@ def load():
     L.mb_pme_plan.argtypes = [vp, C.c_double, C.c_double, C.c_int, vp, vp, vp, C.c_int]
     L.mb_forces_energy_all.argtypes = [vp, vp, vp, vp, i64]
     L.mb_set_lj_dispersion_correction.argtypes = [vp, dbl]
+    L.mb_set_implicit_solvent.argtypes = [vp, C.POINTER(MBGbsa), vp, vp, vp, vp, vp, vp, vp, vp]
     L.mb_random_velocities.argtypes = [vp, vp, dbl, C.c_uint64, C.c_uint64]
     L.mb_kinetic_energy_tensor.argtypes = [vp, vp, C.POINTER(dbl)]
     L.mb_decomp_plan.argtypes = [C.c_int, C.c_int, C.c_int, C.c_int, vp, vp, C.POINTER(i32), vp, C.POINTER(i32), C.c_int]

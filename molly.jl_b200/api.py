@@ -283,6 +283,105 @@ class LJDispersionCorrection:
     dist_cutoff: float
 
 
+class _GBFactors:
+    """factor_solute = -k / eps_solute and factor_solvent = k / eps_solvent, zero for a zero dielectric
+    (implicit_solvent.jl:399-409), derived from the dielectrics whenever they are read."""
+
+    @property
+    def factor_solute(self):
+        return -COULOMB_CONST / self.solute_dielectric if self.solute_dielectric != 0 else 0.0
+
+    @property
+    def factor_solvent(self):
+        return COULOMB_CONST / self.solvent_dielectric if self.solvent_dielectric != 0 else 0.0
+
+
+@dataclass
+class ImplicitSolventOBC(_GBFactors):
+    """ImplicitSolventOBC general interaction (src/interactions/implicit_solvent.jl:337-432) at array level: per-atom
+    offset_radii (radius - offset) and scaled_offset_radii (screen x offset radius), the OBC alpha, beta, gamma (scalars;
+    GBOBCII: 1.0, 0.8, 4.85, GBOBCI: 0.8, 0.0, 2.909125) and the struct's scalars. Radii from elements (mbondi2_radii)
+    are the caller's, as the reference's constructor computes them. Run on the device by mb_set_implicit_solvent (three
+    all-pairs passes, inside the captured step graphs). No virial."""
+    offset_radii: object
+    scaled_offset_radii: object
+    alpha: float = 0.8
+    beta: float = 0.0
+    gamma: float = 2.909125
+    solvent_dielectric: float = 78.5
+    solute_dielectric: float = 1.0
+    kappa: float = 0.0
+    offset: float = 0.009
+    dist_cutoff: float = 0.0
+    probe_radius: float = 0.14
+    sa_factor: float = 28.3919551
+    use_ACE: bool = True
+
+    def __post_init__(self):
+        self.offset_radii = np.ascontiguousarray(self.offset_radii, np.float64)
+        self.scaled_offset_radii = np.ascontiguousarray(self.scaled_offset_radii, np.float64)
+        if self.offset_radii.shape != self.scaled_offset_radii.shape or self.offset_radii.ndim != 1:
+            raise ValueError("offset_radii and scaled_offset_radii must be 1-D arrays of the same length")
+
+    def per_atom(self):
+        n = len(self.offset_radii)
+        return [self.offset_radii, self.scaled_offset_radii] + [np.full(n, float(v)) for v in (self.alpha, self.beta, self.gamma)]
+
+    def neck(self):
+        return 0, None, None, None, 0.0, 0.0
+
+
+@dataclass
+class ImplicitSolventGBN2(_GBFactors):
+    """ImplicitSolventGBN2 general interaction (src/interactions/implicit_solvent.jl:443-583) at array level: per-atom
+    offset_radii, scaled_offset_radii, alphas, betas, gammas, and the neck lookup as classes: neck_class[i] in
+    [0, n_classes) and the tables d0[c_i, c_j] = the reference's d0s[i, j], m0 likewise (not symmetric), in nm and nm^-1.
+    Atoms of equal radius (offset_radii + offset) share a class. Run on the device by mb_set_implicit_solvent. No virial."""
+    offset_radii: object
+    scaled_offset_radii: object
+    alpha: object
+    beta: object
+    gamma: object
+    neck_class: object
+    d0: object
+    m0: object
+    solvent_dielectric: float = 78.5
+    solute_dielectric: float = 1.0
+    kappa: float = 0.0
+    offset: float = 0.0195141
+    dist_cutoff: float = 0.0
+    probe_radius: float = 0.14
+    sa_factor: float = 28.3919551
+    use_ACE: bool = True
+    neck_scale: float = 0.826836
+    neck_cut: float = 0.68
+
+    def __post_init__(self):
+        for name in ("offset_radii", "scaled_offset_radii", "alpha", "beta", "gamma"):
+            setattr(self, name, np.ascontiguousarray(getattr(self, name), np.float64))
+            if getattr(self, name).shape != np.shape(self.offset_radii) or getattr(self, name).ndim != 1:
+                raise ValueError(f"{name}: a 1-D array with one value per atom")
+        self.neck_class = np.ascontiguousarray(self.neck_class, np.int32)
+        self.d0 = np.ascontiguousarray(self.d0, np.float64)
+        self.m0 = np.ascontiguousarray(self.m0, np.float64)
+        nc = len(self.d0)
+        if self.neck_class.shape != self.offset_radii.shape:
+            raise ValueError("neck_class: one class per atom")
+        if self.d0.shape != (nc, nc) or self.m0.shape != (nc, nc) or not 0 < nc <= capi.MB_GB_MAX_NECK_CLASSES:
+            raise ValueError(f"d0 and m0 must be square tables of the same size, 1 .. {capi.MB_GB_MAX_NECK_CLASSES} classes")
+        if self.neck_class.min() < 0 or self.neck_class.max() >= nc:
+            raise ValueError("neck_class outside the tables")
+
+    def per_atom(self):
+        return [self.offset_radii, self.scaled_offset_radii, self.alpha, self.beta, self.gamma]
+
+    def neck(self):
+        return len(self.d0), self.neck_class, self.d0, self.m0, self.neck_scale, self.neck_cut
+
+
+_GB_TYPES = (ImplicitSolventOBC, ImplicitSolventGBN2)
+
+
 @dataclass
 class InteractionList2Atoms:
     """InteractionList2Atoms of HarmonicBond (src/types.jl:89-157, interactions/harmonic_bond.jl): 1-based is/js,
@@ -555,6 +654,9 @@ def mts_levels(sys, sim) -> dict:
         if isinstance(gi, PME) and f != 1:
             raise TypeError(f"{type(sim).__name__}: PME at a fraction other than 1 is not supported (the stock Molly "
                             "path handles it)")
+        if isinstance(gi, _GB_TYPES) and f != 1:
+            raise TypeError(f"{type(sim).__name__}: implicit solvent at a fraction other than 1 is not supported (the "
+                            "engine evaluates it with level 0)")
     parts = {}
     for sil, f in zip(sys.specific_inter_lists, sim.si_fractions):
         n = len(sil.arrays()[0])
@@ -799,13 +901,32 @@ class System:
             if isinstance(gi, LJDispersionCorrection):
                 capi.check(L.mb_set_lj_dispersion_correction(ctx, float(gi.dist_cutoff)))
                 continue
+            if isinstance(gi, _GB_TYPES):
+                self._set_implicit_solvent(gi)
+                continue
             if not isinstance(gi, PME):
-                raise ValueError("only PME and LJDispersionCorrection are supported as general interactions")
+                raise ValueError("only PME, LJDispersionCorrection, ImplicitSolventOBC and ImplicitSolventGBN2 are supported "
+                                 "as general interactions")
             pairs = np.zeros((0, 2), np.int32) if gi.excluded_pairs is None else np.asarray(gi.excluded_pairs, np.int32).reshape(-1, 2)
             pi, pj = np.ascontiguousarray(pairs[:, 0]), np.ascontiguousarray(pairs[:, 1])
             self._keep_pme = (pi, pj)
             capi.check(L.mb_set_pme(ctx, float(gi.dist_cutoff), float(gi.error_tol), int(gi.order), float(gi.eps_r), len(pi),
                                     pi.ctypes.data, pj.ctypes.data))
+
+    def _set_implicit_solvent(self, gi):
+        arrays = [np.ascontiguousarray(a, np.float64) for a in gi.per_atom()]
+        if any(len(a) != self.n for a in arrays):
+            raise ValueError(f"{type(gi).__name__}: per-atom arrays of {len(arrays[0])} atoms for a system of {self.n}")
+        nc, cls, d0, m0, neck_scale, neck_cut = gi.neck()
+        p = capi.MBGbsa(dist_cutoff=float(gi.dist_cutoff), offset=float(gi.offset), probe_radius=float(gi.probe_radius),
+                        sa_factor=float(gi.sa_factor), factor_solute=float(gi.factor_solute),
+                        factor_solvent=float(gi.factor_solvent), kappa=float(gi.kappa), neck_scale=float(neck_scale),
+                        neck_cut=float(neck_cut), use_ace=int(bool(gi.use_ACE)), n_neck_classes=int(nc))
+        keep = arrays + ([np.ascontiguousarray(cls, np.int32), np.ascontiguousarray(d0, np.float64).ravel(),
+                          np.ascontiguousarray(m0, np.float64).ravel()] if nc else [])
+        self._keep_gb = keep
+        ptr = [a.ctypes.data for a in keep] + ([None] * 3 if not nc else [])
+        capi.check(self._L.mb_set_implicit_solvent(self._ctx, C.byref(p), *ptr))
 
     def close(self):
         if self._ctx is not None:

@@ -14,6 +14,7 @@
 #include "cells.cuh"
 #include "common.cuh"
 #include "force.cuh"
+#include "gbsa.cuh"
 #include "langevin.cuh"
 #include "minimize.cuh"
 #include "mts.cuh"
@@ -344,6 +345,8 @@ class EngineBase {
     virtual int set_specific_levels(int kind, int64_t n, const int32_t* level) = 0;
     virtual int set_pme(double r_cut, double error_tol, int order, double eps_r, int64_t n_pairs, const int32_t* pi, const int32_t* pj) = 0;
     virtual int set_dispersion(double r_cut) = 0;
+    virtual int set_implicit_solvent(const mb_gbsa_t* p, const double* or_, const double* sr, const double* alpha, const double* beta,
+                                     const double* gamma, const int32_t* cls, const double* d0, const double* m0) = 0;
     virtual int random_velocities(void* vels, double kT, uint64_t ctr1, uint64_t key) = 0;
     virtual int kinetic_tensor(const void* vels, double* out9) = 0;
     virtual int minimize_sd(void* coords, mb_sd_params_t* p) = 0;
@@ -935,12 +938,12 @@ class Engine : public EngineBase {
         return m;
     }
     bool has_lists() const { return sp_n_[0] + sp_n_[1] + sp_n_[2] > 0; }
-    bool has_specific() const { return has_lists() || pme_on_; }  // everything that is added after the pair kernel
+    bool has_specific() const { return has_lists() || pme_on_ || gb_on_; }  // everything that is added after the pair kernel
     // the slot of every atom for kernels that index atoms in original order (null: the all-pairs path keeps that order)
     const int* slot_of() const { return path_ == 1 ? d_inv_orig_.as<int>() : nullptr; }
     // add the bonded forces to f4 (slot order on the brick path, original order on the all-pairs path; default d_f4_);
     // with energy: per-kernel partials are summed into d_sp_energy_ (double, device). level: the terms of one
-    // multiple-time-step level (PME belongs to level 0), or -1 for all of them
+    // multiple-time-step level (PME and GB belong to level 0), or -1 for all of them
     int launch_bonded(bool energy, T4* f4 = nullptr, int level = -1) {
         if (!f4) f4 = d_f4_.as<T4>();
         if (!has_specific() || (level > 0 && !has_lists())) return MB_OK;
@@ -978,6 +981,128 @@ class Engine : public EngineBase {
         }
         MB_CUDA(cudaGetLastError());
         if (pme_on_ && level <= 0) MB_TRY(launch_pme(energy, f4));
+        if (gb_on_ && level <= 0) MB_TRY(launch_gb(energy, f4));
+        return MB_OK;
+    }
+
+    // ---- generalized-Born implicit solvent (gbsa.cuh) -------------------------------------------------------------------
+    int set_implicit_solvent(const mb_gbsa_t* p, const double* or_, const double* sr, const double* alpha, const double* beta,
+                             const double* gamma, const int32_t* cls, const double* d0, const double* m0) override {
+        const std::string who = "mb_set_implicit_solvent: ";
+        if (!p) {
+            if (gb_on_) drop_graphs();
+            gb_on_ = false;
+            return MB_OK;
+        }
+        if (n_ <= 0) return set_error(MB_ERR_STATE, who + "set atoms first");
+        if (decomposed()) return set_error(MB_ERR_INVALID, who + "not available in decomposed (multi-GPU) runs");
+        const int nc = p->n_neck_classes;
+        if (nc < 0 || nc > GB_MAX_CLASSES) return set_error(MB_ERR_INVALID, who + "n_neck_classes outside 0 .. MB_GB_MAX_NECK_CLASSES");
+        if (!or_ || !sr || !alpha || !beta || !gamma || (nc > 0 && (!cls || !d0 || !m0))) return set_error(MB_ERR_INVALID, who + "null array");
+        const double sc[9] = {p->dist_cutoff, p->offset, p->probe_radius, p->sa_factor, p->factor_solute, p->factor_solvent,
+                              p->kappa, p->neck_scale, p->neck_cut};
+        for (double v : sc)
+            if (!std::isfinite(v)) return set_error(MB_ERR_INVALID, who + "non-finite parameter");
+        if (p->dist_cutoff < 0) return set_error(MB_ERR_INVALID, who + "negative dist_cutoff");
+        if (p->offset < 0) return set_error(MB_ERR_INVALID, who + "negative offset");
+        const int64_t n = n_;
+        std::vector<T4> par(n), abg(n);
+        for (int64_t i = 0; i < n; i++) {
+            const double v[5] = {or_[i], sr[i], alpha[i], beta[i], gamma[i]};
+            for (double x : v)
+                if (!std::isfinite(x)) return set_error(MB_ERR_INVALID, who + "non-finite per-atom value");
+            if (!(or_[i] > 0)) return set_error(MB_ERR_INVALID, who + "an offset radius <= 0");
+            const int c = nc > 0 ? cls[i] : 0;
+            if (nc > 0 && (c < 0 || c >= nc)) return set_error(MB_ERR_INVALID, who + "a neck class out of range");
+            const T o = (T)or_[i];
+            par[i] = make4<T>(o, (T)sr[i], o + (T)p->offset, (T)c);  // radius = offset radius + offset, in T as the reference
+            abg[i] = make4<T>((T)alpha[i], (T)beta[i], (T)gamma[i], (T)0);
+        }
+        std::vector<T> tab(2 * (size_t)std::max(nc * nc, 1), (T)0);
+        for (int k = 0; k < nc * nc; k++) {
+            if (!std::isfinite(d0[k]) || !std::isfinite(m0[k])) return set_error(MB_ERR_INVALID, who + "non-finite d0 / m0");
+            tab[k] = (T)d0[k];
+            tab[(size_t)nc * nc + k] = (T)m0[k];
+        }
+        const int nib = (int)((n + GB_THREADS - 1) / GB_THREADS);
+        const int tiles = (int)((n + GB_CHUNK - 1) / GB_CHUNK);
+        // split j so that the grid holds about four CTAs per SM (1170 atoms: 10 atom blocks alone fill 10 SMs)
+        int ns = std::min(tiles, std::max(1, (4 * sm_count_ + nib - 1) / nib));
+        gb_chunk_ = ((tiles + ns - 1) / ns) * GB_CHUNK;
+        gb_nsplit_ = (int)((n + gb_chunk_ - 1) / gb_chunk_);
+        const size_t np = (size_t)n + 16;
+        MB_CUDA(d_gb_par_.ensure(np * sizeof(T4)));
+        MB_CUDA(d_gb_abg_.ensure(np * sizeof(T4)));
+        MB_CUDA(d_gb_tab_.ensure(tab.size() * sizeof(T)));
+        MB_CUDA(d_gb_B_.ensure(np * sizeof(T)));
+        MB_CUDA(d_gb_b_.ensure(np * sizeof(T)));
+        MB_CUDA(d_gb_st_.ensure(np * sizeof(dbl4)));
+        MB_CUDA(d_gb_pd_.ensure((size_t)gb_nsplit_ * n * sizeof(double)));
+        MB_CUDA(d_gb_pf_.ensure((size_t)gb_nsplit_ * n * sizeof(T4)));
+        MB_CUDA(d_gb_pe_.ensure(((size_t)nib * gb_nsplit_ + nib) * sizeof(double)));
+        MB_CUDA(d_gb_tk_.ensure(((size_t)nib + 1) * sizeof(unsigned int)));
+        MB_CUDA(cudaMemcpy(d_gb_par_.p, par.data(), n * sizeof(T4), cudaMemcpyHostToDevice));
+        MB_CUDA(cudaMemcpy(d_gb_abg_.p, abg.data(), n * sizeof(T4), cudaMemcpyHostToDevice));
+        MB_CUDA(cudaMemcpy(d_gb_tab_.p, tab.data(), tab.size() * sizeof(T), cudaMemcpyHostToDevice));
+        MB_CUDA(cudaMemset(d_gb_tk_.p, 0, ((size_t)nib + 1) * sizeof(unsigned int)));
+        GbParams<T>& P = gb_p_;
+        memset(&P, 0, sizeof(P));
+        P.n = (int)n;
+        P.n_cls = nc;
+        P.chunk = gb_chunk_;
+        P.use_ace = p->use_ace ? 1 : 0;
+        P.rc = (T)p->dist_cutoff;
+        P.rc2 = (T)(p->dist_cutoff * p->dist_cutoff);
+        P.offset = (T)p->offset;
+        P.neck_scale = (T)p->neck_scale;
+        P.neck_cut = (T)p->neck_cut;
+        P.kappa = (T)p->kappa;
+        P.f_solute = (T)p->factor_solute;
+        P.f_solvent = (T)p->factor_solvent;
+        P.offset_d = (double)(T)p->offset;
+        P.probe = (double)(T)p->probe_radius;
+        P.sa_factor = (double)(T)p->sa_factor;
+        gb_n_ = n;
+        gb_on_ = true;
+        drop_graphs();  // the graphs bake the GB parameters and buffers in
+        return MB_OK;
+    }
+    // the three GB passes into f4 (slot order), with energy added to d_sp_energy_
+    int launch_gb(bool energy, T4* f4) {
+        if (gb_n_ != n_) return set_error(MB_ERR_STATE, "implicit solvent: the atom count changed since mb_set_implicit_solvent");
+        if (decomposed()) return set_error(MB_ERR_INVALID, "implicit solvent: not available in decomposed (multi-GPU) runs");
+        GbArgs<T> a;
+        a.par = d_gb_par_.as<T4>();
+        a.abg = d_gb_abg_.as<T4>();
+        a.d0 = d_gb_tab_.as<T>();
+        a.m0 = d_gb_tab_.as<T>() + (size_t)gb_p_.n_cls * gb_p_.n_cls;
+        a.orig = d_orig_.as<int>();  // (the identity on the all-pairs path)
+        a.pos4 = d_pos4_.as<T4>();
+        a.f4 = f4;
+        a.B = d_gb_B_.as<T>();
+        a.b = d_gb_b_.as<T>();
+        a.st = d_gb_st_.as<dbl4>();
+        a.pd = d_gb_pd_.as<double>();
+        a.pf = d_gb_pf_.as<T4>();
+        a.pe = d_gb_pe_.as<double>();
+        a.tk = d_gb_tk_.as<unsigned int>();
+        a.acc = energy ? d_sp_energy_.as<double>() : nullptr;
+        const dim3 grid((unsigned)((n_ + GB_THREADS - 1) / GB_THREADS), (unsigned)gb_nsplit_);
+        auto go = [&](auto box) {
+            using B = decltype(box);
+            gb_born_kernel<T, B><<<grid, GB_THREADS, 0, stream_>>>(gb_p_, a, box);
+            with_const<true, false>(energy, [&](auto EN) { gb_pair_kernel<T, EN, B><<<grid, GB_THREADS, 0, stream_>>>(gb_p_, a, box); });
+            gb_chain_kernel<T, B><<<grid, GB_THREADS, 0, stream_>>>(gb_p_, a, box);
+        };
+        if (tric_.on) {
+            go(tric_);
+        } else {
+            BoxT bx;
+            for (int d = 0; d < 3; d++) bx.L[d] = box_[d];
+            go(bx);
+        }
+        launches_ += 3;
+        MB_CUDA(cudaGetLastError());
         return MB_OK;
     }
 
@@ -2288,6 +2413,7 @@ class Engine : public EngineBase {
             if (decomposed())
                 return set_error(MB_ERR_INVALID, "mb_simulate_vv: velocity-rescaling thermostats are not available in decomposed (multi-GPU) runs");
         }
+        if (decomposed() && gb_on_) return set_error(MB_ERR_INVALID, "implicit solvent is not available in decomposed (multi-GPU) runs");
         LogRun lr;
         MB_TRY(log_begin(log, p, lr));
         CallerBuf xb, vb;
@@ -2794,6 +2920,13 @@ class Engine : public EngineBase {
     int pme_plan_ = -1;
     std::vector<int> pme_pairs_;
     DevBuf d_pme_grid_, d_pme_bsm_[3], d_pme_partial_, d_pme_pairs_;
+    // generalized-Born implicit solvent (gbsa.cuh): parameters, per-atom inputs (original order), per-atom results (slot
+    // order), per-split partials, tickets (fixed addresses while set: the step graphs bake them in)
+    bool gb_on_ = false;
+    int64_t gb_n_ = 0;
+    int gb_nsplit_ = 1, gb_chunk_ = GB_CHUNK;
+    GbParams<T> gb_p_ = {};
+    DevBuf d_gb_par_, d_gb_abg_, d_gb_tab_, d_gb_B_, d_gb_b_, d_gb_st_, d_gb_pd_, d_gb_pf_, d_gb_pe_, d_gb_tk_;
     DevBuf d_mass_in_, d_charge_in_, d_ljp_in_;
     DevBuf d_pos4_, d_vel4_, d_f4_, d_xref4_, d_lj2_, d_orig_, d_inv_orig_, d_mass_;
     DevBuf d_pos4_t_, d_vel4_t_, d_lj2_t_, d_orig_t_, d_mass_t_;
@@ -2917,6 +3050,12 @@ int mb_set_pme(mb_ctx* ctx, double r_cut, double error_tol, int order, double ep
     return ctx->e->set_pme(r_cut, error_tol, order, eps_r, n_pairs, pi, pj);
 }
 int mb_set_lj_dispersion_correction(mb_ctx* ctx, double dist_cutoff) { MB_CTX_GUARD(ctx); return ctx->e->set_dispersion(dist_cutoff); }
+int mb_set_implicit_solvent(mb_ctx* ctx, const mb_gbsa_t* p, const double* offset_radii, const double* scaled_offset_radii,
+                            const double* alpha, const double* beta, const double* gamma, const int32_t* neck_class,
+                            const double* d0, const double* m0) {
+    MB_CTX_GUARD(ctx);
+    return ctx->e->set_implicit_solvent(p, offset_radii, scaled_offset_radii, alpha, beta, gamma, neck_class, d0, m0);
+}
 int mb_random_velocities(mb_ctx* ctx, void* vels, double kT, uint64_t rng_ctr1, uint64_t rng_key) {
     MB_CTX_GUARD(ctx);
     return ctx->e->random_velocities(vels, kT, rng_ctr1, rng_key);
