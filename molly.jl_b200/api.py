@@ -1079,6 +1079,16 @@ def steepest_descent(sys: System, sim: SteepestDescentMinimizer, init_step: int 
     return sys, trace
 
 
+# simulator type -> its parameter struct and C entry point (each takes an optional log plan; NULL: no logging)
+_SIMULATE_ENTRY = {
+    VelocityVerlet: (capi.MBVVParams, "mb_simulate_vv_log"),
+    Langevin: (capi.MBLangevinParams, "mb_simulate_langevin"),
+    NoseHoover: (capi.MBNoseHooverParams, "mb_simulate_nose_hoover"),
+    MTSIntegrator: (capi.MBMTSParams, "mb_simulate_mts"),
+    MTSLangevinIntegrator: (capi.MBMTSParams, "mb_simulate_mts"),
+}
+
+
 def simulate(sys: System, sim, n_steps: Optional[int] = None, init_step: int = 0, rng=None, max_retries: int = 2,
              run_loggers=None):
     """simulate!(sys, sim, ...) dispatched on the simulator's type.
@@ -1101,43 +1111,20 @@ def simulate(sys: System, sim, n_steps: Optional[int] = None, init_step: int = 0
             raise NotImplementedError("loggers are not run during a minimisation on the device (run_loggers must be false)")
         steepest_descent(sys, sim, init_step=init_step, max_retries=max_retries)
         return sys
-    mts = isinstance(sim, (MTSIntegrator, MTSLangevinIntegrator))
-    if not (mts or isinstance(sim, (VelocityVerlet, Langevin, NoseHoover))):
+    entry = next((e for t, e in _SIMULATE_ENTRY.items() if isinstance(sim, t)), None)
+    if entry is None:
         raise TypeError(f"unsupported simulator {type(sim).__name__}")
+    params_t, entry = entry
     if n_steps is None:
         raise TypeError(f"simulate(sys, ::{type(sim).__name__}, n_steps) needs n_steps")
     if run_loggers is None:
         run_loggers = True
     _check_run_loggers(run_loggers)
     couplings = sim.coupling if isinstance(sim.coupling, (tuple, list)) else ((sim.coupling,) if sim.coupling else ())
+    mts = params_t is capi.MBMTSParams
+    p = params_t()  # (zero-filled: no Andersen thermostat, no noise)
     vc = None
-    if mts:
-        if couplings:
-            raise TypeError(f"unsupported coupling {couplings[0]!r} with {type(sim).__name__} (the stock Molly path handles it)")
-        levels = mts_levels(sys, sim)
-        p = capi.MBMTSParams()
-        p.n_levels = len(sim.ordered_fractions)
-        p.fractions[:p.n_levels] = sim.ordered_fractions
-        if isinstance(sim, MTSLangevinIntegrator):
-            p.langevin = 1
-            p.kT = sys.k * sim.temperature
-            p.friction = float(sim.friction)
-    elif isinstance(sim, Langevin):
-        if couplings:
-            raise TypeError(f"unsupported coupling {couplings[0]!r} with Langevin (the stock Molly path handles it)")
-        p = capi.MBLangevinParams()
-        p.kT = sys.k * sim.temperature
-        p.friction = float(sim.friction)
-    elif isinstance(sim, NoseHoover):
-        if couplings:
-            raise TypeError(f"unsupported coupling {couplings[0]!r} with NoseHoover (the stock Molly path handles it)")
-        p = capi.MBNoseHooverParams()
-        p.kT = sys.k * sim.temperature
-        p.damping = float(sim.damping)
-    else:
-        p = capi.MBVVParams()
-        p.andersen_kT = 0.0
-        p.andersen_prob = 0.0
+    if isinstance(sim, VelocityVerlet):
         for c in couplings:
             if isinstance(c, _SCALING_THERMOSTATS) and len(couplings) == 1:  # (one thermostat per run)
                 vc = c.descriptor(sys.k)
@@ -1146,6 +1133,19 @@ def simulate(sys: System, sim, n_steps: Optional[int] = None, init_step: int = 0
                 p.andersen_prob = sim.dt / c.coupling_const
             else:
                 raise TypeError(f"unsupported coupling {c!r} (the stock Molly path handles it)")
+    elif couplings:
+        raise TypeError(f"unsupported coupling {couplings[0]!r} with {type(sim).__name__} (the stock Molly path handles it)")
+    if mts:
+        levels = mts_levels(sys, sim)
+        p.n_levels = len(sim.ordered_fractions)
+        p.fractions[:p.n_levels] = sim.ordered_fractions
+        p.langevin = int(isinstance(sim, MTSLangevinIntegrator))
+    if isinstance(sim, (Langevin, NoseHoover, MTSLangevinIntegrator)):
+        p.kT = sys.k * sim.temperature
+    if isinstance(sim, (Langevin, MTSLangevinIntegrator)):
+        p.friction = float(sim.friction)
+    if isinstance(sim, NoseHoover):
+        p.damping = float(sim.damping)
     p.dt = float(sim.dt)
     p.n_steps = int(n_steps)
     p.init_step = int(init_step)
@@ -1163,20 +1163,9 @@ def simulate(sys: System, sim, n_steps: Optional[int] = None, init_step: int = 0
     backup = (sys.coords.copy(), sys.velocities.copy()) if host else None
     plan = _LogPlan(sys, int(n_steps), int(init_step), run_loggers) if sys.loggers and run_loggers is not False else None
     scale = 1.0
-    for attempt in range(max_retries + 1):
-        if isinstance(sim, Langevin):
-            rc = sys._L.mb_simulate_langevin(ctx, _ptr(sys.coords), _ptr(sys.velocities), C.byref(p),
-                                             C.byref(plan.desc) if plan is not None else None)
-        elif isinstance(sim, NoseHoover):
-            rc = sys._L.mb_simulate_nose_hoover(ctx, _ptr(sys.coords), _ptr(sys.velocities), C.byref(p),
-                                                C.byref(plan.desc) if plan is not None else None)
-        elif mts:
-            rc = sys._L.mb_simulate_mts(ctx, _ptr(sys.coords), _ptr(sys.velocities), C.byref(p),
-                                        C.byref(plan.desc) if plan is not None else None)
-        elif plan is None:
-            rc = sys._L.mb_simulate_vv(ctx, _ptr(sys.coords), _ptr(sys.velocities), C.byref(p))
-        else:  # a retry overwrites the records of the failed attempt
-            rc = sys._L.mb_simulate_vv_log(ctx, _ptr(sys.coords), _ptr(sys.velocities), C.byref(p), C.byref(plan.desc))
+    for attempt in range(max_retries + 1):  # (a retry overwrites the records of the failed attempt)
+        rc = getattr(sys._L, entry)(ctx, _ptr(sys.coords), _ptr(sys.velocities), C.byref(p),
+                                    C.byref(plan.desc) if plan is not None else None)
         if rc == capi.MB_ERR_CAPACITY and backup is not None and attempt < max_retries:
             sys.coords[...], sys.velocities[...] = backup
             scale *= 2.0

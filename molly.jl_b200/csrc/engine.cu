@@ -316,6 +316,27 @@ static void pme_plan_host(const double box[3], double r_cut, double error_tol, i
     }
 }
 
+// The integrator of one simulate call: VelocityVerlet (vv.cuh), Langevin (langevin.cuh), Nose-Hoover (nosehoover.cuh) or the
+// multiple-time-step integrators (mts.cuh). Each mb_simulate_* entry point fills one from its own parameters.
+enum { INTEG_VV = 0, INTEG_LANGEVIN = 1, INTEG_NH = 2, INTEG_MTS = 3, INTEG_MTS_LANGEVIN = 4 };
+static bool is_mts(int kind) { return kind == INTEG_MTS || kind == INTEG_MTS_LANGEVIN; }
+struct Integrator {
+    int kind = INTEG_VV;  // INTEG_*
+    double dt = 0;
+    int64_t n_steps = 0, init_step = 0;
+    int remove_cm_every = 0;
+    uint64_t rng_ctr1 = 0, rng_key = 0;
+    double andersen_kT = 0, andersen_prob = 0;  // VelocityVerlet's Andersen thermostat (kT <= 0 or prob <= 0: none)
+    double kT = 0, friction = 0, damping = 0;   // Langevin and MTSLangevinIntegrator: kT, friction; Nose-Hoover: kT, damping
+    int n_levels = 0;                           // the multiple-time-step integrators' ordered fractions (0 levels: none)
+    std::array<int, MTS_MAX_LEVELS> fractions = {};
+    // What the step graphs bake in (GraphKey): every field but n_steps, init_step and the RNG keys, which are uploaded
+    // into Control on every call
+    auto graph_fields() const {
+        return std::tie(kind, dt, remove_cm_every, andersen_kT, andersen_prob, kT, friction, damping, n_levels, fractions);
+    }
+};
+
 class EngineBase {
    public:
     virtual ~EngineBase() {}
@@ -328,10 +349,7 @@ class EngineBase {
                                const int32_t* sj) = 0;
     virtual int set_neighbor_policy(double r_list, int rebuild_every) = 0;
     virtual int forces_energy(const void* coords, void* fs, void* pe, void* vir, int64_t step_n, bool with_specific) = 0;
-    // lg, nh, mts: the Langevin, Nose-Hoover or multiple-time-step integrator's parameters (at most one), all NULL for
-    // VelocityVerlet (p then carries the fields they share)
-    virtual int simulate(void* coords, void* vels, const mb_vv_params_t* p, const mb_langevin_params_t* lg,
-                         const mb_nosehoover_params_t* nh, const mb_mts_params_t* mts, mb_log_t* log) = 0;
+    virtual int simulate(void* coords, void* vels, const Integrator& ig, mb_log_t* log) = 0;
     virtual int remove_cm(void* vels) = 0;
     virtual int kinetic_energy(const void* vels, double* out) = 0;
     virtual int rebuild(const void* coords) = 0;
@@ -1857,21 +1875,41 @@ class Engine : public EngineBase {
     // One MD step enqueued on the stream. In capture mode the neighbour rebuild becomes the body of a CUDA-graph
     // conditional node driven by decide_kernel, otherwise the gated pipeline is enqueued when it may be needed.
     struct StepCfg {
+        Integrator ig;    // the call's integrator
         T dt, dt_half, skin_half2, kT;
-        double prob, inv_mass;
+        double inv_mass;
         int do_cm;        // 0/1 constant, or -1: caller decides per step (stream path only)
         bool thermostat;
         int* flag_ptr;
         VCouple vc;       // velocity-rescaling thermostat (kind VC_NONE: none)
-        int integrator;   // INTEG_*: VelocityVerlet (vv.cuh), Langevin (langevin.cuh), Nose-Hoover (nosehoover.cuh) or the
-                          // multiple-time-step integrators (mts.cuh)
         LangevinCoef lc;  // Langevin's (or MTSLangevinIntegrator's) c, sqrt(1 - c^2) and kT
         NhCoef nc;        // Nose-Hoover's dt / (2 Q^2) and Nf k T0
-        int n_levels;     // multiple-time-step integrators: the ordered fractions
-        std::array<int, MTS_MAX_LEVELS> fractions;
     };
-    enum { INTEG_VV = 0, INTEG_LANGEVIN = 1, INTEG_NH = 2, INTEG_MTS = 3, INTEG_MTS_LANGEVIN = 4 };
-    static bool is_mts(int integrator) { return integrator == INTEG_MTS || integrator == INTEG_MTS_LANGEVIN; }
+    // Langevin's c = exp(-dt friction), sqrt(1 - c^2) and kT (src/simulators.jl:1092-1097), in double. MTSLangevinIntegrator
+    // runs its O step at the innermost substep, with f the innermost fraction: c = exp(-dt friction / f) (:1736-1738);
+    // Langevin passes f = 1, which divides exactly.
+    static LangevinCoef langevin_coef(const Integrator& ig, int f) {
+        const double c = exp(-ig.dt * ig.friction / f);
+        return LangevinCoef{c, sqrt(1.0 - c * c), ig.kT};
+    }
+    StepCfg step_cfg(const Integrator& ig) const {  // (skin_half2 and flag_ptr follow from the path: simulate sets them)
+        StepCfg c;
+        c.ig = ig;
+        c.dt = (T)ig.dt;
+        c.dt_half = (T)ig.dt / (T)2;
+        c.inv_mass = (total_mass_ > 0) ? 1.0 / total_mass_ : 0.0;
+        c.thermostat = ig.andersen_kT > 0 && ig.andersen_prob > 0;
+        c.kT = (T)ig.andersen_kT;
+        c.do_cm = (ig.remove_cm_every == 0) ? 0 : (ig.remove_cm_every == 1 ? 1 : -1);
+        c.vc = VCouple{vcoupling.kind, vcoupling.n_steps, 3 * (long long)n_ - 3, vcoupling.kT, ig.dt, vcoupling.tau, total_mass_};
+        c.lc = LangevinCoef{1.0, 0.0, 0.0};
+        if (ig.kind == INTEG_LANGEVIN) c.lc = langevin_coef(ig, 1);
+        if (ig.kind == INTEG_MTS_LANGEVIN) c.lc = langevin_coef(ig, ig.fractions[ig.n_levels - 1]);
+        c.nc = NhCoef{0.0, 1.0};
+        if (ig.kind == INTEG_NH)  // NoseHoover(dt, temperature, damping): dt / (2 damping^2) and Nf k T0 (src/simulators.jl:1575-1579), in double
+            c.nc = NhCoef{ig.dt / (2.0 * ig.damping * ig.damping), (double)(3 * (long long)n_ - 3) * ig.kT};
+        return c;
+    }
     // what one step does beyond the plain VelocityVerlet step
     struct StepOpts {
         int do_cm = 0;                   // remove_CM_motion after this step's kick
@@ -1900,6 +1938,19 @@ class Engine : public EngineBase {
         MB_CUDA(cudaStreamUpdateCaptureDependencies(stream_, &cnode, 1, cudaStreamSetCaptureDependencies));
         return MB_OK;
     }
+    // What follows a drift (single GPU): the all-pairs path wraps; the cell-list path splices the conditional rebuild node
+    // (capture) or enqueues the gated rebuild when it may be needed (no fixed interval, or `due`: the interval's rebuild)
+    int after_drift(Capture* cap, bool due) {
+        if (path_ == 0) {
+            wrap_kernel<T><<<(int)((n_ + 255) / 256), 256, 0, stream_>>>((int)n_, geom(), d_pos4_.as<T4>());
+            launches_++;
+        } else if (cap) {
+            MB_TRY(splice_rebuild(*cap));
+        } else if (rebuild_every_ == 0 || due) {
+            MB_TRY(enqueue_rebuild(true, false));
+        }
+        return MB_OK;
+    }
     // The grid of an integration pass (K1, K2, the Langevin step, NH1, NH2) over n atoms: CTAs of VV_THREADS threads with
     // per_thread atoms each, at most per_sm CTAs per SM. The grid decides how grid_sum groups the sums, so a pass keeps its
     // grid from one release to the next. Each CTA writes `width` doubles to d_partial_, which is checked to hold them.
@@ -1912,10 +1963,9 @@ class Engine : public EngineBase {
         return MB_OK;
     }
     int enqueue_step(const StepCfg& c, const StepOpts& o, Capture* cap = nullptr) {
-        if (is_mts(c.integrator)) return enqueue_mts_step(c, o, cap);
+        if (is_mts(c.ig.kind)) return enqueue_mts_step(c, o, cap);
         const bool dec = decomposed() && path_ == 1;
         const int s0 = dec ? own_s0_ : 0, n_own = dec ? own_n_ : (int)n_;
-        const int nb = std::max(1, (n_own + 255) / 256);
         Control* ctl = d_ctl_.as<Control>();
         CmState<T>* cm = d_cm_.as<CmState<T>>();
         // decomposed run over peer memory (peer.cuh): K1 mirrors the boundary slots into the neighbours while it drifts
@@ -1933,13 +1983,13 @@ class Engine : public EngineBase {
         }
         prof_.begin(Prof::VV);
         int grid;
-        if (c.integrator == INTEG_LANGEVIN) {  // (single GPU: s0 = 0)
+        if (c.ig.kind == INTEG_LANGEVIN) {  // (single GPU: s0 = 0)
             MB_TRY(integ_grid(grid, n_own, 1, 8, 3));
             langevin_step_kernel<T><<<grid, VV_THREADS, 0, stream_>>>(
                 n_own, c.dt, c.dt_half, c.skin_half2, c.lc, o.do_cm, c.inv_mass, cm, d_f4_.as<T4>(), d_xref4_.as<T4>(),
                 d_pos4_.as<T4>(), d_vel4_.as<T4>(), d_orig_.as<int>(), d_mass_.as<T>(), d_partial_.as<double>(), c.flag_ptr, ctl,
                 cap ? cap->rebuild : 0, cap && path_ == 1 ? 1 : 0, ext_map());
-        } else if (c.integrator == INTEG_NH) {  // (single GPU: s0 = 0)
+        } else if (c.ig.kind == INTEG_NH) {  // (single GPU: s0 = 0)
             MB_TRY(integ_grid(grid, n_own, 1, 8, 2));
             nh_kick_drift_kernel<T><<<grid, VV_THREADS, 0, stream_>>>(
                 n_own, c.dt, c.dt_half, c.skin_half2, c.nc, d_nh_.as<NhState>(), cm, d_f4_.as<T4>(), d_xref4_.as<T4>(),
@@ -1961,12 +2011,7 @@ class Engine : public EngineBase {
             clear_cm_kernel<T><<<1, 1, 0, stream_>>>(cm);
             launches_++;
         }
-        if (path_ == 0) {
-            wrap_kernel<T><<<nb, 256, 0, stream_>>>((int)n_, geom(), d_pos4_.as<T4>());
-            launches_++;
-        } else if (cap) {
-            MB_TRY(splice_rebuild(*cap));
-        } else if (dec) {
+        if (dec) {  // (the decomposed step is never captured)
             if (o.rebuild_hint) {
                 // neighbour rebuild on a decomposed box: replicate positions and velocities, rebuild (identical sort on every
                 // rank, lists only for the owned slab), then refresh the slot ranges and halo segments
@@ -1980,18 +2025,18 @@ class Engine : public EngineBase {
                 MB_TRY(halo_exchange());
             }
         } else {
-            if (rebuild_every_ == 0 || o.rebuild_hint) MB_TRY(enqueue_rebuild(true, false));
+            MB_TRY(after_drift(cap, o.rebuild_hint));
         }
         const int s0b = dec ? own_s0_ : 0, n_ownb = dec ? own_n_ : (int)n_;  // ownership may have changed in the rebuild
         const int nb2 = std::max(1, (n_ownb + 255) / 256);
         MB_TRY(launch_pairs(false, d_f4_.as<T4>(), dec));
         MB_TRY(launch_bonded(false));
-        if (c.integrator == INTEG_LANGEVIN) {  // these forces are the next step's kick: the step ends here
+        if (c.ig.kind == INTEG_LANGEVIN) {  // these forces are the next step's kick: the step ends here
             if (o.log_mask) MB_TRY(enqueue_log(c, o.log_mask));
             MB_CUDA(cudaGetLastError());
             return MB_OK;
         }
-        if (c.integrator == INTEG_NH) {
+        if (c.ig.kind == INTEG_NH) {
             MB_TRY(integ_grid(grid, n_ownb, 1, 8, 3));
             prof_.begin(Prof::VV);
             nh_kick2_kernel<T><<<grid, VV_THREADS, 0, stream_>>>(n_ownb, c.dt_half, o.do_cm, c.inv_mass, d_nh_.as<NhState>(),
@@ -2029,7 +2074,7 @@ class Engine : public EngineBase {
             launches_++;
         }
         if (c.thermostat && !thermo_in_k1(c).on) {
-            andersen_kernel<T><<<nb2, 256, 0, stream_>>>(s0b, n_ownb, (int)n_, c.kT, c.prob, d_orig_.as<int>(), d_mass_.as<T>(), d_vel4_.as<T4>(), cm, ctl);
+            andersen_kernel<T><<<nb2, 256, 0, stream_>>>(s0b, n_ownb, (int)n_, c.kT, c.ig.andersen_prob, d_orig_.as<int>(), d_mass_.as<T>(), d_vel4_.as<T4>(), cm, ctl);
             launches_++;
         }
         if (o.log_mask) MB_TRY(enqueue_log(c, o.log_mask));
@@ -2055,8 +2100,8 @@ class Engine : public EngineBase {
         return launch_bonded(false, d_f4_mts_.as<T4>(), level);
     }
     int enqueue_mts_level(const StepCfg& c, const StepOpts& o, Capture* cap, int l, bool recompute, MtsWalk& w) {
-        const int n = (int)n_, n_inner = c.fractions[c.n_levels - 1];
-        const double dt_x = (double)c.dt / c.fractions[l];
+        const int n = (int)n_, n_inner = c.ig.fractions[c.ig.n_levels - 1];
+        const double dt_x = (double)c.dt / c.ig.fractions[l];
         const T dt_v = (T)(dt_x / 2);
         T4* f = (l == 0) ? d_f4_.as<T4>() : d_f4_mts_.as<T4>();
         Control* ctl = d_ctl_.as<Control>();
@@ -2072,14 +2117,14 @@ class Engine : public EngineBase {
                 launches_++;
             }
         };
-        const int reps = c.fractions[l] / (l == 0 ? 1 : c.fractions[l - 1]);
+        const int reps = c.ig.fractions[l] / (l == 0 ? 1 : c.ig.fractions[l - 1]);
         for (int r = 0; r < reps; r++) {
             if (recompute) MB_TRY(mts_forces(l));
             const int apply_cm = w.cm_taken ? 0 : 1;
-            if (l == c.n_levels - 1) {
+            if (l == c.ig.n_levels - 1) {
                 const int last = (w.substep == n_inner - 1) ? 1 : 0;
                 prof_.begin(Prof::VV);
-                with_const<true, false>(c.integrator == INTEG_MTS_LANGEVIN, [&](auto LG) {
+                with_const<true, false>(c.ig.kind == INTEG_MTS_LANGEVIN, [&](auto LG) {
                     mts_kick_drift_kernel<T, LG><<<grid, VV_THREADS, 0, stream_>>>(
                         n, dt_v, (T)dt_x, (T)(dt_x / 2), c.skin_half2, c.lc, w.substep, apply_cm, last, cm, f, d_xref4_.as<T4>(),
                         d_pos4_.as<T4>(), d_vel4_.as<T4>(), d_orig_.as<int>(), c.flag_ptr, ctl, cap ? cap->rebuild : 0,
@@ -2089,16 +2134,7 @@ class Engine : public EngineBase {
                 launches_++;
                 first_kick_done();
                 w.substep++;
-                if (last) {
-                    if (path_ == 0) {
-                        wrap_kernel<T><<<(n + 255) / 256, 256, 0, stream_>>>(n, geom(), d_pos4_.as<T4>());
-                        launches_++;
-                    } else if (cap) {
-                        MB_TRY(splice_rebuild(*cap));
-                    } else if (rebuild_every_ == 0 || o.rebuild_hint) {
-                        MB_TRY(enqueue_rebuild(true, false));
-                    }
-                }
+                if (last) MB_TRY(after_drift(cap, o.rebuild_hint));
             } else {
                 prof_.begin(Prof::VV);
                 mts_kick_kernel<T><<<grid, VV_THREADS, 0, stream_>>>(n, dt_v, apply_cm, cm, f, d_vel4_.as<T4>());
@@ -2160,27 +2196,21 @@ class Engine : public EngineBase {
             th.on = 1;
             th.n = (int)n_;
             th.kT = c.kT;
-            th.prob = c.prob;
+            th.prob = c.ig.andersen_prob;
             th.orig = d_orig_.as<int>();
             th.mass = d_mass_.as<T>();
         }
         return th;
     }
 
-    // What a simulate call chooses that its step graphs bake in: the step options, the thermostat and integrator
-    // parameters (kernel arguments) and the log mask, the LOG_* records the graph ends with (0: a plain step). The logging
-    // kernel's destinations are read from the device descriptor (d_log_desc_), so they are not part of it.
+    // What a simulate call chooses that its step graphs bake in: the integrator's fields (Integrator::graph_fields), the
+    // velocity-rescaling thermostat (K2's arguments) and the log mask, the LOG_* records the graph ends with (0: a plain
+    // step). The logging kernel's destinations are read from the device descriptor (d_log_desc_), so they are not part of it.
     struct GraphKey {
-        int do_cm, log_mask, integrator;  // INTEG_*
-        double dt, andersen_kT, andersen_prob;
-        double integ_kT, friction, damping;  // Langevin's (MTSLangevinIntegrator's) kT and friction, or Nose-Hoover's kT and damping
-        mb_vcoupling_t vc;                   // the velocity-rescaling thermostat (K2's arguments)
-        int n_levels;                        // the multiple-time-step integrators' ordered fractions (0 levels: none)
-        std::array<int, MTS_MAX_LEVELS> fractions;
-        auto fields() const {
-            return std::tie(do_cm, log_mask, integrator, dt, andersen_kT, andersen_prob, integ_kT, friction, damping, vc.kind,
-                            vc.n_steps, vc.kT, vc.tau, n_levels, fractions);
-        }
+        Integrator ig;
+        mb_vcoupling_t vc;
+        int log_mask;
+        auto fields() const { return std::tuple_cat(ig.graph_fields(), std::tie(vc.kind, vc.n_steps, vc.kT, vc.tau, log_mask)); }
         bool operator==(const GraphKey& o) const { return fields() == o.fields(); }
     };
     // A captured graph: a step graph (one per log mask; the host loop picks one per step) or the minimiser's loop.
@@ -2294,7 +2324,7 @@ class Engine : public EngineBase {
         size_t frame_bytes = 0;
     };
     // validate the request, plan the destinations and upload the logging kernel's descriptor (read by log_kernel only)
-    int log_begin(mb_log_t* log, const mb_vv_params_t* p, LogRun& lr) {
+    int log_begin(mb_log_t* log, const Integrator& ig, LogRun& lr) {
         lr.log = log;
         if (!log) return MB_OK;
         if (decomposed()) return set_error(MB_ERR_INVALID, "mb_simulate_vv_log: logging is not available in decomposed (multi-GPU) runs");
@@ -2304,7 +2334,7 @@ class Engine : public EngineBase {
         for (int k = 0; k < 3; k++) {
             if (every[k] < 0 || cap[k] < 0) return set_error(MB_ERR_INVALID, "mb_simulate_vv_log: negative interval or capacity");
             if (every[k] > 0 && !outs[k]) return set_error(MB_ERR_INVALID, "mb_simulate_vv_log: null output for a non-zero interval");
-            lr.n[k] = log_count(every[k], p->init_step, p->n_steps, log->log_initial != 0);
+            lr.n[k] = log_count(every[k], ig.init_step, ig.n_steps, log->log_initial != 0);
             if (lr.n[k] > cap[k])
                 return set_error(MB_ERR_INVALID, "mb_simulate_vv_log: capacity too small: this call writes " + std::to_string(lr.n[k]) +
                                                      (k == 0 ? " energy records" : k == 1 ? " coordinate frames" : " velocity frames"));
@@ -2361,61 +2391,68 @@ class Engine : public EngineBase {
         return MB_OK;
     }
 
-    // mb_simulate_vv, mb_simulate_vv_log, mb_simulate_langevin, mb_simulate_nose_hoover and mb_simulate_mts: one body, one
-    // step loop, one graph builder
-    int simulate(void* coords, void* vels, const mb_vv_params_t* p, const mb_langevin_params_t* lg, const mb_nosehoover_params_t* nh,
-                 const mb_mts_params_t* mts, mb_log_t* log) override {
-        MB_TRY(prepare());
-        if (!coords || !vels || !p) return set_error(MB_ERR_INVALID, "null argument");
-        if (p->n_steps < 0 || !(p->dt > 0)) return set_error(MB_ERR_INVALID, "n_steps < 0 or dt <= 0");
-        if (lg) {
-            if (!(std::isfinite(lg->kT) && lg->kT >= 0)) return set_error(MB_ERR_INVALID, "mb_simulate_langevin: kT must be finite and >= 0");
-            if (!(std::isfinite(lg->friction) && lg->friction >= 0))
-                return set_error(MB_ERR_INVALID, "mb_simulate_langevin: friction must be finite and >= 0");
+    // The refusals of a simulate call, made before any work; each names the call's C entry point
+    int check_simulate(const void* coords, const void* vels, const Integrator& ig) {
+        static const char* const entry[] = {"mb_simulate_vv", "mb_simulate_langevin", "mb_simulate_nose_hoover", "mb_simulate_mts",
+                                            "mb_simulate_mts"};
+        static const char* const name[] = {"VelocityVerlet", "Langevin", "Nose-Hoover", "the multiple-time-step integrators",
+                                           "the multiple-time-step integrators"};
+        if (!coords || !vels) return set_error(MB_ERR_INVALID, "null argument");
+        if (ig.n_steps < 0 || !(ig.dt > 0)) return set_error(MB_ERR_INVALID, "n_steps < 0 or dt <= 0");
+        const std::string who = std::string(entry[ig.kind]) + ": ";
+        if (is_mts(ig.kind)) {
+            if (ig.n_levels < 1 || ig.n_levels > MB_MTS_MAX_LEVELS)
+                return set_error(MB_ERR_INVALID, who + "n_levels must be in 1 .. MB_MTS_MAX_LEVELS");
+            if (ig.fractions[0] != 1) return set_error(MB_ERR_INVALID, who + "the first ordered fraction must be 1");
+            for (int l = 1; l < ig.n_levels; l++)
+                if (!(ig.fractions[l] > ig.fractions[l - 1] && ig.fractions[l] % ig.fractions[l - 1] == 0))
+                    return set_error(MB_ERR_INVALID, who + "fraction " + std::to_string(ig.fractions[l]) +
+                                                         " is not a larger multiple of fraction " + std::to_string(ig.fractions[l - 1]));
+            if (ig.fractions[ig.n_levels - 1] > 1024)
+                return set_error(MB_ERR_INVALID, who + "more than 1024 innermost substeps per outer step");
+            if (max_specific_level() >= ig.n_levels)
+                return set_error(MB_ERR_INVALID, who + "a specific interaction sits at level " + std::to_string(max_specific_level()) +
+                                                     " of " + std::to_string(ig.n_levels) + " (mb_set_specific_levels)");
         }
-        if (nh) {
+        if (ig.kind == INTEG_LANGEVIN || ig.kind == INTEG_MTS_LANGEVIN) {
+            if (!(std::isfinite(ig.kT) && ig.kT >= 0)) return set_error(MB_ERR_INVALID, who + "kT must be finite and >= 0");
+            if (!(std::isfinite(ig.friction) && ig.friction >= 0)) return set_error(MB_ERR_INVALID, who + "friction must be finite and >= 0");
+        }
+        if (ig.kind == INTEG_NH) {
             // (kT = 0 would make T / T0 infinite)
-            if (!(std::isfinite(nh->kT) && nh->kT > 0)) return set_error(MB_ERR_INVALID, "mb_simulate_nose_hoover: kT must be finite and > 0");
-            if (!(std::isfinite(nh->damping) && nh->damping > 0))
-                return set_error(MB_ERR_INVALID, "mb_simulate_nose_hoover: damping must be finite and > 0");
-            if (n_ < 2) return set_error(MB_ERR_INVALID, "mb_simulate_nose_hoover: needs at least 2 atoms (Nf = 3N - 3 > 0)");
+            if (!(std::isfinite(ig.kT) && ig.kT > 0)) return set_error(MB_ERR_INVALID, who + "kT must be finite and > 0");
+            if (!(std::isfinite(ig.damping) && ig.damping > 0)) return set_error(MB_ERR_INVALID, who + "damping must be finite and > 0");
+            if (n_ < 2) return set_error(MB_ERR_INVALID, who + "needs at least 2 atoms (Nf = 3N - 3 > 0)");
         }
-        if (mts) {
-            if (mts->n_levels < 1 || mts->n_levels > MB_MTS_MAX_LEVELS)
-                return set_error(MB_ERR_INVALID, "mb_simulate_mts: n_levels must be in 1 .. MB_MTS_MAX_LEVELS");
-            if (mts->fractions[0] != 1) return set_error(MB_ERR_INVALID, "mb_simulate_mts: the first ordered fraction must be 1");
-            for (int l = 1; l < mts->n_levels; l++)
-                if (!(mts->fractions[l] > mts->fractions[l - 1] && mts->fractions[l] % mts->fractions[l - 1] == 0))
-                    return set_error(MB_ERR_INVALID, "mb_simulate_mts: fraction " + std::to_string(mts->fractions[l]) +
-                                                         " is not a larger multiple of fraction " + std::to_string(mts->fractions[l - 1]));
-            if (mts->fractions[mts->n_levels - 1] > 1024)
-                return set_error(MB_ERR_INVALID, "mb_simulate_mts: more than 1024 innermost substeps per outer step");
-            if (max_specific_level() >= mts->n_levels)
-                return set_error(MB_ERR_INVALID, "mb_simulate_mts: a specific interaction sits at level " + std::to_string(max_specific_level()) +
-                                                     " of " + std::to_string(mts->n_levels) + " (mb_set_specific_levels)");
-            if (mts->langevin) {
-                if (!(std::isfinite(mts->kT) && mts->kT >= 0)) return set_error(MB_ERR_INVALID, "mb_simulate_mts: kT must be finite and >= 0");
-                if (!(std::isfinite(mts->friction) && mts->friction >= 0))
-                    return set_error(MB_ERR_INVALID, "mb_simulate_mts: friction must be finite and >= 0");
-            }
-        }
-        if (lg || nh || mts) {
-            const std::string who = lg ? "mb_simulate_langevin" : (nh ? "mb_simulate_nose_hoover" : "mb_simulate_mts");
+        if (ig.kind != INTEG_VV) {
             if (vcoupling.kind != MB_VC_NONE)
-                return set_error(MB_ERR_INVALID, who + ": a velocity coupling is set on the context (couplings with " +
-                                                     (lg ? "Langevin" : (nh ? "Nose-Hoover" : "the multiple-time-step integrators")) +
+                return set_error(MB_ERR_INVALID, who + "a velocity coupling is set on the context (couplings with " + name[ig.kind] +
                                                      " are not supported)");
-            if (decomposed()) return set_error(MB_ERR_INVALID, who + ": not available in decomposed (multi-GPU) runs");
-        }
-        if (vcoupling.kind != MB_VC_NONE) {
-            if (p->andersen_kT > 0 && p->andersen_prob > 0)
-                return set_error(MB_ERR_INVALID, "mb_simulate_vv: at most one thermostat per call (Andersen and a velocity-rescaling thermostat)");
+            if (decomposed()) return set_error(MB_ERR_INVALID, who + "not available in decomposed (multi-GPU) runs");
+        } else if (vcoupling.kind != MB_VC_NONE) {
+            if (ig.andersen_kT > 0 && ig.andersen_prob > 0)
+                return set_error(MB_ERR_INVALID, who + "at most one thermostat per call (Andersen and a velocity-rescaling thermostat)");
             if (decomposed())
-                return set_error(MB_ERR_INVALID, "mb_simulate_vv: velocity-rescaling thermostats are not available in decomposed (multi-GPU) runs");
+                return set_error(MB_ERR_INVALID, who + "velocity-rescaling thermostats are not available in decomposed (multi-GPU) runs");
         }
         if (decomposed() && gb_on_) return set_error(MB_ERR_INVALID, "implicit solvent is not available in decomposed (multi-GPU) runs");
+        return MB_OK;
+    }
+
+    // mb_simulate_vv, mb_simulate_vv_log, mb_simulate_langevin, mb_simulate_nose_hoover and mb_simulate_mts: one body, one
+    // step loop, one graph builder
+    int simulate(void* coords, void* vels, const Integrator& call, mb_log_t* log) override {
+        MB_TRY(prepare());
+        MB_TRY(check_simulate(coords, vels, call));
+        // one level without noise is the VelocityVerlet step: it runs as one (after the refusals, which name mb_simulate_mts)
+        Integrator ig = call;
+        if (ig.kind == INTEG_MTS && ig.n_levels == 1) {
+            ig.kind = INTEG_VV;
+            ig.n_levels = 0;
+            ig.fractions.fill(0);
+        }
         LogRun lr;
-        MB_TRY(log_begin(log, p, lr));
+        MB_TRY(log_begin(log, ig, lr));
         CallerBuf xb, vb;
         MB_TRY(caller_xyz(coords, d_stage_a_, true, xb));
         MB_TRY(caller_xyz(vels, d_stage_c_, true, vb));
@@ -2424,42 +2461,9 @@ class Engine : public EngineBase {
         CmState<T>* cm = d_cm_.as<CmState<T>>();
         clear_cm_kernel<T><<<1, 1, 0, stream_>>>(cm);
         launches_++;
-        if (nh) MB_CUDA(cudaMemsetAsync(d_nh_.p, 0, sizeof(NhState), stream_));  // zeta = 0 at the start of every call
-        StepCfg c;
-        c.dt = (T)p->dt;
-        c.dt_half = (T)p->dt / (T)2;
-        c.inv_mass = (total_mass_ > 0) ? 1.0 / total_mass_ : 0.0;
-        c.thermostat = p->andersen_kT > 0 && p->andersen_prob > 0;
-        c.kT = (T)p->andersen_kT;
-        c.prob = p->andersen_prob;
-        c.do_cm = (p->remove_cm_every == 0) ? 0 : (p->remove_cm_every == 1 ? 1 : -1);
-        c.vc = VCouple{vcoupling.kind, vcoupling.n_steps, 3 * (long long)n_ - 3, vcoupling.kT, p->dt, vcoupling.tau, total_mass_};
-        c.integrator = lg ? INTEG_LANGEVIN : (nh ? INTEG_NH : INTEG_VV);
-        c.lc = LangevinCoef{1.0, 0.0, 0.0};
-        c.nc = NhCoef{0.0, 1.0};
-        c.n_levels = 0;
-        c.fractions.fill(0);
-        // one level without noise is the VelocityVerlet step: it runs as one
-        if (mts && (mts->langevin || mts->n_levels > 1)) {
-            c.integrator = mts->langevin ? INTEG_MTS_LANGEVIN : INTEG_MTS;
-            c.n_levels = mts->n_levels;
-            std::copy_n(mts->fractions, mts->n_levels, c.fractions.begin());
-            if (mts->langevin) {  // MTSLangevinIntegrator: vel_scale, noise_scale (src/simulators.jl:1736-1738), in double
-                c.lc.vel_scale = exp(-p->dt * mts->friction / mts->fractions[mts->n_levels - 1]);
-                c.lc.noise_scale = sqrt(1.0 - c.lc.vel_scale * c.lc.vel_scale);
-                c.lc.kT = mts->kT;
-            }
-            if (c.n_levels > 1) MB_CUDA(d_f4_mts_.ensure(((size_t)n_ + 16) * sizeof(T4)));
-        }
-        if (nh) {  // NoseHoover(dt, temperature, damping): dt / (2 damping^2) and Nf k T0 (src/simulators.jl:1575-1579), in double
-            c.nc.coef = p->dt / (2.0 * nh->damping * nh->damping);
-            c.nc.nf_kT = (double)(3 * (long long)n_ - 3) * nh->kT;
-        }
-        if (lg) {  // Langevin(dt, temperature, friction): vel_scale, noise_scale (src/simulators.jl:1092-1097), in double
-            c.lc.vel_scale = exp(-p->dt * lg->friction);
-            c.lc.noise_scale = sqrt(1.0 - c.lc.vel_scale * c.lc.vel_scale);
-            c.lc.kT = lg->kT;
-        }
+        if (ig.kind == INTEG_NH) MB_CUDA(cudaMemsetAsync(d_nh_.p, 0, sizeof(NhState), stream_));  // zeta = 0 at the start of every call
+        StepCfg c = step_cfg(ig);
+        if (c.ig.n_levels > 1) MB_CUDA(d_f4_mts_.ensure(((size_t)n_ + 16) * sizeof(T4)));
         if (path_ == 0) {
             init_slots(xb.as<T>());
             // velocities + wrap through ingest with an identity order (geometry only needs L)
@@ -2479,10 +2483,10 @@ class Engine : public EngineBase {
             struct Tail { int rebuild_every; long long step, init_step; unsigned int rng[4]; unsigned int max_disp2_bits, call_max_disp2_bits; } t;
             static_assert(sizeof(Tail) == sizeof(Control) - offsetof(Control, rebuild_every), "Control tail layout");
             t.rebuild_every = (decomposed() && path_ == 1) ? 0 : rebuild_every_;  // decomposed: the host counts the interval
-            t.step = p->init_step;
-            t.init_step = p->init_step;
-            t.rng[0] = (unsigned int)p->rng_ctr1; t.rng[1] = (unsigned int)(p->rng_ctr1 >> 32);
-            t.rng[2] = (unsigned int)p->rng_key; t.rng[3] = (unsigned int)(p->rng_key >> 32);
+            t.step = ig.init_step;
+            t.init_step = ig.init_step;
+            t.rng[0] = (unsigned int)ig.rng_ctr1; t.rng[1] = (unsigned int)(ig.rng_ctr1 >> 32);
+            t.rng[2] = (unsigned int)ig.rng_key; t.rng[3] = (unsigned int)(ig.rng_key >> 32);
             t.max_disp2_bits = 0;
             t.call_max_disp2_bits = 0;
             MB_CUDA(cudaMemcpyAsync(reinterpret_cast<char*>(ctl) + offsetof(Control, rebuild_every), &t, sizeof(t),
@@ -2492,7 +2496,7 @@ class Engine : public EngineBase {
         cm_deferred_epoch_ = 0;
         adapt_span_ = since_rebuild_;
         bool cm_pending = false;  // host mirror of cm->valid
-        if (p->init_step == 0 && p->remove_cm_every != 0) {
+        if (ig.init_step == 0 && ig.remove_cm_every != 0) {
             // remove_CM_motion! before the first force evaluation (simulators.jl:563): zero-length kick
             int grid;
             MB_TRY(integ_grid(grid, (int)n_, 1, 8, 3));
@@ -2511,7 +2515,7 @@ class Engine : public EngineBase {
             MB_TRY(p2p_setup());  // collective; falls back to the NCCL transport on every rank if any mapping fails
         }
         MB_TRY(launch_pairs(false, d_f4_.as<T4>(), dec));
-        MB_TRY(launch_bonded(false, nullptr, is_mts(c.integrator) ? 0 : -1));  // (multiple time steps: F_0 of level 0)
+        MB_TRY(launch_bonded(false, nullptr, is_mts(c.ig.kind) ? 0 : -1));  // (multiple time steps: F_0 of level 0)
         if (dec) {
             const unsigned long long e0 = ++epoch_;  // this force evaluation read the replicated state: tell the pushers
             if (p2p_active()) {
@@ -2520,7 +2524,7 @@ class Engine : public EngineBase {
             }
         }
         if (log && log->log_initial) {  // apply_loggers! at init_step (run_loggers == true), after F0
-            const int m = log_mask_at(log, p->init_step);
+            const int m = log_mask_at(log, ig.init_step);
             if (m) {
                 MB_TRY(enqueue_log(c, m));
                 MB_TRY(log_step(lr, m));
@@ -2528,16 +2532,13 @@ class Engine : public EngineBase {
         }
 
         // CUDA-graph path: static per-step sequence (remove_CM_motion in {0,1})
-        bool use_graph = graphs_usable() && c.do_cm >= 0 && p->n_steps >= 4 &&
+        bool use_graph = graphs_usable() && c.do_cm >= 0 && ig.n_steps >= 4 &&
                          !dec;  // the decomposed step issues NCCL calls with per-rebuild sizes
         if (use_graph) {
             // one executable per log mask this call uses (the plain step and the log steps)
             bool need[8] = {false, false, false, false, false, false, false, false};
-            for (int64_t k = 1; k <= p->n_steps; k++) need[log_mask_at(log, p->init_step + k)] = true;
-            GraphKey key{c.do_cm, 0, c.integrator, p->dt, p->andersen_kT, p->andersen_prob,
-                         lg ? lg->kT : (nh ? nh->kT : (c.integrator == INTEG_MTS_LANGEVIN ? mts->kT : 0.0)),
-                         lg ? lg->friction : (c.integrator == INTEG_MTS_LANGEVIN ? mts->friction : 0.0), nh ? nh->damping : 0.0,
-                         vcoupling, c.n_levels, c.fractions};
+            for (int64_t k = 1; k <= ig.n_steps; k++) need[log_mask_at(log, ig.init_step + k)] = true;
+            GraphKey key{ig, vcoupling, 0};
             for (int m = 0; m < 8 && use_graph; m++) {
                 if (!need[m]) continue;
                 key.log_mask = m;
@@ -2551,18 +2552,18 @@ class Engine : public EngineBase {
         }
         graph_used_ = use_graph;
         if (use_graph) {
-            for (int64_t k = 1; k <= p->n_steps; k++) {
-                const int m = log_mask_at(log, p->init_step + k);
+            for (int64_t k = 1; k <= ig.n_steps; k++) {
+                const int m = log_mask_at(log, ig.init_step + k);
                 MB_CUDA(cudaGraphLaunch(graphs_[m].exec, stream_));
                 launches_ += graphs_[m].launches;  // rebuild-body kernels are not counted
                 n_force_evals_ += (m & LOG_ENERGY) ? 2 : 1;
                 MB_TRY(log_step(lr, m));
             }
-            n_steps_ += p->n_steps;
+            n_steps_ += ig.n_steps;
         } else {
-            for (int64_t k = 1; k <= p->n_steps; k++) {
-                const int64_t step_n = p->init_step + k;
-                const int do_cm = (p->remove_cm_every != 0 && step_n % p->remove_cm_every == 0) ? 1 : 0;
+            for (int64_t k = 1; k <= ig.n_steps; k++) {
+                const int64_t step_n = ig.init_step + k;
+                const int do_cm = (ig.remove_cm_every != 0 && step_n % ig.remove_cm_every == 0) ? 1 : 0;
                 const bool clear_after_k1 = cm_pending && !do_cm;  // K1 consumed v_cm; nothing overwrites it this step
                 // decomposed: fixed interval counted on the host (identical on every rank), adapted per call from the displacements
                 bool hint;
@@ -2575,9 +2576,9 @@ class Engine : public EngineBase {
                 }
                 StepOpts o;
                 o.do_cm = do_cm;
-                o.clear_cm_after_k1 = clear_after_k1 && (c.integrator == INTEG_VV || is_mts(c.integrator));
+                o.clear_cm_after_k1 = clear_after_k1 && (c.ig.kind == INTEG_VV || is_mts(c.ig.kind));
                 o.rebuild_hint = hint;
-                o.defer_cm = k < p->n_steps;
+                o.defer_cm = k < ig.n_steps;
                 o.log_mask = log_mask_at(log, step_n);
                 MB_TRY(enqueue_step(c, o));
                 MB_TRY(log_step(lr, o.log_mask));
@@ -2585,9 +2586,9 @@ class Engine : public EngineBase {
                 n_steps_++;
             }
         }
-        if (c.thermostat && !dec && p->n_steps > 0) {
+        if (c.thermostat && !dec && ig.n_steps > 0) {
             // the thermostat of the last step (the earlier ones ran inside the next step's drift kernel)
-            andersen_kernel<T><<<nb, 256, 0, stream_>>>(0, (int)n_, (int)n_, c.kT, c.prob, d_orig_.as<int>(), d_mass_.as<T>(), d_vel4_.as<T4>(), cm, ctl);
+            andersen_kernel<T><<<nb, 256, 0, stream_>>>(0, (int)n_, (int)n_, c.kT, c.ig.andersen_prob, d_orig_.as<int>(), d_mass_.as<T>(), d_vel4_.as<T4>(), cm, ctl);
             launches_++;
         }
         if (dec) {
@@ -2636,14 +2637,7 @@ class Engine : public EngineBase {
                                                            path_ == 1 ? g_.skin_half2 : (T)0, ext_map(), d_ctl_.as<Control>(),
                                                            d_sd_st_.as<SdState>(), cap ? cap->rebuild : 0, cap && path_ == 1 ? 1 : 0);
         launches_++;
-        if (path_ == 0) {
-            wrap_kernel<T><<<(int)((n_ + 255) / 256), 256, 0, stream_>>>((int)n_, g_ap_, d_pos4_.as<T4>());
-            launches_++;
-        } else if (cap) {
-            MB_TRY(splice_rebuild(*cap));
-        } else {
-            MB_TRY(enqueue_rebuild(true, false));
-        }
+        MB_TRY(after_drift(cap, true));  // (the exact displacement trigger whatever rebuild_every says)
         return enqueue_sd_eval(false, cap);
     }
     // The iteration loop: a conditional WHILE node (continue flag set by the decide kernel) whose body is one iteration, with
@@ -2960,6 +2954,20 @@ struct mb_ctx {
     if (!(ctx) || !(ctx)->e) return mb::set_error(MB_ERR_INVALID, "null context"); \
     if (cudaSetDevice((ctx)->device) != cudaSuccess) return mb::set_error(MB_ERR_CUDA, "cudaSetDevice failed")
 
+// the fields every mb_simulate_* parameter struct has, and the draws' keys; each entry point adds its method's fields
+template <typename P>
+static mb::Integrator integrator_call(int kind, const P* p, uint64_t rng_ctr1, uint64_t rng_key) {
+    mb::Integrator ig;
+    ig.kind = kind;
+    ig.dt = p->dt;
+    ig.n_steps = p->n_steps;
+    ig.init_step = p->init_step;
+    ig.remove_cm_every = p->remove_cm_every;
+    ig.rng_ctr1 = rng_ctr1;
+    ig.rng_key = rng_key;
+    return ig;
+}
+
 extern "C" {
 
 const char* mb_last_error(void) { return mb::g_last_error.c_str(); }
@@ -3061,31 +3069,42 @@ int mb_random_velocities(mb_ctx* ctx, void* vels, double kT, uint64_t rng_ctr1, 
     return ctx->e->random_velocities(vels, kT, rng_ctr1, rng_key);
 }
 int mb_kinetic_energy_tensor(mb_ctx* ctx, const void* vels, double* ke_tensor9_host) { MB_CTX_GUARD(ctx); return ctx->e->kinetic_tensor(vels, ke_tensor9_host); }
-int mb_simulate_vv(mb_ctx* ctx, void* coords, void* vels, const mb_vv_params_t* p) {
-    MB_CTX_GUARD(ctx);
-    return ctx->e->simulate(coords, vels, p, nullptr, nullptr, nullptr, nullptr);
-}
+int mb_simulate_vv(mb_ctx* ctx, void* coords, void* vels, const mb_vv_params_t* p) { return mb_simulate_vv_log(ctx, coords, vels, p, nullptr); }
 int mb_simulate_vv_log(mb_ctx* ctx, void* coords, void* vels, const mb_vv_params_t* p, mb_log_t* log) {
     MB_CTX_GUARD(ctx);
-    return ctx->e->simulate(coords, vels, p, nullptr, nullptr, nullptr, log);
+    if (!p) return mb::set_error(MB_ERR_INVALID, "null argument");
+    mb::Integrator ig = integrator_call(mb::INTEG_VV, p, p->rng_ctr1, p->rng_key);
+    ig.andersen_kT = p->andersen_kT;
+    ig.andersen_prob = p->andersen_prob;
+    return ctx->e->simulate(coords, vels, ig, log);
 }
 int mb_simulate_langevin(mb_ctx* ctx, void* coords, void* vels, const mb_langevin_params_t* p, mb_log_t* log) {
     MB_CTX_GUARD(ctx);
     if (!p) return mb::set_error(MB_ERR_INVALID, "null argument");
-    const mb_vv_params_t vp = {p->dt, p->n_steps, p->init_step, p->remove_cm_every, 0.0, 0.0, p->rng_ctr1, p->rng_key};
-    return ctx->e->simulate(coords, vels, &vp, p, nullptr, nullptr, log);
+    mb::Integrator ig = integrator_call(mb::INTEG_LANGEVIN, p, p->rng_ctr1, p->rng_key);
+    ig.kT = p->kT;
+    ig.friction = p->friction;
+    return ctx->e->simulate(coords, vels, ig, log);
 }
 int mb_simulate_nose_hoover(mb_ctx* ctx, void* coords, void* vels, const mb_nosehoover_params_t* p, mb_log_t* log) {
     MB_CTX_GUARD(ctx);
     if (!p) return mb::set_error(MB_ERR_INVALID, "null argument");
-    const mb_vv_params_t vp = {p->dt, p->n_steps, p->init_step, p->remove_cm_every, 0.0, 0.0, 0, 0};
-    return ctx->e->simulate(coords, vels, &vp, nullptr, p, nullptr, log);
+    mb::Integrator ig = integrator_call(mb::INTEG_NH, p, 0, 0);
+    ig.kT = p->kT;
+    ig.damping = p->damping;
+    return ctx->e->simulate(coords, vels, ig, log);
 }
 int mb_simulate_mts(mb_ctx* ctx, void* coords, void* vels, const mb_mts_params_t* p, mb_log_t* log) {
     MB_CTX_GUARD(ctx);
     if (!p) return mb::set_error(MB_ERR_INVALID, "null argument");
-    const mb_vv_params_t vp = {p->dt, p->n_steps, p->init_step, p->remove_cm_every, 0.0, 0.0, p->rng_ctr1, p->rng_key};
-    return ctx->e->simulate(coords, vels, &vp, nullptr, nullptr, p, log);
+    mb::Integrator ig = integrator_call(p->langevin ? mb::INTEG_MTS_LANGEVIN : mb::INTEG_MTS, p, p->rng_ctr1, p->rng_key);
+    ig.n_levels = p->n_levels;
+    std::copy_n(p->fractions, std::clamp(p->n_levels, 0, MB_MTS_MAX_LEVELS), ig.fractions.begin());
+    if (p->langevin) {  // (MTSIntegrator has neither)
+        ig.kT = p->kT;
+        ig.friction = p->friction;
+    }
+    return ctx->e->simulate(coords, vels, ig, log);
 }
 int mb_minimize_sd(mb_ctx* ctx, void* coords, mb_sd_params_t* p) { MB_CTX_GUARD(ctx); return ctx->e->minimize_sd(coords, p); }
 int mb_set_velocity_coupling(mb_ctx* ctx, const mb_vcoupling_t* c) {

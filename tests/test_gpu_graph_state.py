@@ -1,6 +1,7 @@
 """Captured graphs follow the context they run on: a setter called between two runs on the same context (masses, box or
 LJ cutoff through the C ABI, as a C or Julia caller would) must give the run a fresh context configured with the changed
-state would give, bit for bit, on the all-pairs and cell-list paths and for the minimiser."""
+state would give, bit for bit, on the all-pairs and cell-list paths and for the minimiser. So must a change of one
+integrator or thermostat parameter between two runs on the same context."""
 import ctypes as C
 
 import numpy as np
@@ -65,6 +66,61 @@ def test_setter_between_simulate_calls(system, change):
         assert sys_.stats()["graph_mode"] == 1
     assert np.array_equal(s.coords, ref.coords)
     assert np.array_equal(s.velocities, ref.velocities)
+    s.close()
+    ref.close()
+
+
+def _readme():
+    return H.make_system(H.readme_system(100, 2.0, seed=1), _lj(1.0), F64)
+
+
+def _chains():
+    """Chain molecules with bonded terms (test_gpu_mts): the bonded forces add with float atomics, so two contexts agree to
+    1e-12 nm, not bit for bit. A graph replayed with the old fractions or friction is off by many orders more."""
+    from test_gpu_mts import _molecules
+    return _molecules()[1]
+
+
+def _mts(si, friction=None):
+    if friction is None:
+        return mb.MTSIntegrator(0.002, pi_fractions=(1, 1), si_fractions=si)
+    return mb.MTSLangevinIntegrator(0.002, 120.0, friction, pi_fractions=(1, 1), si_fractions=si)
+
+
+# (system, the first call's integrator, the second call's): one parameter differs
+INTEGRATOR_CHANGES = {
+    "langevin-friction": (_readme, mb.Langevin(0.002, 300.0, 1.0), mb.Langevin(0.002, 300.0, 5.0)),
+    "langevin-temperature": (_readme, mb.Langevin(0.002, 300.0, 1.0), mb.Langevin(0.002, 350.0, 1.0)),
+    "nosehoover-damping": (_readme, mb.NoseHoover(0.002, 300.0, 0.2), mb.NoseHoover(0.002, 300.0, 0.05)),
+    # every list keeps its level, so the context keeps its graphs and only the key tells the calls apart
+    "mts-fractions": (_chains, _mts((2, 2, 1)), _mts((4, 4, 1))),
+    "mtslangevin-friction": (_chains, _mts((4, 2, 1), 10.0), _mts((4, 2, 1), 5.0)),
+    "andersen-coupling-const": (_readme, mb.VelocityVerlet(0.002, coupling=mb.AndersenThermostat(300.0, 0.1)),
+                                mb.VelocityVerlet(0.002, coupling=mb.AndersenThermostat(300.0, 0.02))),
+    "bussi-coupling-const": (_readme, mb.VelocityVerlet(0.002, coupling=mb.VelocityRescaleThermostat(300.0, 0.1)),
+                             mb.VelocityVerlet(0.002, coupling=mb.VelocityRescaleThermostat(300.0, 0.02))),
+}
+
+
+@pytest.mark.parametrize("change", list(INTEGRATOR_CHANGES))
+def test_integrator_parameter_between_simulate_calls(change):
+    """A step graph keeps the integrator's parameters by value: the second call, with one of them changed, must not replay
+    the first call's graph, and gives what a fresh context gives from the same state."""
+    make, first, second = INTEGRATOR_CHANGES[change]
+    s = make()
+    mb.simulate(s, first, N_STEPS, rng=np.random.default_rng(0))
+    assert s.stats()["graph_mode"] == 1
+    ref = make()
+    ref.coords[...], ref.velocities[...] = s.coords, s.velocities
+    for sys_ in (s, ref):
+        mb.simulate(sys_, second, N_STEPS, init_step=N_STEPS, rng=np.random.default_rng(1))
+        assert sys_.stats()["graph_mode"] == 1
+    if make is _chains:
+        from test_gpu_mts import _close
+        assert _close((s.coords, s.velocities), (ref.coords, ref.velocities))
+    else:
+        assert np.array_equal(s.coords, ref.coords)
+        assert np.array_equal(s.velocities, ref.velocities)
     s.close()
     ref.close()
 
