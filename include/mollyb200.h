@@ -402,6 +402,48 @@ typedef struct {
 } mb_mts_params_t;
 int mb_simulate_mts(mb_ctx* ctx, void* coords, void* vels, const mb_mts_params_t* p, mb_log_t* log);
 
+/* simulate!(sys, LangevinSplitting(dt, temperature, friction, splitting; remove_CM_motion), n_steps)
+ * (src/simulators.jl:1212-1398; BAOAB is Leimkuhler and Matthews 2013, OBABO Bussi and Parrinello 2007; "BAB" is the
+ * VelocityVerlet step and "BAOA" the Langevin step). ops[0 .. n_ops) is the splitting, a string over 'A', 'B' and 'O'. Each
+ * letter takes the effective step dt / count(letter, splitting):
+ *   A: x += v dt_A;   B: v += F/m dt_B;   O: v = c_i v + sigma_i xi with xi ~ N(0, 1)^3,
+ *   c_i = exp(-friction dt / n_O / m_i), sigma_i = sqrt(kT / m_i (1 - c_i^2)) (n_O: the O's in the splitting).
+ * The friction is a mass per time (g mol^-1 ps^-1), unlike mb_simulate_langevin's. Prologue as mb_simulate_vv: wrap, CM
+ * removal when init_step == 0 and remove_cm_every != 0, neighbours, F0, loggers at init_step. Step n: the letters in
+ * order; wrap; CM removal when n % remove_cm_every == 0; neighbours; loggers (mb_log_t, as for mb_simulate_vv_log; NULL: no
+ * logging). Forces are recomputed as the reference recomputes them: they are known at the start of a step unless an A
+ * follows the last B, an A makes them unknown, and a B recomputes them only when they are unknown. So BAOAB, OBABO, ABOBA,
+ * BAOA, AB and BA evaluate the forces once per step, BABAB twice, and a splitting without an A or without a B never. A B that
+ * recomputes before any A of its step is served by an evaluation at the end of the step before (the first: F0), at the same
+ * positions. Each stretch of letters between two evaluations is one fused kernel. Where the engine differs from the
+ * reference:
+ *  - random numbers: xi of atom i (1-based original index) at the j-th O (0-based) of step n is the Box-Muller transform of
+ *    one Philox4x32-10 block with counter (i, n, ctr1 + j as a 64-bit sum) and key `rng_key`; for j = 0 this is
+ *    mb_simulate_langevin's draw. A function of (keys, step, j, atom) only, so a run split into calls with the same keys takes
+ *    the same draws; the reference's draws agree in distribution only, as for Langevin;
+ *  - neighbours: the exact displacement trigger of mb_simulate_vv, tested after every stretch of letters that moves the
+ *    atoms, so every force evaluation reads current lists. The all-pairs path wraps at those points, not after every A;
+ *  - f32: c_i and sigma_i are formed in double from the context's 1/m (rounded to the dtype), and c_i v + sigma_i xi is
+ *    formed in double and rounded once;
+ *  - massless atoms (1/m = 0) get no kick and no noise (c_i = 1, sigma_i = 0);
+ *  - at most MB_SPLIT_MAX_OPS letters (the passes are unrolled into the captured step graph).
+ * MB_ERR_INVALID before any work for an empty splitting, a letter other than 'A', 'B', 'O', more than MB_SPLIT_MAX_OPS
+ * letters, dt <= 0, n_steps < 0, kT or friction negative or not finite, a velocity coupling set on the context, a
+ * decomposed (multi-GPU) context, and the logging errors of mb_simulate_vv_log. MB_ERR_CAPACITY as in mb_simulate_vv. */
+#define MB_SPLIT_MAX_OPS 32
+typedef struct {
+    double dt;
+    int64_t n_steps;
+    int64_t init_step;
+    int32_t remove_cm_every;    /* LangevinSplitting.remove_CM_motion (default 1; 0 = never) */
+    double kT;                  /* k * temperature in kJ/mol */
+    double friction;            /* g mol^-1 ps^-1 (mass per time) */
+    uint64_t rng_ctr1, rng_key; /* the draws' keys */
+    int32_t n_ops;              /* letters in ops */
+    char ops[MB_SPLIT_MAX_OPS]; /* the splitting: 'A', 'B', 'O' (not NUL-terminated) */
+} mb_splitting_params_t;
+int mb_simulate_langevin_splitting(mb_ctx* ctx, void* coords, void* vels, const mb_splitting_params_t* p, mb_log_t* log);
+
 /* simulate!(sys, SteepestDescentMinimizer(step_size, max_steps, tol)) (src/simulators.jl:183-274) on the device: wrap the
  * coordinates, E = potential energy; then for step n = init_step+1 .. init_step+max_steps: F = forces, m = max |F_i|,
  * x <- wrap(x + h F / m), E_trial = potential energy; E_trial < E accepts (h <- 6h/5, E <- E_trial), otherwise x is restored

@@ -11,6 +11,7 @@
 #   Molly.simulate!(sys, sim::SteepestDescentMinimizer; ...)                                                simulators.jl:183
 #   Molly.simulate!(sys, sim::Langevin, n_steps; ...) with coupling === nothing                              simulators.jl:1101
 #   Molly.simulate!(sys, sim::NoseHoover, n_steps; ...) with coupling === nothing                            simulators.jl:1534
+#   Molly.simulate!(sys, sim::LangevinSplitting, n_steps; ...) with at most 32 letters                      simulators.jl:1252
 #   Molly.simulate!(sys, sim::AbstractMTSIntegrator, n_steps; ...) with coupling === nothing                 simulators.jl:1850
 # (Molly.remove_CM_motion! for CuArray Systems is NOT redefined: the stock extension owns that exact signature)
 # and falls through to the stock methods (invoke) for anything it does not recognise: non-cubic boundaries,
@@ -68,6 +69,20 @@ struct MBLangevinParams
     friction::Float64
     rng_ctr1::UInt64
     rng_key::UInt64
+end
+
+# mb_splitting_params_t (mb_simulate_langevin_splitting)
+struct MBSplittingParams
+    dt::Float64
+    n_steps::Int64
+    init_step::Int64
+    remove_cm_every::Int32
+    kT::Float64
+    friction::Float64
+    rng_ctr1::UInt64
+    rng_key::UInt64
+    n_ops::Int32
+    ops::NTuple{32, UInt8}
 end
 
 # mb_nosehoover_params_t (mb_simulate_nose_hoover)
@@ -504,6 +519,45 @@ function Molly.simulate!(sys::System{3, <:CuArray, T}, sim::Langevin, n_steps::I
         end
     end
     check(ccall((:mb_simulate_langevin, LIB), Cint, (Ptr{Cvoid}, CuPtr{Cvoid}, CuPtr{Cvoid}, Ref{MBLangevinParams}, Ptr{MBLog}),
+                ctx.handle, pointer(sys.coords), pointer(sys.velocities), Ref(p), C_NULL))
+    return sys
+end
+
+# ---- simulate!(sys, ::LangevinSplitting, n) (src/simulators.jl:1252-1398) --------------------------------------------------
+# Taken over under the conditions of the Langevin method above (LangevinSplitting has no coupling) when the splitting has 1 to
+# 32 letters, all of them A, B or O: one mb_simulate_langevin_splitting call. The friction is a mass per time, converted to
+# g mol^-1 ps^-1 (a plain number is taken as that). An invalid letter runs the stock method, which raises its ArgumentError.
+function Molly.simulate!(sys::System{3, <:CuArray, T}, sim::LangevinSplitting, n_steps::Integer;
+                         init_step=0, rng=Random.default_rng(), run_loggers=true, kwargs...) where T
+    descs = engine_eligible(sys, sys.pairwise_inters)
+    device_logs = run_loggers == false || isempty(sys.loggers) ||
+                  all(l -> !isnothing(device_log_kind(l)), values(sys.loggers))
+    ops = collect(String(sim.splitting))
+    if isnothing(descs) || !device_logs || !general_ok(sys) || !gb_ok(sys) ||
+            !all(!isnothing, map(specific_desc, sys.specific_inter_lists)) ||
+            !(1 <= length(ops) <= 32) || !all(op -> op in ('A', 'B', 'O'), ops)
+        # stock: simulate!(sys, sim::LangevinSplitting, n_steps_or_time; ...) src/simulators.jl:1252
+        return invoke(Molly.simulate!, Tuple{Any, LangevinSplitting, Any}, sys, sim, n_steps;
+                      init_step=init_step, rng=rng, run_loggers=run_loggers, kwargs...)
+    end
+    ctx = context_for(sys, descs)
+    set_specific!(ctx, sys)
+    set_implicit_solvent!(ctx, sys)
+    set_velocity_coupling!(ctx, nothing)
+    friction = sim.friction isa Unitful.Quantity ? Float64(ustrip(u"g * mol^-1 * ps^-1", sim.friction)) : Float64(sim.friction)
+    letters = ntuple(i -> i <= length(ops) ? UInt8(ops[i]) : 0x00, 32)
+    p = MBSplittingParams(_ps(sim.dt), n_steps, init_step, Int32(sim.remove_CM_motion),
+                          Float64(ustrip(sys.k * sim.temperature)), friction, rand(rng, UInt64), rand(rng, UInt64),
+                          Int32(length(ops)), letters)
+    if run_loggers != false && !isempty(sys.loggers)
+        return simulate_logged!(sys, ctx, n_steps, init_step, run_loggers) do lg
+            ccall((:mb_simulate_langevin_splitting, LIB), Cint,
+                  (Ptr{Cvoid}, CuPtr{Cvoid}, CuPtr{Cvoid}, Ref{MBSplittingParams}, Ref{MBLog}),
+                  ctx.handle, pointer(sys.coords), pointer(sys.velocities), Ref(p), lg)
+        end
+    end
+    check(ccall((:mb_simulate_langevin_splitting, LIB), Cint,
+                (Ptr{Cvoid}, CuPtr{Cvoid}, CuPtr{Cvoid}, Ref{MBSplittingParams}, Ptr{MBLog}),
                 ctx.handle, pointer(sys.coords), pointer(sys.velocities), Ref(p), C_NULL))
     return sys
 end

@@ -23,9 +23,11 @@ EXPORTED = [
     "mb_set_lj_dispersion_correction", "mb_random_velocities", "mb_kinetic_energy_tensor", "mb_set_box_triclinic",
     "mb_simulate_vv_log", "mb_minimize_sd", "mb_set_velocity_coupling", "mb_simulate_langevin",
     "mb_simulate_nose_hoover", "mb_set_specific_levels", "mb_simulate_mts", "mb_set_implicit_solvent",
+    "mb_simulate_langevin_splitting",
 ]
 MB_GB_MAX_NECK_CLASSES = 32
 MB_MTS_MAX_LEVELS = 8
+MB_SPLIT_MAX_OPS = 32
 
 
 class MBInter(C.Structure):
@@ -84,6 +86,14 @@ class MBMTSParams(C.Structure):
         ("dt", C.c_double), ("n_steps", C.c_int64), ("init_step", C.c_int64), ("remove_cm_every", C.c_int32),
         ("n_levels", C.c_int32), ("fractions", C.c_int32 * MB_MTS_MAX_LEVELS), ("langevin", C.c_int32), ("reserved_", C.c_int32),
         ("kT", C.c_double), ("friction", C.c_double), ("rng_ctr1", C.c_uint64), ("rng_key", C.c_uint64),
+    ]
+
+
+class MBSplittingParams(C.Structure):
+    _fields_ = [
+        ("dt", C.c_double), ("n_steps", C.c_int64), ("init_step", C.c_int64), ("remove_cm_every", C.c_int32),
+        ("kT", C.c_double), ("friction", C.c_double), ("rng_ctr1", C.c_uint64), ("rng_key", C.c_uint64),
+        ("n_ops", C.c_int32), ("ops", C.c_char * MB_SPLIT_MAX_OPS),
     ]
 
 
@@ -147,6 +157,7 @@ def load():
     L.mb_simulate_langevin.argtypes = [vp, vp, vp, C.POINTER(MBLangevinParams), C.POINTER(MBLog)]
     L.mb_simulate_nose_hoover.argtypes = [vp, vp, vp, C.POINTER(MBNoseHooverParams), C.POINTER(MBLog)]
     L.mb_simulate_mts.argtypes = [vp, vp, vp, C.POINTER(MBMTSParams), C.POINTER(MBLog)]
+    L.mb_simulate_langevin_splitting.argtypes = [vp, vp, vp, C.POINTER(MBSplittingParams), C.POINTER(MBLog)]
     L.mb_set_specific_levels.argtypes = [vp, C.c_int, i64, vp]
     L.mb_minimize_sd.argtypes = [vp, vp, C.POINTER(MBSDParams)]
     L.mb_set_velocity_coupling.argtypes = [vp, C.POINTER(MBVCoupling)]

@@ -13,6 +13,7 @@ julia/MollyB200Ext.jl, see INTEGRATION.md):
     VelocityRescaleThermostat                       simulate, see mb_set_velocity_coupling)
     SteepestDescentMinimizer                        src/simulators.jl:183-274 (simulate dispatches on the simulator)
     Langevin                                        src/simulators.jl:1065-1210 (mb_simulate_langevin)
+    LangevinSplitting                               src/simulators.jl:1212-1398 (mb_simulate_langevin_splitting)
     NoseHoover                                      src/simulators.jl:1491-1614 (mb_simulate_nose_hoover)
     MTSIntegrator, MTSLangevinIntegrator            src/simulators.jl:1616-1940 (mb_simulate_mts)
     forces, forces_virial, potential_energy         src/force.jl:678-720, src/energy.jl:202-248
@@ -531,6 +532,36 @@ class Langevin:
             raise ValueError(f"remove_CM_motion must be non-negative, found {self.remove_CM_motion}")
         self.vel_scale = math.exp(-self.dt * self.friction)
         self.noise_scale = math.sqrt(1 - self.vel_scale ** 2)
+
+
+@dataclass
+class LangevinSplitting:
+    """LangevinSplitting(dt, temperature, friction, splitting; remove_CM_motion=1) — src/simulators.jl:1212-1398, the
+    Langevin integrator with any splitting of A (positions), B (forces) and O (friction and noise) steps, run on the device
+    by mb_simulate_langevin_splitting (see include/mollyb200.h for where the engine differs from the reference). dt in ps,
+    temperature in K, friction in g mol^-1 ps^-1 (a mass per time, unlike Langevin's). "BAOAB" samples configurations well
+    (Leimkuhler-Matthews), "BAB" is the VelocityVerlet step and "BAOA" the Langevin step. Raises ValueError where the
+    reference raises ArgumentError (a letter other than A, B, O), and for what the engine refuses: an empty splitting, more
+    than MB_SPLIT_MAX_OPS letters, dt, temperature or friction out of range."""
+    dt: float
+    temperature: float
+    friction: float
+    splitting: str
+    remove_CM_motion: int = 1
+
+    def __post_init__(self):
+        if not (math.isfinite(self.dt) and self.dt > 0):
+            raise ValueError(f"dt must be finite and positive, found {self.dt}")
+        _check_temperature(self.temperature)
+        if not (math.isfinite(self.friction) and self.friction >= 0):
+            raise ValueError(f"friction must be finite and non-negative, found {self.friction}")
+        if not isinstance(self.splitting, str) or not all(op in "ABO" for op in self.splitting):
+            raise ValueError("splitting must contain only A, B, and O steps")
+        if not 1 <= len(self.splitting) <= capi.MB_SPLIT_MAX_OPS:
+            raise ValueError(f"splitting must have 1 to {capi.MB_SPLIT_MAX_OPS} letters, found {len(self.splitting)}")
+        self.remove_CM_motion = int(self.remove_CM_motion)  # Int(remove_CM_motion): false -> 0
+        if self.remove_CM_motion < 0:
+            raise ValueError(f"remove_CM_motion must be non-negative, found {self.remove_CM_motion}")
 
 
 @dataclass
@@ -1083,6 +1114,7 @@ def steepest_descent(sys: System, sim: SteepestDescentMinimizer, init_step: int 
 _SIMULATE_ENTRY = {
     VelocityVerlet: (capi.MBVVParams, "mb_simulate_vv_log"),
     Langevin: (capi.MBLangevinParams, "mb_simulate_langevin"),
+    LangevinSplitting: (capi.MBSplittingParams, "mb_simulate_langevin_splitting"),
     NoseHoover: (capi.MBNoseHooverParams, "mb_simulate_nose_hoover"),
     MTSIntegrator: (capi.MBMTSParams, "mb_simulate_mts"),
     MTSLangevinIntegrator: (capi.MBMTSParams, "mb_simulate_mts"),
@@ -1097,6 +1129,8 @@ def simulate(sys: System, sim, n_steps: Optional[int] = None, init_step: int = 0
     velocities and appends to the histories of sys.loggers (recorded on the device, see _LogPlan).
     Langevin: simulate!(sys, sim, n_steps; run_loggers=true) — src/simulators.jl:1101-1210, the same arguments and loggers
     as VelocityVerlet; the velocities are half a step behind the positions.
+    LangevinSplitting: simulate!(sys, sim, n_steps; run_loggers=true) — src/simulators.jl:1252-1398, the same arguments and
+    loggers as VelocityVerlet.
     NoseHoover: simulate!(sys, sim, n_steps; run_loggers=true) — src/simulators.jl:1534-1614, the same arguments and loggers
     as VelocityVerlet; zeta starts at 0 in every call.
     MTSIntegrator, MTSLangevinIntegrator: simulate!(sys, sim, n_steps; run_loggers=true) — src/simulators.jl:1783-1940,
@@ -1120,7 +1154,8 @@ def simulate(sys: System, sim, n_steps: Optional[int] = None, init_step: int = 0
     if run_loggers is None:
         run_loggers = True
     _check_run_loggers(run_loggers)
-    couplings = sim.coupling if isinstance(sim.coupling, (tuple, list)) else ((sim.coupling,) if sim.coupling else ())
+    coupling = getattr(sim, "coupling", None)  # (LangevinSplitting has none)
+    couplings = coupling if isinstance(coupling, (tuple, list)) else ((coupling,) if coupling else ())
     mts = params_t is capi.MBMTSParams
     p = params_t()  # (zero-filled: no Andersen thermostat, no noise)
     vc = None
@@ -1140,10 +1175,13 @@ def simulate(sys: System, sim, n_steps: Optional[int] = None, init_step: int = 0
         p.n_levels = len(sim.ordered_fractions)
         p.fractions[:p.n_levels] = sim.ordered_fractions
         p.langevin = int(isinstance(sim, MTSLangevinIntegrator))
-    if isinstance(sim, (Langevin, NoseHoover, MTSLangevinIntegrator)):
+    if isinstance(sim, (Langevin, NoseHoover, MTSLangevinIntegrator, LangevinSplitting)):
         p.kT = sys.k * sim.temperature
-    if isinstance(sim, (Langevin, MTSLangevinIntegrator)):
+    if isinstance(sim, (Langevin, MTSLangevinIntegrator, LangevinSplitting)):
         p.friction = float(sim.friction)
+    if isinstance(sim, LangevinSplitting):
+        p.n_ops = len(sim.splitting)
+        p.ops = sim.splitting.encode()
     if isinstance(sim, NoseHoover):
         p.damping = float(sim.damping)
     p.dt = float(sim.dt)

@@ -21,6 +21,7 @@
 #include "nosehoover.cuh"
 #include "pair.cuh"
 #include "pme.cuh"
+#include "splitting.cuh"
 #include "vv.cuh"
 static_assert(mb::MTS_MAX_LEVELS == MB_MTS_MAX_LEVELS, "mts.cuh levels = MB_MTS_MAX_LEVELS");
 static_assert((int)mb::VC_NONE == (int)MB_VC_NONE && (int)mb::VC_IMMEDIATE == (int)MB_VC_IMMEDIATE &&
@@ -316,9 +317,11 @@ static void pme_plan_host(const double box[3], double r_cut, double error_tol, i
     }
 }
 
-// The integrator of one simulate call: VelocityVerlet (vv.cuh), Langevin (langevin.cuh), Nose-Hoover (nosehoover.cuh) or the
-// multiple-time-step integrators (mts.cuh). Each mb_simulate_* entry point fills one from its own parameters.
-enum { INTEG_VV = 0, INTEG_LANGEVIN = 1, INTEG_NH = 2, INTEG_MTS = 3, INTEG_MTS_LANGEVIN = 4 };
+// The integrator of one simulate call: VelocityVerlet (vv.cuh), Langevin (langevin.cuh), Nose-Hoover (nosehoover.cuh), the
+// multiple-time-step integrators (mts.cuh) or LangevinSplitting (splitting.cuh). Each mb_simulate_* entry point fills one
+// from its own parameters.
+enum { INTEG_VV = 0, INTEG_LANGEVIN = 1, INTEG_NH = 2, INTEG_MTS = 3, INTEG_MTS_LANGEVIN = 4, INTEG_SPLIT = 5 };
+static_assert(SPLIT_MAX_OPS == MB_SPLIT_MAX_OPS, "splitting length");
 static bool is_mts(int kind) { return kind == INTEG_MTS || kind == INTEG_MTS_LANGEVIN; }
 struct Integrator {
     int kind = INTEG_VV;  // INTEG_*
@@ -327,15 +330,76 @@ struct Integrator {
     int remove_cm_every = 0;
     uint64_t rng_ctr1 = 0, rng_key = 0;
     double andersen_kT = 0, andersen_prob = 0;  // VelocityVerlet's Andersen thermostat (kT <= 0 or prob <= 0: none)
-    double kT = 0, friction = 0, damping = 0;   // Langevin and MTSLangevinIntegrator: kT, friction; Nose-Hoover: kT, damping
+    double kT = 0, friction = 0, damping = 0;   // Langevin, MTSLangevinIntegrator and LangevinSplitting: kT, friction;
+                                                // Nose-Hoover: kT, damping
     int n_levels = 0;                           // the multiple-time-step integrators' ordered fractions (0 levels: none)
     std::array<int, MTS_MAX_LEVELS> fractions = {};
+    int n_ops = 0;                              // LangevinSplitting's splitting: the letters 'A', 'B', 'O' (0: none)
+    std::array<char, SPLIT_MAX_OPS> ops = {};
     // What the step graphs bake in (GraphKey): every field but n_steps, init_step and the RNG keys, which are uploaded
     // into Control on every call
     auto graph_fields() const {
-        return std::tie(kind, dt, remove_cm_every, andersen_kT, andersen_prob, kT, friction, damping, n_levels, fractions);
+        return std::tie(kind, dt, remove_cm_every, andersen_kT, andersen_prob, kT, friction, damping, n_levels, fractions, n_ops,
+                        ops);
     }
 };
+
+// LangevinSplitting's step cut into passes at its force evaluations (simulate!'s force_computation_steps, src/simulators.jl:
+// 1305-1324). Forces are known at the start of a step unless an A follows the last B; an A makes them unknown and a B
+// recomputes them only when they are unknown. A recomputing B is served by an evaluation right after the last A in front of
+// it; only O's lie between the two, so the positions are the same. One that has no A in front of it in the step is served by
+// an evaluation at the end of the step before (at the first step: the call's F0). Passes never come out empty.
+struct SplitPlan {
+    int n_pass = 0, n_evals = 0;                // passes and force evaluations per step
+    std::array<SplitProg, SPLIT_MAX_OPS> pass;  // (apply_cm, last set; the letters as SPLIT_*)
+    std::array<bool, SPLIT_MAX_OPS> eval_after; // a force evaluation follows the pass (the last pass: the end-of-step one)
+    int count[3] = {0, 0, 0};                   // letters A, B, O in the splitting
+};
+static SplitPlan split_plan(const Integrator& ig) {
+    SplitPlan sp;
+    const int n = ig.n_ops;
+    std::array<int, SPLIT_MAX_OPS> op = {};
+    int last_b = -1;
+    for (int k = 0; k < n; k++) {
+        op[k] = ig.ops[k] == 'A' ? SPLIT_A : (ig.ops[k] == 'B' ? SPLIT_B : SPLIT_O);
+        sp.count[op[k]]++;
+        if (op[k] == SPLIT_B) last_b = k;
+    }
+    bool a_after_last_b = false;  // the splitting matches ^.*B[^B]*A[^B]*$
+    for (int k = last_b + 1; last_b >= 0 && k < n; k++) a_after_last_b |= op[k] == SPLIT_A;
+    std::array<bool, SPLIT_MAX_OPS> cut = {};  // an evaluation after letter k
+    bool known = !a_after_last_b, end_eval = false;
+    int last_a = -1;
+    for (int k = 0; k < n; k++) {
+        if (op[k] == SPLIT_A) { known = false; last_a = k; }
+        if (op[k] == SPLIT_B && !known) {
+            known = true;
+            if (last_a >= 0) cut[last_a] = true;
+            else end_eval = true;
+        }
+    }
+    sp.pass.fill(SplitProg{});
+    sp.eval_after.fill(false);
+    int j = 0;
+    for (int k = 0; k < n; k++) {
+        SplitProg& pg = sp.pass[sp.n_pass];
+        if (pg.n_ops == 0) pg.o_base = j;
+        pg.ops |= (unsigned long long)op[k] << (2 * pg.n_ops);
+        pg.n_ops++;
+        j += op[k] == SPLIT_O ? 1 : 0;
+        pg.has_a |= op[k] == SPLIT_A;
+        pg.has_b |= op[k] == SPLIT_B;
+        pg.has_o |= op[k] == SPLIT_O;
+        if (cut[k] || k == n - 1) {
+            sp.eval_after[sp.n_pass] = cut[k] || end_eval;
+            sp.n_evals += sp.eval_after[sp.n_pass] ? 1 : 0;
+            sp.n_pass++;
+        }
+    }
+    sp.pass[0].apply_cm = 1;  // (every pass reads v)
+    sp.pass[sp.n_pass - 1].last = 1;
+    return sp;
+}
 
 class EngineBase {
    public:
@@ -1884,6 +1948,8 @@ class Engine : public EngineBase {
         VCouple vc;       // velocity-rescaling thermostat (kind VC_NONE: none)
         LangevinCoef lc;  // Langevin's (or MTSLangevinIntegrator's) c, sqrt(1 - c^2) and kT
         NhCoef nc;        // Nose-Hoover's dt / (2 Q^2) and Nf k T0
+        SplitCoef<T> sc;  // LangevinSplitting's dt_A, dt_B, -friction dt_O and kT
+        SplitPlan sp;     // LangevinSplitting's passes and evaluations
     };
     // Langevin's c = exp(-dt friction), sqrt(1 - c^2) and kT (src/simulators.jl:1092-1097), in double. MTSLangevinIntegrator
     // runs its O step at the innermost substep, with f the innermost fraction: c = exp(-dt friction / f) (:1736-1738);
@@ -1908,6 +1974,13 @@ class Engine : public EngineBase {
         c.nc = NhCoef{0.0, 1.0};
         if (ig.kind == INTEG_NH)  // NoseHoover(dt, temperature, damping): dt / (2 damping^2) and Nf k T0 (src/simulators.jl:1575-1579), in double
             c.nc = NhCoef{ig.dt / (2.0 * ig.damping * ig.damping), (double)(3 * (long long)n_ - 3) * ig.kT};
+        c.sc = SplitCoef<T>{};
+        if (ig.kind == INTEG_SPLIT) {  // effective steps dt / count(letter); the O rate -friction dt / n_O as the reference forms it
+            c.sp = split_plan(ig);
+            const int* k = c.sp.count;
+            c.sc = SplitCoef<T>{k[SPLIT_A] ? (T)(ig.dt / k[SPLIT_A]) : (T)0, k[SPLIT_B] ? (T)(ig.dt / k[SPLIT_B]) : (T)0,
+                                k[SPLIT_O] ? -ig.friction * ig.dt / k[SPLIT_O] : 0.0, ig.kT};
+        }
         return c;
     }
     // what one step does beyond the plain VelocityVerlet step
@@ -1918,23 +1991,41 @@ class Engine : public EngineBase {
         bool defer_cm = false;           // decomposed: the next step's K1 sums the slabs' momenta itself
         int log_mask = 0;                // LOG_* records after the step
     };
-    // capture mode (capture_graph): the handles of the conditional rebuild node (cell-list path) and of the WHILE loop (if
-    // any), and the rebuild node's body once splice_rebuild has added it
-    struct Capture { cudaGraphConditionalHandle rebuild = 0, loop = 0; cudaGraph_t body = nullptr; };
-    // a conditional IF node on the rebuild handle in place of the gated rebuild; capture_graph fills its body
+    // capture mode (capture_graph): the handle of the WHILE loop (if any) and, on the cell-list path, one (handle, body) per
+    // conditional rebuild node: CUDA ties a handle to one conditional node, and a graph with a handle that no node reads does
+    // not instantiate. So each handle is created when the kernel that publishes its decision is enqueued (rebuild_handle),
+    // and a step with several rebuild points (LangevinSplitting) gets one per point.
+    struct Capture {
+        cudaGraphConditionalHandle loop = 0;
+        cudaGraph_t graph = nullptr;                       // the graph the handles belong to
+        std::vector<cudaGraphConditionalHandle> rebuild;  // rebuild[i]: the handle of the i-th rebuild node
+        std::vector<cudaGraph_t> body;                     // the bodies splice_rebuild has added, in order
+    };
+    // the handle the next rebuild node will read (0 on the all-pairs path), for the kernel that publishes its decision
+    cudaGraphConditionalHandle rebuild_handle(Capture* cap) {
+        if (!cap || path_ != 1) return 0;
+        if (cap->rebuild.size() <= cap->body.size()) {
+            cudaGraphConditionalHandle h = 0;
+            if (cudaGraphConditionalHandleCreate(&h, cap->graph, 0, cudaGraphCondAssignDefault) != cudaSuccess) return 0;
+            cap->rebuild.push_back(h);  // (a failure leaves one handle short, which splice_rebuild reports)
+        }
+        return cap->rebuild[cap->body.size()];
+    }
+    // a conditional IF node on the next rebuild handle in place of the gated rebuild; capture_graph fills its body
     int splice_rebuild(Capture& cap) {
+        if (cap.rebuild.size() <= cap.body.size()) return set_error(MB_ERR_CUDA, "no conditional handle for a rebuild node");
         cudaStreamCaptureStatus status;
         const cudaGraphNode_t* deps = nullptr;
         size_t ndeps = 0;
         cudaGraph_t gcap = nullptr;
         MB_CUDA(cudaStreamGetCaptureInfo_v2(stream_, &status, nullptr, &gcap, &deps, &ndeps));
         cudaGraphNodeParams cp = {cudaGraphNodeTypeConditional};
-        cp.conditional.handle = cap.rebuild;
+        cp.conditional.handle = cap.rebuild[cap.body.size()];
         cp.conditional.type = cudaGraphCondTypeIf;
         cp.conditional.size = 1;
         cudaGraphNode_t cnode;
         MB_CUDA(cudaGraphAddNode(&cnode, gcap, deps, ndeps, &cp));
-        cap.body = cp.conditional.phGraph_out[0];
+        cap.body.push_back(cp.conditional.phGraph_out[0]);
         MB_CUDA(cudaStreamUpdateCaptureDependencies(stream_, &cnode, 1, cudaStreamSetCaptureDependencies));
         return MB_OK;
     }
@@ -1964,6 +2055,7 @@ class Engine : public EngineBase {
     }
     int enqueue_step(const StepCfg& c, const StepOpts& o, Capture* cap = nullptr) {
         if (is_mts(c.ig.kind)) return enqueue_mts_step(c, o, cap);
+        if (c.ig.kind == INTEG_SPLIT) return enqueue_split_step(c, o, cap);
         const bool dec = decomposed() && path_ == 1;
         const int s0 = dec ? own_s0_ : 0, n_own = dec ? own_n_ : (int)n_;
         Control* ctl = d_ctl_.as<Control>();
@@ -1988,13 +2080,13 @@ class Engine : public EngineBase {
             langevin_step_kernel<T><<<grid, VV_THREADS, 0, stream_>>>(
                 n_own, c.dt, c.dt_half, c.skin_half2, c.lc, o.do_cm, c.inv_mass, cm, d_f4_.as<T4>(), d_xref4_.as<T4>(),
                 d_pos4_.as<T4>(), d_vel4_.as<T4>(), d_orig_.as<int>(), d_mass_.as<T>(), d_partial_.as<double>(), c.flag_ptr, ctl,
-                cap ? cap->rebuild : 0, cap && path_ == 1 ? 1 : 0, ext_map());
+                rebuild_handle(cap), cap && path_ == 1 ? 1 : 0, ext_map());
         } else if (c.ig.kind == INTEG_NH) {  // (single GPU: s0 = 0)
             MB_TRY(integ_grid(grid, n_own, 1, 8, 2));
             nh_kick_drift_kernel<T><<<grid, VV_THREADS, 0, stream_>>>(
                 n_own, c.dt, c.dt_half, c.skin_half2, c.nc, d_nh_.as<NhState>(), cm, d_f4_.as<T4>(), d_xref4_.as<T4>(),
                 d_pos4_.as<T4>(), d_vel4_.as<T4>(), d_mass_.as<T>(), d_partial_.as<double>(), c.flag_ptr, ctl,
-                cap ? cap->rebuild : 0, cap && path_ == 1 ? 1 : 0, ext_map());
+                rebuild_handle(cap), cap && path_ == 1 ? 1 : 0, ext_map());
         } else {
             const Thermo<T> th = thermo_in_k1(c);
             const int thk = th.on ? TH_ANDERSEN : (c.vc.kind != VC_NONE ? TH_SCALE : TH_NONE);
@@ -2002,7 +2094,7 @@ class Engine : public EngineBase {
             with_const<TH_NONE, TH_ANDERSEN, TH_SCALE>(thk, [&](auto TH) {
                 vv_kick_drift_kernel<T, TH><<<grid, VV_THREADS, 0, stream_>>>(
                     s0, n_own, c.dt, c.dt_half, c.skin_half2, cm, d_f4_.as<T4>(), d_xref4_.as<T4>(), d_pos4_.as<T4>(), d_vel4_.as<T4>(),
-                    c.flag_ptr, ctl, cap ? cap->rebuild : 0, cap && path_ == 1 ? 1 : 0, push, ext_map(), th);
+                    c.flag_ptr, ctl, rebuild_handle(cap), cap && path_ == 1 ? 1 : 0, push, ext_map(), th);
             });
         }
         prof_.end(Prof::VV);
@@ -2127,7 +2219,7 @@ class Engine : public EngineBase {
                 with_const<true, false>(c.ig.kind == INTEG_MTS_LANGEVIN, [&](auto LG) {
                     mts_kick_drift_kernel<T, LG><<<grid, VV_THREADS, 0, stream_>>>(
                         n, dt_v, (T)dt_x, (T)(dt_x / 2), c.skin_half2, c.lc, w.substep, apply_cm, last, cm, f, d_xref4_.as<T4>(),
-                        d_pos4_.as<T4>(), d_vel4_.as<T4>(), d_orig_.as<int>(), c.flag_ptr, ctl, cap ? cap->rebuild : 0,
+                        d_pos4_.as<T4>(), d_vel4_.as<T4>(), d_orig_.as<int>(), c.flag_ptr, ctl, rebuild_handle(cap),
                         cap && path_ == 1 ? 1 : 0, ext_map());
                 });
                 prof_.end(Prof::VV);
@@ -2163,6 +2255,33 @@ class Engine : public EngineBase {
     int enqueue_mts_step(const StepCfg& c, const StepOpts& o, Capture* cap) {
         MtsWalk w;
         MB_TRY(enqueue_mts_level(c, o, cap, 0, false, w));
+        if (o.log_mask) MB_TRY(enqueue_log(c, o.log_mask));
+        MB_CUDA(cudaGetLastError());
+        return MB_OK;
+    }
+    // One LangevinSplitting step (splitting.cuh): its passes in order (SplitPlan). A pass that moves the atoms is followed by
+    // the rebuild node (capture), the gated rebuild (stream: always enqueued, the device flag decides) or the wrap (all-pairs
+    // path); a force evaluation into d_f4_ follows where the plan puts one. Graph and stream issue the same kernels.
+    int enqueue_split_step(const StepCfg& c, const StepOpts& o, Capture* cap) {
+        const int n = (int)n_;
+        Control* ctl = d_ctl_.as<Control>();
+        for (int p = 0; p < c.sp.n_pass; p++) {
+            const SplitProg& pg = c.sp.pass[p];
+            int grid;
+            MB_TRY(integ_grid(grid, n, 1, 8, 3));
+            prof_.begin(Prof::VV);
+            split_pass_kernel<T><<<grid, VV_THREADS, 0, stream_>>>(
+                n, pg, c.sc, c.skin_half2, o.do_cm, c.inv_mass, d_cm_.as<CmState<T>>(), d_f4_.as<T4>(), d_xref4_.as<T4>(),
+                d_pos4_.as<T4>(), d_vel4_.as<T4>(), d_orig_.as<int>(), d_mass_.as<T>(), d_partial_.as<double>(), c.flag_ptr, ctl,
+                pg.has_a ? rebuild_handle(cap) : 0, cap && path_ == 1 ? 1 : 0, ext_map());
+            prof_.end(Prof::VV);
+            launches_++;
+            if (pg.has_a) MB_TRY(after_drift(cap, true));
+            if (c.sp.eval_after[p]) {
+                MB_TRY(launch_pairs(false, d_f4_.as<T4>()));
+                MB_TRY(launch_bonded(false));
+            }
+        }
         if (o.log_mask) MB_TRY(enqueue_log(c, o.log_mask));
         MB_CUDA(cudaGetLastError());
         return MB_OK;
@@ -2223,6 +2342,7 @@ class Engine : public EngineBase {
         cudaGraph_t graph = nullptr;
         cudaGraphExec_t exec = nullptr;
         int64_t launches = 0;  // kernels per launch outside the rebuild body
+        int64_t evals = 0;     // force evaluations (pair-force launches) per launch
         GraphKey key = {};
         void drop() {
             if (exec) cudaGraphExecDestroy(exec);
@@ -2271,8 +2391,7 @@ class Engine : public EngineBase {
             if (cudaGraphAddNode(&wnode, g.graph, nullptr, 0, &cp) != cudaSuccess) return fail();
             into = cp.conditional.phGraph_out[0];
         }
-        if (path_ == 1 && cudaGraphConditionalHandleCreate(&cap.rebuild, g.graph, 0, cudaGraphCondAssignDefault) != cudaSuccess)
-            return fail();
+        cap.graph = g.graph;  // (the rebuild handles are created as the step reaches its rebuild points: rebuild_handle)
         auto capture_into = [&](cudaGraph_t graph, auto body) {
             cudaGraph_t out = nullptr;
             return cudaStreamBeginCaptureToGraph(stream_, graph, nullptr, nullptr, 0, cudaStreamCaptureModeRelaxed) == cudaSuccess &&
@@ -2280,14 +2399,18 @@ class Engine : public EngineBase {
         };
         if (!capture_into(into, [&] { return enqueue(cap); })) return fail();
         g.launches = launches_ - launches_before;
-        if (path_ == 1 && !(cap.body && capture_into(cap.body, [&] { return enqueue_rebuild(true, false); }))) return fail();
+        g.evals = n_force_evals_ - evals_before;
+        // (a LangevinSplitting step whose splitting has no A moves no atom and has no rebuild node)
+        for (cudaGraph_t body : cap.body)
+            if (!capture_into(body, [&] { return enqueue_rebuild(true, false); })) return fail();
         if (cudaGraphInstantiate(&g.exec, g.graph, 0) != cudaSuccess) return fail();
         launches_ = launches_before;
         return MB_OK;
     }
     // One MD step (K1, [IF rebuild], force, K2, [thermostat], [log records]; Langevin: L, [IF rebuild], force,
     // [log records]; Nose-Hoover: NH1, [IF rebuild], force, NH2, [log records]; multiple time steps: the unrolled substeps
-    // of enqueue_mts_step, [log records]) as an executable graph.
+    // of enqueue_mts_step, [log records]; LangevinSplitting: the passes of enqueue_split_step, [log records]) as an
+    // executable graph.
     int build_step_graph(const StepCfg& c, const GraphKey& key) {
         StepOpts o;
         o.do_cm = c.do_cm;
@@ -2394,9 +2517,9 @@ class Engine : public EngineBase {
     // The refusals of a simulate call, made before any work; each names the call's C entry point
     int check_simulate(const void* coords, const void* vels, const Integrator& ig) {
         static const char* const entry[] = {"mb_simulate_vv", "mb_simulate_langevin", "mb_simulate_nose_hoover", "mb_simulate_mts",
-                                            "mb_simulate_mts"};
+                                            "mb_simulate_mts", "mb_simulate_langevin_splitting"};
         static const char* const name[] = {"VelocityVerlet", "Langevin", "Nose-Hoover", "the multiple-time-step integrators",
-                                           "the multiple-time-step integrators"};
+                                           "the multiple-time-step integrators", "LangevinSplitting"};
         if (!coords || !vels) return set_error(MB_ERR_INVALID, "null argument");
         if (ig.n_steps < 0 || !(ig.dt > 0)) return set_error(MB_ERR_INVALID, "n_steps < 0 or dt <= 0");
         const std::string who = std::string(entry[ig.kind]) + ": ";
@@ -2414,7 +2537,14 @@ class Engine : public EngineBase {
                 return set_error(MB_ERR_INVALID, who + "a specific interaction sits at level " + std::to_string(max_specific_level()) +
                                                      " of " + std::to_string(ig.n_levels) + " (mb_set_specific_levels)");
         }
-        if (ig.kind == INTEG_LANGEVIN || ig.kind == INTEG_MTS_LANGEVIN) {
+        if (ig.kind == INTEG_SPLIT) {
+            if (ig.n_ops < 1 || ig.n_ops > MB_SPLIT_MAX_OPS)
+                return set_error(MB_ERR_INVALID, who + "the splitting must have 1 .. MB_SPLIT_MAX_OPS letters");
+            for (int k = 0; k < ig.n_ops; k++)
+                if (ig.ops[k] != 'A' && ig.ops[k] != 'B' && ig.ops[k] != 'O')
+                    return set_error(MB_ERR_INVALID, who + "splitting must contain only A, B, and O steps");
+        }
+        if (ig.kind == INTEG_LANGEVIN || ig.kind == INTEG_MTS_LANGEVIN || ig.kind == INTEG_SPLIT) {
             if (!(std::isfinite(ig.kT) && ig.kT >= 0)) return set_error(MB_ERR_INVALID, who + "kT must be finite and >= 0");
             if (!(std::isfinite(ig.friction) && ig.friction >= 0)) return set_error(MB_ERR_INVALID, who + "friction must be finite and >= 0");
         }
@@ -2556,7 +2686,7 @@ class Engine : public EngineBase {
                 const int m = log_mask_at(log, ig.init_step + k);
                 MB_CUDA(cudaGraphLaunch(graphs_[m].exec, stream_));
                 launches_ += graphs_[m].launches;  // rebuild-body kernels are not counted
-                n_force_evals_ += (m & LOG_ENERGY) ? 2 : 1;
+                n_force_evals_ += graphs_[m].evals;
                 MB_TRY(log_step(lr, m));
             }
             n_steps_ += ig.n_steps;
@@ -2635,7 +2765,7 @@ class Engine : public EngineBase {
         sd_trial_kernel<T><<<nb, SD_THREADS, 0, stream_>>>((int)n_, path_ == 1 ? d_orig_.as<int>() : nullptr, d_sd_f_.as<T4>(),
                                                            d_pos4_.as<T4>(), d_sd_x_.as<T4>(), d_xref4_.as<T4>(),
                                                            path_ == 1 ? g_.skin_half2 : (T)0, ext_map(), d_ctl_.as<Control>(),
-                                                           d_sd_st_.as<SdState>(), cap ? cap->rebuild : 0, cap && path_ == 1 ? 1 : 0);
+                                                           d_sd_st_.as<SdState>(), rebuild_handle(cap), cap && path_ == 1 ? 1 : 0);
         launches_++;
         MB_TRY(after_drift(cap, true));  // (the exact displacement trigger whatever rebuild_every says)
         return enqueue_sd_eval(false, cap);
@@ -3104,6 +3234,16 @@ int mb_simulate_mts(mb_ctx* ctx, void* coords, void* vels, const mb_mts_params_t
         ig.kT = p->kT;
         ig.friction = p->friction;
     }
+    return ctx->e->simulate(coords, vels, ig, log);
+}
+int mb_simulate_langevin_splitting(mb_ctx* ctx, void* coords, void* vels, const mb_splitting_params_t* p, mb_log_t* log) {
+    MB_CTX_GUARD(ctx);
+    if (!p) return mb::set_error(MB_ERR_INVALID, "null argument");
+    mb::Integrator ig = integrator_call(mb::INTEG_SPLIT, p, p->rng_ctr1, p->rng_key);
+    ig.kT = p->kT;
+    ig.friction = p->friction;
+    ig.n_ops = p->n_ops;
+    std::copy_n(p->ops, std::clamp(p->n_ops, 0, MB_SPLIT_MAX_OPS), ig.ops.begin());
     return ctx->e->simulate(coords, vels, ig, log);
 }
 int mb_minimize_sd(mb_ctx* ctx, void* coords, mb_sd_params_t* p) { MB_CTX_GUARD(ctx); return ctx->e->minimize_sd(coords, p); }

@@ -166,14 +166,21 @@ __device__ __forceinline__ void andersen_apply(typename VT<T>::T4& v, int orig_i
 
 // The step bookkeeping of a drift pass (K1, the Langevin step), done by one thread of the last CTA to finish: advance step_n,
 // apply the fixed-interval neighbour policy (find_neighbors every n_steps, src/neighbors.jl:671) and publish the rebuild
-// decision to the CUDA graph's conditional node (when the step runs as a graph).
-__device__ __forceinline__ void step_advance(Control* __restrict__ ctl, cudaGraphConditionalHandle handle, int use_handle) {
+// decision to the CUDA graph's conditional node (when the step runs as a graph). The two halves are separate for
+// LangevinSplitting, whose passes may publish a decision without advancing the step or advance it without a rebuild node.
+__device__ __forceinline__ int step_count(Control* __restrict__ ctl) {  // returns the rebuild decision
     __threadfence();
     const long long step_n = ++ctl->step;
     const long long kk = step_n - ctl->init_step;
     int rb = *(volatile int*)&ctl->rebuild;
     if (ctl->rebuild_every > 0 && kk > 1 && (step_n - 1) % ctl->rebuild_every == 0) { rb = 1; ctl->rebuild = 1; }
+    return rb;
+}
+__device__ __forceinline__ void publish_rebuild(cudaGraphConditionalHandle handle, int use_handle, int rb) {
     if (use_handle) cudaGraphSetConditional(handle, rb ? 1u : 0u);
+}
+__device__ __forceinline__ void step_advance(Control* __restrict__ ctl, cudaGraphConditionalHandle handle, int use_handle) {
+    publish_rebuild(handle, use_handle, step_count(ctl));
 }
 
 // ---- K1: first half kick + drift + displacement check; the last CTA to finish does the step bookkeeping (step_advance).
