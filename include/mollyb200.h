@@ -138,12 +138,36 @@ int mb_energy(mb_ctx* ctx, const void* coords, void* pe, int64_t step_n);
 int mb_forces_energy(mb_ctx* ctx, const void* coords, void* fs_mat, void* pe, void* virial,
                      int64_t step_n);
 
-/* Specific (bonded) interaction lists, SURVEY.md §8(f)-1: InteractionList{2,3,4}Atoms (src/types.jl:89-157) with
- * HarmonicBond (kind 0; params k, r0), HarmonicAngle (kind 1; k, theta0), PeriodicTorsion (kind 2; one
- * (periodicity, phase, k) term per entry — a torsion with several terms is listed several times; impropers are the
- * same struct, src/interactions/periodic_torsion.jl:17-142). atom_idx: n_terms x (kind + 2), 1-based; params: double,
- * n_terms x 2 or 3. Host pointers. They are evaluated inside mb_simulate_vv (specific_forces_gpu!, src/force.jl:1231)
- * and by mb_forces_energy_all; mb_forces / mb_energy stay pairwise-only (the pairwise_*_loop_gpu! seam). */
+/* Specific (bonded) interaction lists, SURVEY.md §8(f)-1: InteractionList{1,2,3,4}Atoms (src/types.jl:89-157) of one
+ * element type per kind. atom_idx: n_terms x atoms, 1-based; params: double, n_terms x params, per term in this order:
+ *
+ *   kind                              atoms  params                    reference (src/interactions/)
+ *   0 MB_SPECIFIC_HARMONIC_BOND       2      k, r0                     harmonic_bond.jl
+ *   1 MB_SPECIFIC_HARMONIC_ANGLE      3      k, theta0                 harmonic_angle.jl
+ *   2 MB_SPECIFIC_PERIODIC_TORSION    4      periodicity, phase, k     periodic_torsion.jl
+ *   3 MB_SPECIFIC_POSITION_RESTRAINT  1      k, x0, y0, z0             harmonic_position_restraint.jl
+ *   4 MB_SPECIFIC_MORSE_BOND          2      D, a, r0                  morse_bond.jl
+ *   5 MB_SPECIFIC_FENE_BOND           2      k, r0, sigma, eps         fene_bond.jl
+ *   6 MB_SPECIFIC_COSINE_ANGLE        3      k, theta0                 cosine_angle.jl
+ *   7 MB_SPECIFIC_UREY_BRADLEY        3      kangle, theta0, kbond, r0 urey_bradley.jl
+ *   8 MB_SPECIFIC_HARMONIC_TORSION    4      k, theta0                 harmonic_torsion.jl
+ *   9 MB_SPECIFIC_RB_TORSION          4      f1, f2, f3, f4            rb_torsion.jl
+ *
+ * PeriodicTorsion has one (periodicity, phase, k) term per entry: a torsion with several terms is listed several times;
+ * impropers are the same struct (periodic_torsion.jl:17-142). Angles are in radians. Each call replaces every term of
+ * its kind: concatenate the lists of one kind (e.g. propers and impropers) into one call. Host pointers. A kind outside
+ * 0 .. MB_SPECIFIC_N_KINDS - 1 or an index outside 1 .. n is refused with MB_ERR_INVALID. The terms are evaluated inside
+ * every mb_simulate_* call, the loggers and mb_minimize_sd (specific_forces_gpu!, src/force.jl:1231) and by
+ * mb_forces_energy_all; mb_forces / mb_energy stay pairwise-only (the pairwise_*_loop_gpu! seam).
+ * Where the engine differs from the reference:
+ *  - RBTorsion: the force is -grad E of the reference's own energy, (f1 (1 + cos th) + f2 (1 - cos 2th) + f3 (1 + cos 3th)
+ *    + f4) / 2. rb_torsion.jl:30 uses dE/dth = (f1 sin th - 2 f2 sin 2th + 3 f3 sin 3th) / 2, which is minus that
+ *    derivative, so its forces push up the energy; the magnitudes agree, the directions are reversed.
+ *  - A torsion with three collinear atoms (a cross product of exactly zero) gets no force, for all three torsion kinds;
+ *    the reference divides by zero there. */
+enum { MB_SPECIFIC_HARMONIC_BOND = 0, MB_SPECIFIC_HARMONIC_ANGLE = 1, MB_SPECIFIC_PERIODIC_TORSION = 2,
+       MB_SPECIFIC_POSITION_RESTRAINT = 3, MB_SPECIFIC_MORSE_BOND = 4, MB_SPECIFIC_FENE_BOND = 5, MB_SPECIFIC_COSINE_ANGLE = 6,
+       MB_SPECIFIC_UREY_BRADLEY = 7, MB_SPECIFIC_HARMONIC_TORSION = 8, MB_SPECIFIC_RB_TORSION = 9, MB_SPECIFIC_N_KINDS = 10 };
 int mb_set_specific(mb_ctx* ctx, int kind, int64_t n_terms, const int32_t* atom_idx, const double* params);
 /* The multiple-time-step level of every term of one kind (mb_simulate_mts): level[t] of the t-th term as mb_set_specific
  * received it, a 0-based index into the integrator's ordered fractions, 0 <= level < MB_MTS_MAX_LEVELS. n_terms must equal

@@ -293,42 +293,67 @@ function Molly.pairwise_pe_loop_gpu!(pe_vec_nounits, buffers, sys::System{3, <:C
 end
 
 # ---- specific (bonded) interaction lists -> mb_set_specific ----------------------------------------------
-# InteractionList{2,3,4}Atoms of HarmonicBond / HarmonicAngle / PeriodicTorsion (src/types.jl:89-157). Anything else
-# makes simulate! fall through to the stock path. A torsion with several Fourier terms becomes one entry per term
-# (zero-k padding terms are dropped), like src/interactions/periodic_torsion.jl:100-142 sums them.
-function specific_desc(sil::InteractionList2Atoms)
+# InteractionList{1,2,3,4}Atoms (src/types.jl:89-157) whose element type is one of the engine's kinds (MB_SPECIFIC_* in
+# include/mollyb200.h). Anything else makes simulate! fall through to the stock path. A PeriodicTorsion with several
+# Fourier terms becomes one entry per term (zero-k padding terms are dropped), like src/interactions/periodic_torsion.jl:100-142
+# sums them. Units are stripped: the engine works in nm, kJ/mol and radians.
+specific_kind(::Type) = nothing
+specific_kind(::Type{<:HarmonicBond}) = 0
+specific_kind(::Type{<:HarmonicAngle}) = 1
+specific_kind(::Type{<:HarmonicPositionRestraint}) = 3
+specific_kind(::Type{<:MorseBond}) = 4
+specific_kind(::Type{<:FENEBond}) = 5
+specific_kind(::Type{<:CosineAngle}) = 6
+specific_kind(::Type{<:UreyBradley}) = 7
+specific_kind(::Type{<:HarmonicTorsion}) = 8
+specific_kind(::Type{<:RBTorsion}) = 9
+# the parameters of one term in mb_set_specific's order
+specific_params(b::HarmonicBond) = (b.k, b.r0)
+specific_params(a::HarmonicAngle) = (a.k, a.θ0)
+specific_params(r::HarmonicPositionRestraint) = (r.k, r.x0...)
+specific_params(b::MorseBond) = (b.D, b.a, b.r0)
+specific_params(b::FENEBond) = (b.k, b.r0, b.σ, b.ϵ)
+specific_params(a::CosineAngle) = (a.k, a.θ0)
+specific_params(a::UreyBradley) = (a.kangle, a.θ0, a.kbond, a.r0)
+specific_params(t::HarmonicTorsion) = (t.k, t.θ0)
+specific_params(t::RBTorsion) = (t.f1, t.f2, t.f3, t.f4)
+
+atom_columns(sil::InteractionList1Atoms) = (sil.is,)
+atom_columns(sil::InteractionList2Atoms) = (sil.is, sil.js)
+atom_columns(sil::InteractionList3Atoms) = (sil.is, sil.js, sil.ks)
+atom_columns(sil::InteractionList4Atoms) = (sil.is, sil.js, sil.ks, sil.ls)
+
+# (kind, atom indices atoms x n (1-based, column = one term), params n_params x n), or nothing
+function specific_desc(sil::Union{InteractionList1Atoms, InteractionList2Atoms, InteractionList3Atoms, InteractionList4Atoms})
     inters = Array(sil.inters)
-    eltype(inters) <: HarmonicBond || return nothing
-    idx = Int32.(vcat(Array(sil.is)', Array(sil.js)'))                       # 2 x n, 1-based, column = one term
-    par = Float64.(vcat([ustrip(b.k) for b in inters]', [ustrip(b.r0) for b in inters]'))
-    return (0, idx, par)
-end
-function specific_desc(sil::InteractionList3Atoms)
-    inters = Array(sil.inters)
-    eltype(inters) <: HarmonicAngle || return nothing
-    idx = Int32.(vcat(Array(sil.is)', Array(sil.js)', Array(sil.ks)'))
-    par = Float64.(vcat([ustrip(a.k) for a in inters]', [ustrip(a.θ0) for a in inters]'))
-    return (1, idx, par)
-end
-function specific_desc(sil::InteractionList4Atoms)
-    inters = Array(sil.inters)
-    eltype(inters) <: PeriodicTorsion || return nothing
-    is, js, ks, ls = Array(sil.is), Array(sil.js), Array(sil.ks), Array(sil.ls)
-    idx, par = Int32[], Float64[]
-    for (t, tor) in enumerate(inters), m in eachindex(tor.periodicities)
-        k = Float64(ustrip(tor.ks[m]))
-        k == 0 && continue
-        append!(idx, (is[t], js[t], ks[t], ls[t]))
-        append!(par, (Float64(tor.periodicities[m]), Float64(ustrip(tor.phases[m])), k))
+    cols = map(Array, atom_columns(sil))
+    if sil isa InteractionList4Atoms && eltype(inters) <: PeriodicTorsion
+        idx, par = Int32[], Float64[]
+        for (t, tor) in enumerate(inters), m in eachindex(tor.periodicities)
+            k = Float64(ustrip(tor.ks[m]))
+            k == 0 && continue
+            append!(idx, (c[t] for c in cols))
+            append!(par, (Float64(tor.periodicities[m]), Float64(ustrip(tor.phases[m])), k))
+        end
+        return (2, reshape(idx, 4, :), reshape(par, 3, :))
     end
-    return (2, reshape(idx, 4, :), reshape(par, 3, :))
+    kind = specific_kind(eltype(inters))
+    isnothing(kind) && return nothing
+    idx = Int32[c[t] for t in eachindex(inters) for c in cols]
+    par = Float64[ustrip(p) for b in inters for p in specific_params(b)]
+    return (kind, reshape(idx, length(cols), :), reshape(par, :, length(inters)))
 end
 specific_desc(::Any) = nothing
 
+# The engine holds one array per kind and each mb_set_specific call replaces it, so the lists of one kind (e.g. an Amber
+# system's proper and improper PeriodicTorsion lists) are concatenated in list order, as the Python System does.
 function set_specific!(ctx::Context, sys)
-    descs = map(specific_desc, sys.specific_inter_lists)
+    descs = collect(map(specific_desc, sys.specific_inter_lists))
     any(isnothing, descs) && return false
-    for (kind, idx, par) in descs     # at most one list per kind (the engine replaces a kind's list on every call)
+    for kind in unique(first.(descs))
+        mine = filter(d -> d[1] == kind, descs)
+        idx = reduce(hcat, [d[2] for d in mine])
+        par = reduce(hcat, [d[3] for d in mine])
         check(ccall((:mb_set_specific, LIB), Cint, (Ptr{Cvoid}, Cint, Int64, Ptr{Int32}, Ptr{Float64}),
                     ctx.handle, kind, size(idx, 2), idx, par))
     end
@@ -598,12 +623,15 @@ end
 # ---- simulate!(sys, ::MTSIntegrator / ::MTSLangevinIntegrator, n) (src/simulators.jl:1616-1940) ------------------------------
 # Taken over under the conditions of the Langevin method above, when every pairwise fraction is 1 (the engine evaluates all
 # pairwise interactions in one kernel, once per outer step): one mb_simulate_mts call. The level of every specific term is
-# the index of its list's fraction in ordered_fractions, set for each list right after set_specific! set its terms (same
-# loop order, so the levels follow the list each kind ends up with). Anything else runs the stock method.
+# the index of its list's fraction in ordered_fractions; the levels of one kind are concatenated in list order, the order in
+# which set_specific! concatenated the terms. Anything else runs the stock method.
 function set_specific_levels!(ctx::Context, sys, sim)
+    levels = Dict{Int, Vector{Int32}}()
     for (sil, f) in zip(sys.specific_inter_lists, sim.si_fractions)
         kind, idx, _ = specific_desc(sil)
-        level = fill(Int32(findfirst(==(f), sim.ordered_fractions) - 1), size(idx, 2))
+        append!(get!(levels, kind, Int32[]), fill(Int32(findfirst(==(f), sim.ordered_fractions) - 1), size(idx, 2)))
+    end
+    for (kind, level) in levels
         check(ccall((:mb_set_specific_levels, LIB), Cint, (Ptr{Cvoid}, Cint, Int64, Ptr{Int32}),
                     ctx.handle, kind, length(level), level))
     end

@@ -17,4 +17,5 @@ from .api import (Atom, CubicBoundary, TriclinicBoundary, System, NoCutoff, Dist
                   comm_unique_id, comm_init, decomp_plan, InteractionList2Atoms, InteractionList3Atoms,
                   InteractionList4Atoms, PotentialEnergyLogger, KineticEnergyLogger, TotalEnergyLogger, TemperatureLogger,
                   CoordinatesLogger, VelocitiesLogger, values, record_steps, SteepestDescentMinimizer, steepest_descent,
-                  sd_log_lines, ImplicitSolventOBC, ImplicitSolventGBN2)
+                  sd_log_lines, ImplicitSolventOBC, ImplicitSolventGBN2, InteractionList1Atoms, MorseBonds, FENEBonds,
+                  CosineAngles, UreyBradleys, HarmonicTorsions, RBTorsions, add_position_restraints)

@@ -26,6 +26,10 @@ EXPORTED = [
     "mb_simulate_langevin_splitting",
 ]
 MB_GB_MAX_NECK_CLASSES = 32
+# specific interaction kinds of mb_set_specific (include/mollyb200.h)
+(MB_SPECIFIC_HARMONIC_BOND, MB_SPECIFIC_HARMONIC_ANGLE, MB_SPECIFIC_PERIODIC_TORSION, MB_SPECIFIC_POSITION_RESTRAINT,
+ MB_SPECIFIC_MORSE_BOND, MB_SPECIFIC_FENE_BOND, MB_SPECIFIC_COSINE_ANGLE, MB_SPECIFIC_UREY_BRADLEY, MB_SPECIFIC_HARMONIC_TORSION,
+ MB_SPECIFIC_RB_TORSION, MB_SPECIFIC_N_KINDS) = range(11)
 MB_MTS_MAX_LEVELS = 8
 MB_SPLIT_MAX_OPS = 32
 

@@ -435,6 +435,153 @@ class InteractionList4Atoms:
         return np.ascontiguousarray(idx), np.ascontiguousarray(par)
 
 
+def _list_arrays(idx_cols, par_cols):
+    idx = np.stack([np.asarray(c).reshape(-1) for c in idx_cols], 1).astype(np.int32)
+    par = np.stack([np.broadcast_to(np.asarray(c, np.float64), (len(idx),)) for c in par_cols], 1)
+    return np.ascontiguousarray(idx), np.ascontiguousarray(par)
+
+
+@dataclass
+class InteractionList1Atoms:
+    """InteractionList1Atoms of HarmonicPositionRestraint (interactions/harmonic_position_restraint.jl): 1-based is_,
+    per-term k (kJ mol^-1 nm^-2) and restraint position x0 (n x 3, nm). The displacement to x0 is minimum-image."""
+    is_: object
+    k: object
+    x0: object
+    kind = capi.MB_SPECIFIC_POSITION_RESTRAINT
+
+    def arrays(self):
+        x0 = np.asarray(self.x0, np.float64).reshape(-1, 3)
+        return _list_arrays([self.is_], [self.k, x0[:, 0], x0[:, 1], x0[:, 2]])
+
+
+@dataclass
+class MorseBonds:
+    """InteractionList2Atoms of MorseBond (interactions/morse_bond.jl): V = D (1 - exp(-a (r - r0)))^2."""
+    is_: object
+    js: object
+    D: object
+    a: object
+    r0: object
+    kind = capi.MB_SPECIFIC_MORSE_BOND
+
+    def arrays(self):
+        return _list_arrays([self.is_, self.js], [self.D, self.a, self.r0])
+
+
+@dataclass
+class FENEBonds:
+    """InteractionList2Atoms of FENEBond (interactions/fene_bond.jl): V = -k r0^2 / 2 ln(1 - (r / r0)^2) plus WCA(sigma,
+    eps) for r < 2^(1/6) sigma. Undefined (NaN) for r >= r0, as in the reference."""
+    is_: object
+    js: object
+    k: object
+    r0: object
+    sigma: object
+    eps: object
+    kind = capi.MB_SPECIFIC_FENE_BOND
+
+    def arrays(self):
+        return _list_arrays([self.is_, self.js], [self.k, self.r0, self.sigma, self.eps])
+
+
+@dataclass
+class CosineAngles:
+    """InteractionList3Atoms of CosineAngle (interactions/cosine_angle.jl): V = k (1 + cos(theta - theta0)), j in the
+    middle, theta0 in radians."""
+    is_: object
+    js: object
+    ks: object
+    k: object
+    theta0: object
+    kind = capi.MB_SPECIFIC_COSINE_ANGLE
+
+    def arrays(self):
+        return _list_arrays([self.is_, self.js, self.ks], [self.k, self.theta0])
+
+
+@dataclass
+class UreyBradleys:
+    """InteractionList3Atoms of UreyBradley (interactions/urey_bradley.jl): a harmonic angle (kangle, theta0) plus a
+    harmonic bond (kbond, r0) between the outer atoms i and k."""
+    is_: object
+    js: object
+    ks: object
+    kangle: object
+    theta0: object
+    kbond: object
+    r0: object
+    kind = capi.MB_SPECIFIC_UREY_BRADLEY
+
+    def arrays(self):
+        return _list_arrays([self.is_, self.js, self.ks], [self.kangle, self.theta0, self.kbond, self.r0])
+
+
+@dataclass
+class HarmonicTorsions:
+    """InteractionList4Atoms of HarmonicTorsion (interactions/harmonic_torsion.jl): V = k (theta - theta0)^2, with
+    theta - theta0 not wrapped, as in the reference."""
+    is_: object
+    js: object
+    ks: object
+    ls: object
+    k: object
+    theta0: object
+    kind = capi.MB_SPECIFIC_HARMONIC_TORSION
+
+    def arrays(self):
+        return _list_arrays([self.is_, self.js, self.ks, self.ls], [self.k, self.theta0])
+
+
+@dataclass
+class RBTorsions:
+    """InteractionList4Atoms of RBTorsion (interactions/rb_torsion.jl): V = (f1 (1 + cos th) + f2 (1 - cos 2th) +
+    f3 (1 + cos 3th) + f4) / 2. The forces are -grad V; the reference's have the opposite sign (include/mollyb200.h)."""
+    is_: object
+    js: object
+    ks: object
+    ls: object
+    f1: object
+    f2: object
+    f3: object
+    f4: object
+    kind = capi.MB_SPECIFIC_RB_TORSION
+
+    def arrays(self):
+        return _list_arrays([self.is_, self.js, self.ks, self.ls], [self.f1, self.f2, self.f3, self.f4])
+
+
+def add_position_restraints(sys, k, atom_selector=None, restrain_coords=None):
+    """add_position_restraints (src/setup.jl:2059-2100): a System like `sys` with one more specific interaction list, a
+    HarmonicPositionRestraint on every selected atom. k: scalar or one value per atom of the system (kJ mol^-1 nm^-2);
+    atom_selector: boolean mask over the atoms or 1-based indices, None for every atom; restrain_coords: n x 3, by default
+    a copy of the current coordinates."""
+    n = sys.n
+    k_arr = np.asarray(k, np.float64)
+    if k_arr.ndim > 0 and len(k_arr) != n:
+        raise ValueError(f"the system has {n} atoms but there are {len(k_arr)} k values")
+    k_arr = np.broadcast_to(k_arr, (n,))
+    if restrain_coords is None:
+        restrain_coords = sys.coords.cpu().numpy() if hasattr(sys.coords, "data_ptr") else sys.coords
+    x0 = np.array(restrain_coords, np.float64).reshape(n, 3)
+    if atom_selector is None:
+        sel = np.arange(n)
+    else:
+        a = np.asarray(atom_selector)
+        sel = np.flatnonzero(a) if a.dtype == bool else a.astype(np.int64).reshape(-1) - 1
+        if a.dtype == bool and len(a) != n:
+            raise ValueError(f"atom_selector has {len(a)} entries for {n} atoms")
+        if len(sel) and (sel.min() < 0 or sel.max() >= n):
+            raise ValueError("atom_selector: an index outside 1 .. n")
+    restraints = InteractionList1Atoms(sel + 1, k_arr[sel].copy(), x0[sel])
+    def copy(a):
+        return a.clone() if hasattr(a, "data_ptr") else np.array(a)
+    return System(atoms=sys.atoms.copy(), coords=copy(sys.coords), boundary=sys.boundary, velocities=copy(sys.velocities),
+                  pairwise_inters=sys.pairwise_inters, neighbor_finder=sys.neighbor_finder, dtype=sys.dtype, device=sys.device,
+                  k=sys.k, specific_inter_lists=sys.specific_inter_lists + (restraints,), general_inters=sys.general_inters,
+                  loggers=sys.loggers)
+
+
 @dataclass
 class AndersenThermostat:
     temperature: float

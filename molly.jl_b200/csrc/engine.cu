@@ -954,15 +954,16 @@ class Engine : public EngineBase {
         return MB_OK;
     }
 
-    // ---- specific (bonded) interaction lists: kind 0 bond (k, r0), 1 angle (k, theta0), 2 torsion (periodicity, phase, k)
+    // ---- specific (bonded) interaction lists: kind MB_SPECIFIC_*, SPECIFIC_ATOMS / SPECIFIC_PARAMS per term (bonded.cuh)
     int set_specific(int kind, int64_t n, const int32_t* idx, const double* par) override {
-        if (kind < 0 || kind > 2 || n < 0 || (n > 0 && (!idx || !par))) return set_error(MB_ERR_INVALID, "mb_set_specific: bad arguments");
+        if (kind < 0 || kind >= N_SPECIFIC_KINDS || n < 0 || (n > 0 && (!idx || !par)))
+            return set_error(MB_ERR_INVALID, "mb_set_specific: bad arguments");
         if (n_ <= 0) return set_error(MB_ERR_STATE, "mb_set_specific: set atoms first");
-        const int na = kind + 2, np_ = (kind == 2) ? 3 : 2;
+        const int na = SPECIFIC_ATOMS[kind], np_ = SPECIFIC_PARAMS[kind];
         std::vector<int> hidx((size_t)n * na);
         std::vector<T> hpar((size_t)n * np_);
         for (int64_t t = 0; t < n * na; t++) {
-            int a = idx[t] - 1;  // 1-based in, like InteractionList{2,3,4}Atoms (src/types.jl:89-157)
+            int a = idx[t] - 1;  // 1-based in, like InteractionList{1,2,3,4}Atoms (src/types.jl:89-157)
             if (a < 0 || a >= n_) return set_error(MB_ERR_INVALID, "mb_set_specific: atom index out of bounds");
             hidx[t] = a;
         }
@@ -978,15 +979,17 @@ class Engine : public EngineBase {
         h_sp_par_[kind] = std::move(hpar);
         h_sp_level_[kind].assign(n, 0);
         for (int l = 0; l <= MTS_MAX_LEVELS; l++) sp_lvl_off_[kind][l] = (l == 0) ? 0 : n;
-        int64_t mx = std::max(sp_n_[0], std::max(sp_n_[1], sp_n_[2]));
-        MB_CUDA(d_sp_partial_.ensure((size_t)(3 * ((mx + BONDED_THREADS - 1) / BONDED_THREADS) + 8) * sizeof(double)));
+        int64_t blocks = 0;  // one energy partial per CTA of the bonded launch
+        for (int k = 0; k < N_SPECIFIC_KINDS; k++) blocks += (sp_n_[k] + BONDED_THREADS - 1) / BONDED_THREADS;
+        MB_CUDA(d_sp_partial_.ensure((size_t)(blocks + 8) * sizeof(double)));
         drop_graphs();  // the graphs bake the term counts in
         return MB_OK;
     }
     // multiple-time-step levels: the device arrays of a kind hold its terms grouped by level (stable), level l in
     // [sp_lvl_off_[kind][l], sp_lvl_off_[kind][l + 1])
     int set_specific_levels(int kind, int64_t n, const int32_t* level) override {
-        if (kind < 0 || kind > 2 || n < 0 || (n > 0 && !level)) return set_error(MB_ERR_INVALID, "mb_set_specific_levels: bad arguments");
+        if (kind < 0 || kind >= N_SPECIFIC_KINDS || n < 0 || (n > 0 && !level))
+            return set_error(MB_ERR_INVALID, "mb_set_specific_levels: bad arguments");
         if (n != sp_n_[kind])
             return set_error(MB_ERR_INVALID, "mb_set_specific_levels: " + std::to_string(n) + " levels for " + std::to_string(sp_n_[kind]) +
                                                  " terms of kind " + std::to_string(kind) + " (mb_set_specific)");
@@ -994,7 +997,7 @@ class Engine : public EngineBase {
             if (level[t] < 0 || level[t] >= MTS_MAX_LEVELS)
                 return set_error(MB_ERR_INVALID, "mb_set_specific_levels: a level outside 0 .. MB_MTS_MAX_LEVELS - 1");
         if (std::equal(level, level + n, h_sp_level_[kind].begin())) return MB_OK;  // (the captured graphs stay valid)
-        const int na = kind + 2, np_ = (kind == 2) ? 3 : 2;
+        const int na = SPECIFIC_ATOMS[kind], np_ = SPECIFIC_PARAMS[kind];
         std::vector<int64_t> order(n);
         for (int64_t t = 0; t < n; t++) order[t] = t;
         std::stable_sort(order.begin(), order.end(), [&](int64_t a, int64_t b) { return level[a] < level[b]; });
@@ -1015,11 +1018,11 @@ class Engine : public EngineBase {
     // the deepest level any term sits at
     int max_specific_level() const {
         int m = 0;
-        for (int kind = 0; kind < 3; kind++)
+        for (int kind = 0; kind < N_SPECIFIC_KINDS; kind++)
             for (int32_t v : h_sp_level_[kind]) m = std::max(m, (int)v);
         return m;
     }
-    bool has_lists() const { return sp_n_[0] + sp_n_[1] + sp_n_[2] > 0; }
+    bool has_lists() const { return std::any_of(sp_n_, sp_n_ + N_SPECIFIC_KINDS, [](int64_t v) { return v > 0; }); }
     bool has_specific() const { return has_lists() || pme_on_ || gb_on_; }  // everything that is added after the pair kernel
     // the slot of every atom for kernels that index atoms in original order (null: the all-pairs path keeps that order)
     const int* slot_of() const { return path_ == 1 ? d_inv_orig_.as<int>() : nullptr; }
@@ -1038,15 +1041,15 @@ class Engine : public EngineBase {
         }
         double* part = d_sp_partial_.as<double>();
         BondedLists L;
-        int total_blk = 0;
-        for (int kind = 0; kind < 3; kind++) {
+        L.blk0[0] = 0;
+        for (int kind = 0; kind < N_SPECIFIC_KINDS; kind++) {
             const int64_t lo = level < 0 ? 0 : sp_lvl_off_[kind][level], hi = level < 0 ? sp_n_[kind] : sp_lvl_off_[kind][level + 1];
             L.n[kind] = (int)(hi - lo);
-            L.nblk[kind] = (L.n[kind] + BONDED_THREADS - 1) / BONDED_THREADS;
-            L.idx[kind] = d_sp_idx_k_[kind].as<int>() + lo * (kind + 2);
-            L.par[kind] = d_sp_par_k_[kind].as<T>() + lo * (kind == 2 ? 3 : 2);
-            total_blk += L.nblk[kind];
+            L.blk0[kind + 1] = L.blk0[kind] + (L.n[kind] + BONDED_THREADS - 1) / BONDED_THREADS;
+            L.idx[kind] = d_sp_idx_k_[kind].as<int>() + lo * SPECIFIC_ATOMS[kind];
+            L.par[kind] = d_sp_par_k_[kind].as<T>() + lo * SPECIFIC_PARAMS[kind];
         }
+        const int total_blk = L.blk0[N_SPECIFIC_KINDS];
         if (total_blk > 0) {
             auto go = [&](auto box) {
                 with_const<true, false>(energy, [&](auto EN) {
@@ -3029,13 +3032,13 @@ class Engine : public EngineBase {
     PeerWait gate_ = {};
     unsigned long long cm_deferred_epoch_ = 0;
     int plan_key_[3] = {-1, -1, -1};
-    int64_t sp_n_[3] = {0, 0, 0};
-    DevBuf d_sp_idx_k_[3], d_sp_par_k_[3], d_sp_partial_, d_sp_energy_;
+    int64_t sp_n_[N_SPECIFIC_KINDS] = {};
+    DevBuf d_sp_idx_k_[N_SPECIFIC_KINDS], d_sp_par_k_[N_SPECIFIC_KINDS], d_sp_partial_, d_sp_energy_;
     // the terms as mb_set_specific received them, their multiple-time-step levels, and the level ranges of the device arrays
-    std::vector<int> h_sp_idx_[3];
-    std::vector<T> h_sp_par_[3];
-    std::vector<int32_t> h_sp_level_[3];
-    int64_t sp_lvl_off_[3][MTS_MAX_LEVELS + 1] = {};
+    std::vector<int> h_sp_idx_[N_SPECIFIC_KINDS];
+    std::vector<T> h_sp_par_[N_SPECIFIC_KINDS];
+    std::vector<int32_t> h_sp_level_[N_SPECIFIC_KINDS];
+    int64_t sp_lvl_off_[N_SPECIFIC_KINDS][MTS_MAX_LEVELS + 1] = {};
     DevBuf d_f4_mts_;  // forces of the inner multiple-time-step levels (slot order; fixed address: the step graphs bake it in)
     // PME (pme.cuh)
     bool pme_on_ = false, pme_ready_ = false;
