@@ -1991,7 +1991,6 @@ class Engine : public EngineBase {
         int do_cm = 0;                   // remove_CM_motion after this step's kick
         bool clear_cm_after_k1 = false;  // K1 consumed the pending v_cm and nothing overwrites it this step
         bool rebuild_hint = false;       // a fixed-interval rebuild is due (stream path)
-        bool defer_cm = false;           // decomposed: the next step's K1 sums the slabs' momenta itself
         int log_mask = 0;                // LOG_* records after the step
     };
     // capture mode (capture_graph): the handle of the WHILE loop (if any) and, on the cell-list path, one (handle, body) per
@@ -2056,122 +2055,103 @@ class Engine : public EngineBase {
                                                " doubles overruns the partial-sum buffer");
         return MB_OK;
     }
+    // One step of the call's integrator (single GPU; a decomposed run steps with enqueue_decomposed_step)
     int enqueue_step(const StepCfg& c, const StepOpts& o, Capture* cap = nullptr) {
-        if (is_mts(c.ig.kind)) return enqueue_mts_step(c, o, cap);
-        if (c.ig.kind == INTEG_SPLIT) return enqueue_split_step(c, o, cap);
-        const bool dec = decomposed() && path_ == 1;
-        const int s0 = dec ? own_s0_ : 0, n_own = dec ? own_n_ : (int)n_;
+        switch (c.ig.kind) {
+            case INTEG_LANGEVIN: return enqueue_langevin_step(c, o, cap);
+            case INTEG_NH: return enqueue_nh_step(c, o, cap);
+            case INTEG_MTS:
+            case INTEG_MTS_LANGEVIN: return enqueue_mts_step(c, o, cap);
+            case INTEG_SPLIT: return enqueue_split_step(c, o, cap);
+            default: return enqueue_vv_step(c, o, cap);
+        }
+    }
+    // One VelocityVerlet step: K1 (with the previous step's thermostat, thermo_in_k1), [rebuild], forces, K2, [standalone
+    // Andersen kernel], [log records]
+    int enqueue_vv_step(const StepCfg& c, const StepOpts& o, Capture* cap) {
+        const int n = (int)n_;
         Control* ctl = d_ctl_.as<Control>();
         CmState<T>* cm = d_cm_.as<CmState<T>>();
-        // decomposed run over peer memory (peer.cuh): K1 mirrors the boundary slots into the neighbours while it drifts
-        const unsigned long long epoch = dec ? ++epoch_ : 0ull;
-        const bool p2p_halo = dec && p2p_active() && !o.rebuild_hint;  // rebuild steps all-gather the state instead
-        PeerPush<T> push;
-        memset(&push, 0, sizeof(push));
-        if (p2p_halo) push = make_push(epoch, true);
-        if (cm_deferred_epoch_) {  // the previous step left v_cm in the momentum all-to-all (no peer_cm_kernel)
-            push.cm_comm = comm_of(rank_);
-            push.cm_nranks = nranks_;
-            push.cm_epoch = cm_deferred_epoch_;
-            push.cm_inv_mass = c.inv_mass;
-            cm_deferred_epoch_ = 0;
-        }
         prof_.begin(Prof::VV);
         int grid;
-        if (c.ig.kind == INTEG_LANGEVIN) {  // (single GPU: s0 = 0)
-            MB_TRY(integ_grid(grid, n_own, 1, 8, 3));
-            langevin_step_kernel<T><<<grid, VV_THREADS, 0, stream_>>>(
-                n_own, c.dt, c.dt_half, c.skin_half2, c.lc, o.do_cm, c.inv_mass, cm, d_f4_.as<T4>(), d_xref4_.as<T4>(),
-                d_pos4_.as<T4>(), d_vel4_.as<T4>(), d_orig_.as<int>(), d_mass_.as<T>(), d_partial_.as<double>(), c.flag_ptr, ctl,
-                rebuild_handle(cap), cap && path_ == 1 ? 1 : 0, ext_map());
-        } else if (c.ig.kind == INTEG_NH) {  // (single GPU: s0 = 0)
-            MB_TRY(integ_grid(grid, n_own, 1, 8, 2));
-            nh_kick_drift_kernel<T><<<grid, VV_THREADS, 0, stream_>>>(
-                n_own, c.dt, c.dt_half, c.skin_half2, c.nc, d_nh_.as<NhState>(), cm, d_f4_.as<T4>(), d_xref4_.as<T4>(),
-                d_pos4_.as<T4>(), d_vel4_.as<T4>(), d_mass_.as<T>(), d_partial_.as<double>(), c.flag_ptr, ctl,
-                rebuild_handle(cap), cap && path_ == 1 ? 1 : 0, ext_map());
-        } else {
-            const Thermo<T> th = thermo_in_k1(c);
-            const int thk = th.on ? TH_ANDERSEN : (c.vc.kind != VC_NONE ? TH_SCALE : TH_NONE);
-            MB_TRY(integ_grid(grid, n_own, 2, 5, 0));  // two atoms per thread, one wave (48 registers: 5 CTAs per SM)
-            with_const<TH_NONE, TH_ANDERSEN, TH_SCALE>(thk, [&](auto TH) {
-                vv_kick_drift_kernel<T, TH><<<grid, VV_THREADS, 0, stream_>>>(
-                    s0, n_own, c.dt, c.dt_half, c.skin_half2, cm, d_f4_.as<T4>(), d_xref4_.as<T4>(), d_pos4_.as<T4>(), d_vel4_.as<T4>(),
-                    c.flag_ptr, ctl, rebuild_handle(cap), cap && path_ == 1 ? 1 : 0, push, ext_map(), th);
-            });
-        }
-        prof_.end(Prof::VV);
-        launches_++;
-        if (o.clear_cm_after_k1) {  // (VelocityVerlet: the Langevin step and NH2 clear a consumed v_cm themselves)
-            clear_cm_kernel<T><<<1, 1, 0, stream_>>>(cm);
-            launches_++;
-        }
-        if (dec) {  // (the decomposed step is never captured)
-            if (o.rebuild_hint) {
-                // neighbour rebuild on a decomposed box: replicate positions and velocities, rebuild (identical sort on every
-                // rank, lists only for the owned slab), then refresh the slot ranges and halo segments
-                MB_TRY(allgather_state());
-                MB_TRY(set_flag_rebuild());
-                MB_TRY(enqueue_rebuild(true, false));
-                MB_TRY(update_ownership());
-            } else if (p2p_halo) {
-                gate_ = make_wait(epoch);  // the force kernel's CTAs wait for the neighbours' pushes of this epoch
-            } else {
-                MB_TRY(halo_exchange());
-            }
-        } else {
-            MB_TRY(after_drift(cap, o.rebuild_hint));
-        }
-        const int s0b = dec ? own_s0_ : 0, n_ownb = dec ? own_n_ : (int)n_;  // ownership may have changed in the rebuild
-        const int nb2 = std::max(1, (n_ownb + 255) / 256);
-        MB_TRY(launch_pairs(false, d_f4_.as<T4>(), dec));
-        MB_TRY(launch_bonded(false));
-        if (c.ig.kind == INTEG_LANGEVIN) {  // these forces are the next step's kick: the step ends here
-            if (o.log_mask) MB_TRY(enqueue_log(c, o.log_mask));
-            MB_CUDA(cudaGetLastError());
-            return MB_OK;
-        }
-        if (c.ig.kind == INTEG_NH) {
-            MB_TRY(integ_grid(grid, n_ownb, 1, 8, 3));
-            prof_.begin(Prof::VV);
-            nh_kick2_kernel<T><<<grid, VV_THREADS, 0, stream_>>>(n_ownb, c.dt_half, o.do_cm, c.inv_mass, d_nh_.as<NhState>(),
-                                                                 d_f4_.as<T4>(), d_mass_.as<T>(), d_vel4_.as<T4>(),
-                                                                 d_partial_.as<double>(), ctl, cm);
-            prof_.end(Prof::VV);
-            launches_++;
-            if (o.log_mask) MB_TRY(enqueue_log(c, o.log_mask));
-            MB_CUDA(cudaGetLastError());
-            return MB_OK;
-        }
-        const bool p2p_sig = dec && p2p_active();  // (after a rebuild: the new ownership's peers)
-        PeerSignal sig;
-        memset(&sig, 0, sizeof(sig));
-        if (p2p_sig) sig = make_signal(epoch, o.do_cm != 0);
-        MB_TRY(integ_grid(grid, n_ownb, 2, 8, c.vc.kind != VC_NONE ? 4 : 3));
-        prof_.begin(Prof::VV);
-        with_const<true, false>(c.vc.kind != VC_NONE, [&](auto CP) {
-            vv_kick2_kernel<T, CP><<<grid, VV_THREADS, 0, stream_>>>(s0b, n_ownb, c.dt_half, o.do_cm, c.inv_mass, d_f4_.as<T4>(),
-                                                                     d_mass_.as<T>(), d_vel4_.as<T4>(), d_partial_.as<double>(), ctl, cm,
-                                                                     dec ? d_mom_.as<double>() : nullptr, sig, c.vc);
+        const Thermo<T> th = thermo_in_k1(c);
+        const int thk = th.on ? TH_ANDERSEN : (c.vc.kind != VC_NONE ? TH_SCALE : TH_NONE);
+        MB_TRY(integ_grid(grid, n, 2, 5, 0));  // two atoms per thread, one wave (48 registers: 5 CTAs per SM)
+        with_const<TH_NONE, TH_ANDERSEN, TH_SCALE>(thk, [&](auto TH) {
+            vv_kick_drift_kernel<T, TH><<<grid, VV_THREADS, 0, stream_>>>(
+                0, n, c.dt, c.dt_half, c.skin_half2, cm, d_f4_.as<T4>(), d_xref4_.as<T4>(), d_pos4_.as<T4>(), d_vel4_.as<T4>(),
+                c.flag_ptr, ctl, rebuild_handle(cap), cap && path_ == 1 ? 1 : 0, PeerPush<T>{}, ext_map(), th);
         });
         prof_.end(Prof::VV);
         launches_++;
-        if (p2p_sig && o.do_cm && o.defer_cm && !c.thermostat) {
-            cm_deferred_epoch_ = epoch;  // the next step's K1 adds the slabs' sums itself
-        } else if (p2p_sig && o.do_cm) {
-            // sum(m v) of all slabs arrived by peer stores: add them in rank order
-            peer_cm_kernel<T><<<1, 32, 0, stream_>>>(comm_of(rank_), nranks_, epoch, c.inv_mass, cm);
-            launches_++;
-        } else if (dec && o.do_cm) {
-            // global sum(m v): one 24-byte all-reduce per step, then v_cm for the lazy subtraction
-            MB_NCCL(g_nccl.AllReduce(d_mom_.as<double>(), d_mom_.as<double>() + 4, 3, ncclDouble, ncclSum, comm_, stream_));
-            cm_from_sum_kernel<T><<<1, 1, 0, stream_>>>(d_mom_.as<double>() + 4, c.inv_mass, cm);
+        if (o.clear_cm_after_k1) {
+            clear_cm_kernel<T><<<1, 1, 0, stream_>>>(cm);
             launches_++;
         }
-        if (c.thermostat && !thermo_in_k1(c).on) {
-            andersen_kernel<T><<<nb2, 256, 0, stream_>>>(s0b, n_ownb, (int)n_, c.kT, c.ig.andersen_prob, d_orig_.as<int>(), d_mass_.as<T>(), d_vel4_.as<T4>(), cm, ctl);
+        MB_TRY(after_drift(cap, o.rebuild_hint));
+        MB_TRY(launch_pairs(false, d_f4_.as<T4>()));
+        MB_TRY(launch_bonded(false));
+        MB_TRY(integ_grid(grid, n, 2, 8, c.vc.kind != VC_NONE ? 4 : 3));
+        prof_.begin(Prof::VV);
+        with_const<true, false>(c.vc.kind != VC_NONE, [&](auto CP) {
+            vv_kick2_kernel<T, CP><<<grid, VV_THREADS, 0, stream_>>>(0, n, c.dt_half, o.do_cm, c.inv_mass, d_f4_.as<T4>(), d_mass_.as<T>(),
+                                                                     d_vel4_.as<T4>(), d_partial_.as<double>(), ctl, cm, nullptr,
+                                                                     PeerSignal{}, c.vc);
+        });
+        prof_.end(Prof::VV);
+        launches_++;
+        if (c.thermostat && !th.on) {
+            andersen_kernel<T><<<std::max(1, (n + 255) / 256), 256, 0, stream_>>>(0, n, n, c.kT, c.ig.andersen_prob, d_orig_.as<int>(), d_mass_.as<T>(), d_vel4_.as<T4>(), cm, ctl);
             launches_++;
         }
+        if (o.log_mask) MB_TRY(enqueue_log(c, o.log_mask));
+        MB_CUDA(cudaGetLastError());
+        return MB_OK;
+    }
+    // One Langevin step (langevin.cuh): the fused step kernel, [rebuild], forces, [log records]. The forces are the next
+    // step's kick, and the step kernel clears a consumed v_cm itself.
+    int enqueue_langevin_step(const StepCfg& c, const StepOpts& o, Capture* cap) {
+        const int n = (int)n_;
+        prof_.begin(Prof::VV);
+        int grid;
+        MB_TRY(integ_grid(grid, n, 1, 8, 3));
+        langevin_step_kernel<T><<<grid, VV_THREADS, 0, stream_>>>(
+            n, c.dt, c.dt_half, c.skin_half2, c.lc, o.do_cm, c.inv_mass, d_cm_.as<CmState<T>>(), d_f4_.as<T4>(), d_xref4_.as<T4>(),
+            d_pos4_.as<T4>(), d_vel4_.as<T4>(), d_orig_.as<int>(), d_mass_.as<T>(), d_partial_.as<double>(), c.flag_ptr,
+            d_ctl_.as<Control>(), rebuild_handle(cap), cap && path_ == 1 ? 1 : 0, ext_map());
+        prof_.end(Prof::VV);
+        launches_++;
+        MB_TRY(after_drift(cap, o.rebuild_hint));
+        MB_TRY(launch_pairs(false, d_f4_.as<T4>()));
+        MB_TRY(launch_bonded(false));
+        if (o.log_mask) MB_TRY(enqueue_log(c, o.log_mask));
+        MB_CUDA(cudaGetLastError());
+        return MB_OK;
+    }
+    // One Nose-Hoover step (nosehoover.cuh): NH1, [rebuild], forces, NH2, [log records]. NH2 clears a consumed v_cm itself.
+    int enqueue_nh_step(const StepCfg& c, const StepOpts& o, Capture* cap) {
+        const int n = (int)n_;
+        Control* ctl = d_ctl_.as<Control>();
+        CmState<T>* cm = d_cm_.as<CmState<T>>();
+        prof_.begin(Prof::VV);
+        int grid;
+        MB_TRY(integ_grid(grid, n, 1, 8, 2));
+        nh_kick_drift_kernel<T><<<grid, VV_THREADS, 0, stream_>>>(
+            n, c.dt, c.dt_half, c.skin_half2, c.nc, d_nh_.as<NhState>(), cm, d_f4_.as<T4>(), d_xref4_.as<T4>(),
+            d_pos4_.as<T4>(), d_vel4_.as<T4>(), d_mass_.as<T>(), d_partial_.as<double>(), c.flag_ptr, ctl,
+            rebuild_handle(cap), cap && path_ == 1 ? 1 : 0, ext_map());
+        prof_.end(Prof::VV);
+        launches_++;
+        MB_TRY(after_drift(cap, o.rebuild_hint));
+        MB_TRY(launch_pairs(false, d_f4_.as<T4>()));
+        MB_TRY(launch_bonded(false));
+        MB_TRY(integ_grid(grid, n, 1, 8, 3));
+        prof_.begin(Prof::VV);
+        nh_kick2_kernel<T><<<grid, VV_THREADS, 0, stream_>>>(n, c.dt_half, o.do_cm, c.inv_mass, d_nh_.as<NhState>(),
+                                                             d_f4_.as<T4>(), d_mass_.as<T>(), d_vel4_.as<T4>(),
+                                                             d_partial_.as<double>(), ctl, cm);
+        prof_.end(Prof::VV);
+        launches_++;
         if (o.log_mask) MB_TRY(enqueue_log(c, o.log_mask));
         MB_CUDA(cudaGetLastError());
         return MB_OK;
@@ -2310,7 +2290,9 @@ class Engine : public EngineBase {
         return MB_OK;
     }
     // single-GPU step loop: the thermostat of step n runs at the top of step n+1's drift kernel; the last step of a call is
-    // closed by the standalone kernel (simulate)
+    // closed by the standalone kernel (simulate). The test is the rank count, not simulate's `dec`, so that a multi-rank
+    // context applies the thermostat the same way on both paths: on the all-pairs path it takes the single-GPU step loop, but
+    // runs the standalone kernel after every K2 (enqueue_vv_step) as the decomposed step does.
     Thermo<T> thermo_in_k1(const StepCfg& c) const {
         Thermo<T> th;
         memset(&th, 0, sizeof(th));
@@ -2517,6 +2499,118 @@ class Engine : public EngineBase {
         return MB_OK;
     }
 
+    // One decomposed VelocityVerlet step (cell-list path) over the owned slab. The thermostat runs after K2 (thermo_in_k1),
+    // and velocity couplings are refused (check_simulate). defer_cm: another step of this call follows.
+    int enqueue_decomposed_step(const StepCfg& c, const StepOpts& o, bool defer_cm) {
+        Control* ctl = d_ctl_.as<Control>();
+        CmState<T>* cm = d_cm_.as<CmState<T>>();
+        // decomposed run over peer memory (peer.cuh): K1 mirrors the boundary slots into the neighbours while it drifts
+        const unsigned long long epoch = ++epoch_;
+        const bool p2p_halo = p2p_active() && !o.rebuild_hint;  // rebuild steps all-gather the state instead
+        PeerPush<T> push;
+        memset(&push, 0, sizeof(push));
+        if (p2p_halo) push = make_push(epoch, true);
+        if (cm_deferred_epoch_) {  // the previous step left v_cm in the momentum all-to-all (no peer_cm_kernel)
+            push.cm_comm = comm_of(rank_);
+            push.cm_nranks = nranks_;
+            push.cm_epoch = cm_deferred_epoch_;
+            push.cm_inv_mass = c.inv_mass;
+            cm_deferred_epoch_ = 0;
+        }
+        prof_.begin(Prof::VV);
+        int grid;
+        MB_TRY(integ_grid(grid, own_n_, 2, 5, 0));
+        vv_kick_drift_kernel<T, TH_NONE><<<grid, VV_THREADS, 0, stream_>>>(own_s0_, own_n_, c.dt, c.dt_half, c.skin_half2, cm, d_f4_.as<T4>(),
+                                                                          d_xref4_.as<T4>(), d_pos4_.as<T4>(), d_vel4_.as<T4>(), c.flag_ptr,
+                                                                          ctl, 0, 0, push, ext_map(), thermo_in_k1(c));
+        prof_.end(Prof::VV);
+        launches_++;
+        if (o.clear_cm_after_k1) {
+            clear_cm_kernel<T><<<1, 1, 0, stream_>>>(cm);
+            launches_++;
+        }
+        if (o.rebuild_hint) {
+            // neighbour rebuild on a decomposed box: replicate positions and velocities, rebuild (identical sort on every
+            // rank, lists only for the owned slab), then refresh the slot ranges and halo segments
+            MB_TRY(allgather_state());
+            MB_TRY(set_flag_rebuild());
+            MB_TRY(enqueue_rebuild(true, false));
+            MB_TRY(update_ownership());
+        } else if (p2p_halo) {
+            gate_ = make_wait(epoch);  // the force kernel's CTAs wait for the neighbours' pushes of this epoch
+        } else {
+            MB_TRY(halo_exchange());
+        }
+        MB_TRY(launch_pairs(false, d_f4_.as<T4>(), true));  // (own_*: after a rebuild, the new ownership)
+        MB_TRY(launch_bonded(false));
+        const bool p2p_sig = p2p_active();  // (after a rebuild: the new ownership's peers)
+        PeerSignal sig;
+        memset(&sig, 0, sizeof(sig));
+        if (p2p_sig) sig = make_signal(epoch, o.do_cm != 0);
+        MB_TRY(integ_grid(grid, own_n_, 2, 8, 3));
+        prof_.begin(Prof::VV);
+        vv_kick2_kernel<T, false><<<grid, VV_THREADS, 0, stream_>>>(own_s0_, own_n_, c.dt_half, o.do_cm, c.inv_mass, d_f4_.as<T4>(), d_mass_.as<T>(),
+                                                                    d_vel4_.as<T4>(), d_partial_.as<double>(), ctl, cm, d_mom_.as<double>(),
+                                                                    sig, c.vc);
+        prof_.end(Prof::VV);
+        launches_++;
+        if (p2p_sig && o.do_cm && defer_cm && !c.thermostat) {
+            cm_deferred_epoch_ = epoch;  // the next step's K1 adds the slabs' sums itself
+        } else if (p2p_sig && o.do_cm) {
+            // sum(m v) of all slabs arrived by peer stores: add them in rank order
+            peer_cm_kernel<T><<<1, 32, 0, stream_>>>(comm_of(rank_), nranks_, epoch, c.inv_mass, cm);
+            launches_++;
+        } else if (o.do_cm) {
+            // global sum(m v): one 24-byte all-reduce per step, then v_cm for the lazy subtraction
+            MB_NCCL(g_nccl.AllReduce(d_mom_.as<double>(), d_mom_.as<double>() + 4, 3, ncclDouble, ncclSum, comm_, stream_));
+            cm_from_sum_kernel<T><<<1, 1, 0, stream_>>>(d_mom_.as<double>() + 4, c.inv_mass, cm);
+            launches_++;
+        }
+        if (c.thermostat) {
+            andersen_kernel<T><<<std::max(1, (own_n_ + 255) / 256), 256, 0, stream_>>>(own_s0_, own_n_, (int)n_, c.kT, c.ig.andersen_prob, d_orig_.as<int>(), d_mass_.as<T>(), d_vel4_.as<T4>(), cm, ctl);
+            launches_++;
+        }
+        MB_CUDA(cudaGetLastError());
+        return MB_OK;
+    }
+    // The steps of a decomposed run (never captured: the step issues NCCL calls with per-rebuild sizes), between simulate's
+    // shared prologue and epilogue. Lists cover the owned slab; the fixed rebuild interval is counted on the host (identical
+    // on every rank) and adapted per call from the displacements; every rank returns the whole system.
+    int simulate_decomposed(const StepCfg& c, bool cm_pending) {
+        const Integrator& ig = c.ig;
+        graph_used_ = false;
+        cm_deferred_epoch_ = 0;
+        adapt_span_ = since_rebuild_;
+        // lists built from here on cover only the owned slab
+        build_b0_ = own_b0_;
+        build_nb_ = own_nb_;
+        MB_TRY(p2p_setup());  // collective; falls back to the NCCL transport on every rank if any mapping fails
+        MB_TRY(launch_pairs(false, d_f4_.as<T4>(), true));
+        MB_TRY(launch_bonded(false));
+        const unsigned long long e0 = ++epoch_;  // this force evaluation read the replicated state: tell the pushers
+        if (p2p_active()) {
+            peer_signal_kernel<<<1, 32, 0, stream_>>>(make_signal(e0, false));
+            launches_++;
+        }
+        for (int64_t k = 1; k <= ig.n_steps; k++) {
+            const int64_t step_n = ig.init_step + k;
+            const int do_cm = (ig.remove_cm_every != 0 && step_n % ig.remove_cm_every == 0) ? 1 : 0;
+            StepOpts o;
+            o.do_cm = do_cm;
+            o.clear_cm_after_k1 = cm_pending && !do_cm;  // K1 consumed v_cm; nothing overwrites it this step
+            o.rebuild_hint = since_rebuild_ >= decomposed_interval();
+            since_rebuild_ = o.rebuild_hint ? 1 : since_rebuild_ + 1;
+            adapt_span_ = std::max(adapt_span_, since_rebuild_);
+            MB_TRY(enqueue_decomposed_step(c, o, k < ig.n_steps));
+            cm_pending = (do_cm != 0) && !c.thermostat;  // (the standalone thermostat kernel consumes v_cm)
+            n_steps_++;
+        }
+        MB_TRY(allgather_state());  // every rank returns the whole system
+        build_nb_ = -1;
+        if (rebuild_every_ == 0) MB_TRY(adapt_interval());
+        return MB_OK;
+    }
+
     // The refusals of a simulate call, made before any work; each names the call's C entry point
     int check_simulate(const void* coords, const void* vels, const Integrator& ig) {
         static const char* const entry[] = {"mb_simulate_vv", "mb_simulate_langevin", "mb_simulate_nose_hoover", "mb_simulate_mts",
@@ -2569,14 +2663,16 @@ class Engine : public EngineBase {
                 return set_error(MB_ERR_INVALID, who + "velocity-rescaling thermostats are not available in decomposed (multi-GPU) runs");
         }
         if (decomposed() && gb_on_) return set_error(MB_ERR_INVALID, "implicit solvent is not available in decomposed (multi-GPU) runs");
+        if (decomposed() && path_ == 1 && pme_on_) return set_error(MB_ERR_INVALID, "PME is not available in decomposed (multi-GPU) runs yet");
         return MB_OK;
     }
 
-    // mb_simulate_vv, mb_simulate_vv_log, mb_simulate_langevin, mb_simulate_nose_hoover and mb_simulate_mts: one body, one
-    // step loop, one graph builder
+    // Every mb_simulate_* entry point: one prologue and epilogue; in between, the single-GPU step graphs or stream loop, or
+    // the decomposed steps (simulate_decomposed)
     int simulate(void* coords, void* vels, const Integrator& call, mb_log_t* log) override {
         MB_TRY(prepare());
         MB_TRY(check_simulate(coords, vels, call));
+        const bool dec = decomposed() && path_ == 1;  // a decomposed run: each rank integrates its slab (simulate_decomposed)
         // one level without noise is the VelocityVerlet step: it runs as one (after the refusals, which name mb_simulate_mts)
         Integrator ig = call;
         if (ig.kind == INTEG_MTS && ig.n_levels == 1) {
@@ -2609,13 +2705,13 @@ class Engine : public EngineBase {
         } else {
             MB_TRY(sync_state_from(xb.as<T>(), vb.as<T>()));
             c.skin_half2 = g_.skin_half2;  // geometry is chosen by the first build
-            c.flag_ptr = (rebuild_every_ == 0 && !decomposed()) ? &ctl->rebuild : &ctl->disp;
+            c.flag_ptr = (rebuild_every_ == 0 && !dec) ? &ctl->rebuild : &ctl->disp;
         }
         // step bookkeeping lives on the device (tail of Control)
         {
             struct Tail { int rebuild_every; long long step, init_step; unsigned int rng[4]; unsigned int max_disp2_bits, call_max_disp2_bits; } t;
             static_assert(sizeof(Tail) == sizeof(Control) - offsetof(Control, rebuild_every), "Control tail layout");
-            t.rebuild_every = (decomposed() && path_ == 1) ? 0 : rebuild_every_;  // decomposed: the host counts the interval
+            t.rebuild_every = dec ? 0 : rebuild_every_;  // decomposed: the host counts the interval
             t.step = ig.init_step;
             t.init_step = ig.init_step;
             t.rng[0] = (unsigned int)ig.rng_ctr1; t.rng[1] = (unsigned int)(ig.rng_ctr1 >> 32);
@@ -2626,8 +2722,6 @@ class Engine : public EngineBase {
                                     cudaMemcpyHostToDevice, stream_));
             MB_CUDA(cudaStreamSynchronize(stream_));  // t is a local
         }
-        cm_deferred_epoch_ = 0;
-        adapt_span_ = since_rebuild_;
         bool cm_pending = false;  // host mirror of cm->valid
         if (ig.init_step == 0 && ig.remove_cm_every != 0) {
             // remove_CM_motion! before the first force evaluation (simulators.jl:563): zero-length kick
@@ -2639,95 +2733,67 @@ class Engine : public EngineBase {
             launches_++;
             cm_pending = true;
         }
-        const bool dec = decomposed() && path_ == 1;
-        if (dec && pme_on_) return set_error(MB_ERR_INVALID, "PME is not available in decomposed (multi-GPU) runs yet");
         if (dec) {
-            // lists built from here on cover only the owned slab
-            build_b0_ = own_b0_;
-            build_nb_ = own_nb_;
-            MB_TRY(p2p_setup());  // collective; falls back to the NCCL transport on every rank if any mapping fails
-        }
-        MB_TRY(launch_pairs(false, d_f4_.as<T4>(), dec));
-        MB_TRY(launch_bonded(false, nullptr, is_mts(c.ig.kind) ? 0 : -1));  // (multiple time steps: F_0 of level 0)
-        if (dec) {
-            const unsigned long long e0 = ++epoch_;  // this force evaluation read the replicated state: tell the pushers
-            if (p2p_active()) {
-                peer_signal_kernel<<<1, 32, 0, stream_>>>(make_signal(e0, false));
-                launches_++;
+            MB_TRY(simulate_decomposed(c, cm_pending));
+        } else {
+            MB_TRY(launch_pairs(false, d_f4_.as<T4>()));
+            MB_TRY(launch_bonded(false, nullptr, is_mts(c.ig.kind) ? 0 : -1));  // (multiple time steps: F_0 of level 0)
+            if (log && log->log_initial) {  // apply_loggers! at init_step (run_loggers == true), after F0
+                const int m = log_mask_at(log, ig.init_step);
+                if (m) {
+                    MB_TRY(enqueue_log(c, m));
+                    MB_TRY(log_step(lr, m));
+                }
             }
-        }
-        if (log && log->log_initial) {  // apply_loggers! at init_step (run_loggers == true), after F0
-            const int m = log_mask_at(log, ig.init_step);
-            if (m) {
-                MB_TRY(enqueue_log(c, m));
-                MB_TRY(log_step(lr, m));
-            }
-        }
 
-        // CUDA-graph path: static per-step sequence (remove_CM_motion in {0,1})
-        bool use_graph = graphs_usable() && c.do_cm >= 0 && ig.n_steps >= 4 &&
-                         !dec;  // the decomposed step issues NCCL calls with per-rebuild sizes
-        if (use_graph) {
-            // one executable per log mask this call uses (the plain step and the log steps)
-            bool need[8] = {false, false, false, false, false, false, false, false};
-            for (int64_t k = 1; k <= ig.n_steps; k++) need[log_mask_at(log, ig.init_step + k)] = true;
-            GraphKey key{ig, vcoupling, 0};
-            for (int m = 0; m < 8 && use_graph; m++) {
-                if (!need[m]) continue;
-                key.log_mask = m;
-                if (!graphs_[m].exec || !(key == graphs_[m].key)) {
-                    if (build_step_graph(c, key) != MB_OK) {
-                        graph_failed_ = true;  // stay on the stream path for this context
-                        use_graph = false;
+            // CUDA-graph path: static per-step sequence (remove_CM_motion in {0,1})
+            bool use_graph = graphs_usable() && c.do_cm >= 0 && ig.n_steps >= 4;
+            if (use_graph) {
+                // one executable per log mask this call uses (the plain step and the log steps)
+                bool need[8] = {false, false, false, false, false, false, false, false};
+                for (int64_t k = 1; k <= ig.n_steps; k++) need[log_mask_at(log, ig.init_step + k)] = true;
+                GraphKey key{ig, vcoupling, 0};
+                for (int m = 0; m < 8 && use_graph; m++) {
+                    if (!need[m]) continue;
+                    key.log_mask = m;
+                    if (!graphs_[m].exec || !(key == graphs_[m].key)) {
+                        if (build_step_graph(c, key) != MB_OK) {
+                            graph_failed_ = true;  // stay on the stream path for this context
+                            use_graph = false;
+                        }
                     }
                 }
             }
-        }
-        graph_used_ = use_graph;
-        if (use_graph) {
-            for (int64_t k = 1; k <= ig.n_steps; k++) {
-                const int m = log_mask_at(log, ig.init_step + k);
-                MB_CUDA(cudaGraphLaunch(graphs_[m].exec, stream_));
-                launches_ += graphs_[m].launches;  // rebuild-body kernels are not counted
-                n_force_evals_ += graphs_[m].evals;
-                MB_TRY(log_step(lr, m));
-            }
-            n_steps_ += ig.n_steps;
-        } else {
-            for (int64_t k = 1; k <= ig.n_steps; k++) {
-                const int64_t step_n = ig.init_step + k;
-                const int do_cm = (ig.remove_cm_every != 0 && step_n % ig.remove_cm_every == 0) ? 1 : 0;
-                const bool clear_after_k1 = cm_pending && !do_cm;  // K1 consumed v_cm; nothing overwrites it this step
-                // decomposed: fixed interval counted on the host (identical on every rank), adapted per call from the displacements
-                bool hint;
-                if (dec) {
-                    hint = since_rebuild_ >= decomposed_interval();
-                    since_rebuild_ = hint ? 1 : since_rebuild_ + 1;
-                    adapt_span_ = std::max(adapt_span_, since_rebuild_);
-                } else {
-                    hint = rebuild_every_ > 0 && k > 1 && (step_n - 1) % rebuild_every_ == 0;
+            graph_used_ = use_graph;
+            if (use_graph) {
+                for (int64_t k = 1; k <= ig.n_steps; k++) {
+                    const int m = log_mask_at(log, ig.init_step + k);
+                    MB_CUDA(cudaGraphLaunch(graphs_[m].exec, stream_));
+                    launches_ += graphs_[m].launches;  // rebuild-body kernels are not counted
+                    n_force_evals_ += graphs_[m].evals;
+                    MB_TRY(log_step(lr, m));
                 }
-                StepOpts o;
-                o.do_cm = do_cm;
-                o.clear_cm_after_k1 = clear_after_k1 && (c.ig.kind == INTEG_VV || is_mts(c.ig.kind));
-                o.rebuild_hint = hint;
-                o.defer_cm = k < ig.n_steps;
-                o.log_mask = log_mask_at(log, step_n);
-                MB_TRY(enqueue_step(c, o));
-                MB_TRY(log_step(lr, o.log_mask));
-                cm_pending = (do_cm != 0) && !(c.thermostat && dec);  // (the standalone thermostat kernel consumes v_cm)
-                n_steps_++;
+                n_steps_ += ig.n_steps;
+            } else {
+                for (int64_t k = 1; k <= ig.n_steps; k++) {
+                    const int64_t step_n = ig.init_step + k;
+                    const int do_cm = (ig.remove_cm_every != 0 && step_n % ig.remove_cm_every == 0) ? 1 : 0;
+                    StepOpts o;
+                    o.do_cm = do_cm;
+                    o.clear_cm_after_k1 = cm_pending && !do_cm;  // K1 consumed v_cm; nothing overwrites it this step
+                    o.rebuild_hint = rebuild_every_ > 0 && k > 1 && (step_n - 1) % rebuild_every_ == 0;
+                    o.log_mask = log_mask_at(log, step_n);
+                    MB_TRY(enqueue_step(c, o));
+                    MB_TRY(log_step(lr, o.log_mask));
+                    cm_pending = do_cm != 0;
+                    n_steps_++;
+                }
             }
-        }
-        if (c.thermostat && !dec && ig.n_steps > 0) {
-            // the thermostat of the last step (the earlier ones ran inside the next step's drift kernel)
-            andersen_kernel<T><<<nb, 256, 0, stream_>>>(0, (int)n_, (int)n_, c.kT, c.ig.andersen_prob, d_orig_.as<int>(), d_mass_.as<T>(), d_vel4_.as<T4>(), cm, ctl);
-            launches_++;
-        }
-        if (dec) {
-            MB_TRY(allgather_state());  // every rank returns the whole system
-            build_nb_ = -1;
-            if (rebuild_every_ == 0) MB_TRY(adapt_interval());
+            if (thermo_in_k1(c).on && ig.n_steps > 0) {
+                // the thermostat of the last step (the earlier ones ran inside the next step's drift kernel)
+                andersen_kernel<T><<<nb, 256, 0, stream_>>>(0, (int)n_, (int)n_, c.kT, c.ig.andersen_prob, d_orig_.as<int>(), d_mass_.as<T>(), d_vel4_.as<T4>(), cm, ctl);
+                launches_++;
+            }
         }
         // export
         export_kernel<T><<<nb, 256, 0, stream_>>>((int)n_, geom(), d_pos4_.as<T4>(), d_vel4_.as<T4>(), d_orig_.as<int>(), cm, xb.as<T>(),

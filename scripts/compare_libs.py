@@ -6,11 +6,12 @@
    with bonded terms; graph and stream step paths) runs once with each library in a fresh process; kernel_launches,
    n_force_evals and graph_mode from stats() after every call must be identical.
 2. Integration and minimisation runs, each on a fresh context, in a fresh process per library: VelocityVerlet (plain,
-   Immediate, Berendsen, Bussi with n_steps 1 and 5, Andersen), Langevin and NoseHoover under remove_CM_motion 0, 1, 3 and
-   init_step 0, 7, each integrator with all six device loggers, a SteepestDescentMinimizer run and random_velocities; on
-   all-pairs and brick systems, f32 and f64, graph and stream (MOLLYB200_NO_GRAPH=1) paths. The systems have no bonded
-   terms, so no float atomics enter: coordinates, velocities, logger histories and the minimiser trace must be
-   bit-identical, and the stats after every run identical.
+   Immediate, Berendsen, Bussi with n_steps 1 and 5, Andersen), Langevin, NoseHoover, MTSIntegrator with 2 and 3 levels,
+   MTSLangevinIntegrator and LangevinSplitting (BAOAB, OBABO, ABOBA, BAB) under remove_CM_motion 0, 1, 3 and init_step 0,
+   7, each integrator with all six device loggers, a SteepestDescentMinimizer run and random_velocities; on all-pairs and
+   brick systems, f32 and f64, graph and stream (MOLLYB200_NO_GRAPH=1) paths. The systems have no bonded terms, so the
+   inner MTS levels carry zero forces and no float atomics enter: coordinates, velocities, logger histories and the
+   minimiser trace must be bit-identical, and the stats after every run identical.
 3. bench.py --workload c2 / c3 --dump-outputs with each library: C2 coordinates and velocities must be bit-identical. C3 adds
    bonded forces with float atomics, so the OLD library runs it twice and the OLD-vs-NEW difference must lie within
    twice that run-to-run difference.
@@ -67,11 +68,24 @@ def _run_sequence(out):
     lj = lambda nl: (mb.LennardJones(cutoff=mb.ShiftedForceCutoff(1.0), use_neighbors=nl),)
     systems = {"allpairs": (6, False, 0.0), "brick": (8, True, 1.2)}
     dt = 0.002
+
+    def mts(cls, fractions, *args):
+        def make(cm):
+            sim = cls(dt, *args, pi_fractions=(1,), remove_CM_motion=cm)
+            sim.ordered_fractions = fractions  # levels that hold no term: (1,) alone would run as VelocityVerlet
+            return sim
+        return make
+
     integrators = {
         "vv": lambda cm: mb.VelocityVerlet(dt=dt, remove_CM_motion=cm),
         "langevin": lambda cm: mb.Langevin(dt=dt, temperature=100.0, friction=2.0, remove_CM_motion=cm),
         "nosehoover": lambda cm: mb.NoseHoover(dt=dt, temperature=100.0, remove_CM_motion=cm),
+        "mts2": mts(mb.MTSIntegrator, (1, 2)),
+        "mts3": mts(mb.MTSIntegrator, (1, 2, 4)),
+        "mtslangevin": mts(mb.MTSLangevinIntegrator, (1, 2), 100.0, 2.0),
     }
+    for splitting in ("BAOAB", "OBABO", "ABOBA", "BAB"):
+        integrators[f"split-{splitting}"] = lambda cm, sp=splitting: mb.LangevinSplitting(dt, 100.0, 80.0, sp, remove_CM_motion=cm)
     couplings = {"immediate": mb.ImmediateThermostat(120.0), "berendsen": mb.BerendsenThermostat(120.0, 0.05),
                  "bussi1": mb.VelocityRescaleThermostat(120.0, 0.05), "bussi5": mb.VelocityRescaleThermostat(120.0, 0.05, 5),
                  "andersen": mb.AndersenThermostat(120.0, 0.05)}
