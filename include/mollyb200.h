@@ -468,6 +468,65 @@ typedef struct {
 } mb_splitting_params_t;
 int mb_simulate_langevin_splitting(mb_ctx* ctx, void* coords, void* vels, const mb_splitting_params_t* p, mb_log_t* log);
 
+/* simulate!(sys, Verlet(dt; coupling, remove_CM_motion), n_steps) (src/simulators.jl:858-955), the leapfrog integrator: the
+ * velocities are half a step behind the positions. Prologue as mb_simulate_vv: wrap, CM removal when init_step == 0 and
+ * remove_cm_every != 0, neighbours, F0, loggers at init_step. Step n, with a = F/m:
+ *   1. v += a dt
+ *   2. x += v dt (one full drift); wrap
+ *   3. CM removal when n % remove_cm_every == 0
+ *   4. coupling: the Andersen thermostat of mb_simulate_vv when andersen_kT > 0 and andersen_prob > 0, with the same draws
+ *   5. neighbours; F = forces(x) for step n + 1; loggers (mb_log_t, as for mb_simulate_vv_log; NULL: no logging).
+ * The parameters are mb_vv_params_t's. One step is one fused kernel plus the force evaluation (and the Andersen kernel).
+ * Where the engine differs from the reference:
+ *  - the neighbour rebuild is triggered by the exact displacement test (as for mb_simulate_vv);
+ *  - massless atoms (1/m = 0) get no kick.
+ * MB_ERR_INVALID before any work for dt <= 0, n_steps < 0, a velocity coupling set on the context
+ * (mb_set_velocity_coupling; velocity-rescaling couplings with Verlet take the stock path), a decomposed (multi-GPU)
+ * context, and the logging errors of mb_simulate_vv_log. MB_ERR_CAPACITY as in mb_simulate_vv. */
+int mb_simulate_verlet(mb_ctx* ctx, void* coords, void* vels, const mb_vv_params_t* p, mb_log_t* log);
+
+/* simulate!(sys, StormerVerlet(dt), n_steps) (src/simulators.jl:957-1063). No coupling and no CM removal, not even in the
+ * prologue: wrap, neighbours, F0, loggers at init_step. Step n, with a = F/m:
+ *   1. d = v dt + a dt^2 / 2 on the first step of every call, d = v dt + a dt^2 on later steps
+ *   2. x += d; v = d / dt; wrap
+ *   3. neighbours; F = forces(x) for step n + 1; loggers (mb_log_t, as for mb_simulate_vv_log; NULL: no logging).
+ * The reference forms the later steps from vector(x_last, x) + a dt^2 and sets v = vector(x_before, x_after) / dt. The
+ * engine keeps no second coordinate set: at the end of a step v dt is that displacement, so it carries the previous
+ * displacement as the velocity, through cell-list re-sorts and from one call to the next. Where the engine differs from the
+ * reference:
+ *  - f32: v dt is the displacement up to rounding, where the reference takes `vector` of wrapped coordinates, so the two
+ *    differ at the ulp level;
+ *  - the neighbour rebuild is triggered by the exact displacement test (as for mb_simulate_vv);
+ *  - massless atoms (1/m = 0) feel no force.
+ * MB_ERR_INVALID before any work for dt <= 0, n_steps < 0, a velocity coupling set on the context, a decomposed (multi-GPU)
+ * context, and the logging errors of mb_simulate_vv_log. MB_ERR_CAPACITY as in mb_simulate_vv. */
+typedef struct {
+    double dt;
+    int64_t n_steps;
+    int64_t init_step;
+} mb_stormer_params_t;
+int mb_simulate_stormer_verlet(mb_ctx* ctx, void* coords, void* vels, const mb_stormer_params_t* p, mb_log_t* log);
+
+/* simulate!(sys, OverdampedLangevin(dt, temperature, friction; remove_CM_motion), n_steps) (src/simulators.jl:1400-1490),
+ * Brownian dynamics by Euler-Maruyama. Prologue as mb_simulate_vv: wrap, CM removal when init_step == 0 and
+ * remove_cm_every != 0, neighbours, F0, loggers at init_step. Step n, with a = F/m and gamma the friction in ps^-1:
+ *   1. x += a / gamma dt + sqrt(2 dt / gamma) sqrt(kT / m_i) xi with xi ~ N(0, 1)^3; wrap
+ *   2. CM removal of v when n % remove_cm_every == 0. The velocities are otherwise never changed: as in the reference, the
+ *      removal only affects what the loggers see
+ *   3. neighbours; F = forces(x) for step n + 1; loggers (mb_log_t, as for mb_simulate_vv_log; NULL: no logging).
+ * The parameters are mb_langevin_params_t's. One step is one fused kernel plus the force evaluation. Where the engine
+ * differs from the reference:
+ *  - random numbers: xi is mb_simulate_langevin's draw (one Philox4x32-10 block with counter (i, n, ctr1) and key
+ *    `rng_key`, i the 1-based original index). A function of (keys, step, atom) only, so a run split into calls with the
+ *    same keys takes the same draws; the reference's draws agree in distribution only;
+ *  - f32: the displacement is formed in double and the new position rounded once;
+ *  - massless atoms (1/m = 0) do not move (the reference's noise is Inf there);
+ *  - the neighbour rebuild is triggered by the exact displacement test (as for mb_simulate_vv).
+ * MB_ERR_INVALID before any work for dt <= 0, n_steps < 0, kT negative or not finite, friction <= 0 or not finite (the
+ * reference's noise prefactor is infinite at 0), a velocity coupling set on the context, a decomposed (multi-GPU) context,
+ * and the logging errors of mb_simulate_vv_log. MB_ERR_CAPACITY as in mb_simulate_vv. */
+int mb_simulate_overdamped_langevin(mb_ctx* ctx, void* coords, void* vels, const mb_langevin_params_t* p, mb_log_t* log);
+
 /* simulate!(sys, SteepestDescentMinimizer(step_size, max_steps, tol)) (src/simulators.jl:183-274) on the device: wrap the
  * coordinates, E = potential energy; then for step n = init_step+1 .. init_step+max_steps: F = forces, m = max |F_i|,
  * x <- wrap(x + h F / m), E_trial = potential energy; E_trial < E accepts (h <- 6h/5, E <- E_trial), otherwise x is restored

@@ -13,6 +13,9 @@
 #   Molly.simulate!(sys, sim::NoseHoover, n_steps; ...) with coupling === nothing                            simulators.jl:1534
 #   Molly.simulate!(sys, sim::LangevinSplitting, n_steps; ...) with at most 32 letters                      simulators.jl:1252
 #   Molly.simulate!(sys, sim::AbstractMTSIntegrator, n_steps; ...) with coupling === nothing                 simulators.jl:1850
+#   Molly.simulate!(sys, sim::Verlet, n_steps; ...) with coupling nothing or one AndersenThermostat           simulators.jl:868
+#   Molly.simulate!(sys, sim::StormerVerlet, n_steps; ...)                                                   simulators.jl:970
+#   Molly.simulate!(sys, sim::OverdampedLangevin, n_steps; ...)                                              simulators.jl:1427
 # (Molly.remove_CM_motion! for CuArray Systems is NOT redefined: the stock extension owns that exact signature)
 # and falls through to the stock methods (invoke) for anything it does not recognise: non-cubic boundaries,
 # constraints, virtual sites, couplings other than one AndersenThermostat, ImmediateThermostat, BerendsenThermostat or
@@ -93,6 +96,13 @@ struct MBNoseHooverParams
     remove_cm_every::Int32
     kT::Float64
     damping::Float64
+end
+
+# mb_stormer_params_t (mb_simulate_stormer_verlet)
+struct MBStormerParams
+    dt::Float64
+    n_steps::Int64
+    init_step::Int64
 end
 
 # mb_mts_params_t (mb_simulate_mts)
@@ -616,6 +626,103 @@ function Molly.simulate!(sys::System{3, <:CuArray, T}, sim::NoseHoover, n_steps:
         end
     end
     check(ccall((:mb_simulate_nose_hoover, LIB), Cint, (Ptr{Cvoid}, CuPtr{Cvoid}, CuPtr{Cvoid}, Ref{MBNoseHooverParams}, Ptr{MBLog}),
+                ctx.handle, pointer(sys.coords), pointer(sys.velocities), Ref(p), C_NULL))
+    return sys
+end
+
+# ---- simulate!(sys, ::Verlet / ::StormerVerlet / ::OverdampedLangevin, n) (src/simulators.jl:858-1063, :1400-1490) -------
+# Taken over under the conditions of the Langevin method above; Verlet only with coupling nothing or one AndersenThermostat
+# (velocity-rescaling couplings with Verlet run the stock method). One mb_simulate_verlet, mb_simulate_stormer_verlet or
+# mb_simulate_overdamped_langevin call; OverdampedLangevin's friction is in ps^-1. Anything else runs the stock method.
+function plain_takeover_ok(sys, descs, run_loggers)
+    device_logs = run_loggers == false || isempty(sys.loggers) ||
+                  all(l -> !isnothing(device_log_kind(l)), values(sys.loggers))
+    return !isnothing(descs) && device_logs && general_ok(sys) && gb_ok(sys) &&
+           all(!isnothing, map(specific_desc, sys.specific_inter_lists))
+end
+
+function Molly.simulate!(sys::System{3, <:CuArray, T}, sim::Verlet, n_steps::Integer;
+                         init_step=0, rng=Random.default_rng(), run_loggers=true, kwargs...) where T
+    descs = engine_eligible(sys, sys.pairwise_inters)
+    couplings = filter(c -> !(c isa Molly.NoCoupling), sim.coupling isa Tuple ? sim.coupling : (sim.coupling,))
+    couplings = filter(!isnothing, collect(couplings))
+    if !plain_takeover_ok(sys, descs, run_loggers) || length(couplings) > 1 ||
+            !all(c -> c isa AndersenThermostat, couplings)
+        # stock: simulate!(sys, sim::Verlet, n_steps_or_time; ...) src/simulators.jl:868
+        return invoke(Molly.simulate!, Tuple{Any, Verlet, Any}, sys, sim, n_steps;
+                      init_step=init_step, rng=rng, run_loggers=run_loggers, kwargs...)
+    end
+    ctx = context_for(sys, descs)
+    set_specific!(ctx, sys)
+    set_implicit_solvent!(ctx, sys)
+    set_velocity_coupling!(ctx, nothing)
+    kT, prob = 0.0, 0.0
+    for c in couplings
+        kT = Float64(ustrip(sys.k * c.temperature))
+        prob = Float64(ustrip(sim.dt / c.coupling_const))
+    end
+    p = MBVVParams(_ps(sim.dt), n_steps, init_step, Int32(sim.remove_CM_motion), kT, prob, rand(rng, UInt64), rand(rng, UInt64))
+    if run_loggers != false && !isempty(sys.loggers)
+        return simulate_logged!(sys, ctx, n_steps, init_step, run_loggers) do lg
+            ccall((:mb_simulate_verlet, LIB), Cint, (Ptr{Cvoid}, CuPtr{Cvoid}, CuPtr{Cvoid}, Ref{MBVVParams}, Ref{MBLog}),
+                  ctx.handle, pointer(sys.coords), pointer(sys.velocities), Ref(p), lg)
+        end
+    end
+    check(ccall((:mb_simulate_verlet, LIB), Cint, (Ptr{Cvoid}, CuPtr{Cvoid}, CuPtr{Cvoid}, Ref{MBVVParams}, Ptr{MBLog}),
+                ctx.handle, pointer(sys.coords), pointer(sys.velocities), Ref(p), C_NULL))
+    return sys
+end
+
+function Molly.simulate!(sys::System{3, <:CuArray, T}, sim::StormerVerlet, n_steps::Integer;
+                         init_step=0, rng=Random.default_rng(), run_loggers=true, kwargs...) where T
+    descs = engine_eligible(sys, sys.pairwise_inters)
+    if !plain_takeover_ok(sys, descs, run_loggers)
+        # stock: simulate!(sys, sim::StormerVerlet, n_steps_or_time; ...) src/simulators.jl:970
+        return invoke(Molly.simulate!, Tuple{Any, StormerVerlet, Any}, sys, sim, n_steps;
+                      init_step=init_step, rng=rng, run_loggers=run_loggers, kwargs...)
+    end
+    ctx = context_for(sys, descs)
+    set_specific!(ctx, sys)
+    set_implicit_solvent!(ctx, sys)
+    set_velocity_coupling!(ctx, nothing)
+    p = MBStormerParams(_ps(sim.dt), n_steps, init_step)
+    if run_loggers != false && !isempty(sys.loggers)
+        return simulate_logged!(sys, ctx, n_steps, init_step, run_loggers) do lg
+            ccall((:mb_simulate_stormer_verlet, LIB), Cint,
+                  (Ptr{Cvoid}, CuPtr{Cvoid}, CuPtr{Cvoid}, Ref{MBStormerParams}, Ref{MBLog}),
+                  ctx.handle, pointer(sys.coords), pointer(sys.velocities), Ref(p), lg)
+        end
+    end
+    check(ccall((:mb_simulate_stormer_verlet, LIB), Cint,
+                (Ptr{Cvoid}, CuPtr{Cvoid}, CuPtr{Cvoid}, Ref{MBStormerParams}, Ptr{MBLog}),
+                ctx.handle, pointer(sys.coords), pointer(sys.velocities), Ref(p), C_NULL))
+    return sys
+end
+
+function Molly.simulate!(sys::System{3, <:CuArray, T}, sim::OverdampedLangevin, n_steps::Integer;
+                         init_step=0, rng=Random.default_rng(), run_loggers=true, kwargs...) where T
+    descs = engine_eligible(sys, sys.pairwise_inters)
+    friction = sim.friction isa Unitful.Quantity ? Float64(ustrip(u"ps^-1", sim.friction)) : Float64(sim.friction)
+    if !plain_takeover_ok(sys, descs, run_loggers) || !(isfinite(friction) && friction > 0)
+        # stock: simulate!(sys, sim::OverdampedLangevin, n_steps_or_time; ...) src/simulators.jl:1427
+        return invoke(Molly.simulate!, Tuple{Any, OverdampedLangevin, Any}, sys, sim, n_steps;
+                      init_step=init_step, rng=rng, run_loggers=run_loggers, kwargs...)
+    end
+    ctx = context_for(sys, descs)
+    set_specific!(ctx, sys)
+    set_implicit_solvent!(ctx, sys)
+    set_velocity_coupling!(ctx, nothing)
+    p = MBLangevinParams(_ps(sim.dt), n_steps, init_step, Int32(sim.remove_CM_motion),
+                         Float64(ustrip(sys.k * sim.temperature)), friction, rand(rng, UInt64), rand(rng, UInt64))
+    if run_loggers != false && !isempty(sys.loggers)
+        return simulate_logged!(sys, ctx, n_steps, init_step, run_loggers) do lg
+            ccall((:mb_simulate_overdamped_langevin, LIB), Cint,
+                  (Ptr{Cvoid}, CuPtr{Cvoid}, CuPtr{Cvoid}, Ref{MBLangevinParams}, Ref{MBLog}),
+                  ctx.handle, pointer(sys.coords), pointer(sys.velocities), Ref(p), lg)
+        end
+    end
+    check(ccall((:mb_simulate_overdamped_langevin, LIB), Cint,
+                (Ptr{Cvoid}, CuPtr{Cvoid}, CuPtr{Cvoid}, Ref{MBLangevinParams}, Ptr{MBLog}),
                 ctx.handle, pointer(sys.coords), pointer(sys.velocities), Ref(p), C_NULL))
     return sys
 end

@@ -23,7 +23,7 @@ EXPORTED = [
     "mb_set_lj_dispersion_correction", "mb_random_velocities", "mb_kinetic_energy_tensor", "mb_set_box_triclinic",
     "mb_simulate_vv_log", "mb_minimize_sd", "mb_set_velocity_coupling", "mb_simulate_langevin",
     "mb_simulate_nose_hoover", "mb_set_specific_levels", "mb_simulate_mts", "mb_set_implicit_solvent",
-    "mb_simulate_langevin_splitting",
+    "mb_simulate_langevin_splitting", "mb_simulate_verlet", "mb_simulate_stormer_verlet", "mb_simulate_overdamped_langevin",
 ]
 MB_GB_MAX_NECK_CLASSES = 32
 # specific interaction kinds of mb_set_specific (include/mollyb200.h)
@@ -101,6 +101,10 @@ class MBSplittingParams(C.Structure):
     ]
 
 
+class MBStormerParams(C.Structure):
+    _fields_ = [("dt", C.c_double), ("n_steps", C.c_int64), ("init_step", C.c_int64)]
+
+
 class MBVCoupling(C.Structure):
     _fields_ = [("kind", C.c_int32), ("n_steps", C.c_int32), ("kT", C.c_double), ("tau", C.c_double)]
 
@@ -162,6 +166,9 @@ def load():
     L.mb_simulate_nose_hoover.argtypes = [vp, vp, vp, C.POINTER(MBNoseHooverParams), C.POINTER(MBLog)]
     L.mb_simulate_mts.argtypes = [vp, vp, vp, C.POINTER(MBMTSParams), C.POINTER(MBLog)]
     L.mb_simulate_langevin_splitting.argtypes = [vp, vp, vp, C.POINTER(MBSplittingParams), C.POINTER(MBLog)]
+    L.mb_simulate_verlet.argtypes = [vp, vp, vp, C.POINTER(MBVVParams), C.POINTER(MBLog)]
+    L.mb_simulate_stormer_verlet.argtypes = [vp, vp, vp, C.POINTER(MBStormerParams), C.POINTER(MBLog)]
+    L.mb_simulate_overdamped_langevin.argtypes = [vp, vp, vp, C.POINTER(MBLangevinParams), C.POINTER(MBLog)]
     L.mb_set_specific_levels.argtypes = [vp, C.c_int, i64, vp]
     L.mb_minimize_sd.argtypes = [vp, vp, C.POINTER(MBSDParams)]
     L.mb_set_velocity_coupling.argtypes = [vp, C.POINTER(MBVCoupling)]

@@ -15,6 +15,8 @@ julia/MollyB200Ext.jl, see INTEGRATION.md):
     Langevin                                        src/simulators.jl:1065-1210 (mb_simulate_langevin)
     LangevinSplitting                               src/simulators.jl:1212-1398 (mb_simulate_langevin_splitting)
     NoseHoover                                      src/simulators.jl:1491-1614 (mb_simulate_nose_hoover)
+    Verlet, StormerVerlet                           src/simulators.jl:858-1063 (mb_simulate_verlet, mb_simulate_stormer_verlet)
+    OverdampedLangevin                              src/simulators.jl:1400-1490 (mb_simulate_overdamped_langevin)
     MTSIntegrator, MTSLangevinIntegrator            src/simulators.jl:1616-1940 (mb_simulate_mts)
     forces, forces_virial, potential_energy         src/force.jl:678-720, src/energy.jl:202-248
     kinetic_energy, temperature, remove_CM_motion   src/energy.jl:44-175, src/spatial.jl:901-929
@@ -738,6 +740,61 @@ class NoseHoover:
             raise ValueError(f"remove_CM_motion must be non-negative, found {self.remove_CM_motion}")
 
 
+def _check_dt(dt):
+    if not (math.isfinite(dt) and dt > 0):
+        raise ValueError(f"dt must be finite and positive, found {dt}")
+
+
+def _check_remove_cm(sim):
+    sim.remove_CM_motion = int(sim.remove_CM_motion)  # Int(remove_CM_motion): false -> 0
+    if sim.remove_CM_motion < 0:
+        raise ValueError(f"remove_CM_motion must be non-negative, found {sim.remove_CM_motion}")
+
+
+@dataclass
+class Verlet:
+    """Verlet(dt; coupling=None, remove_CM_motion=1) — src/simulators.jl:858-955, the leapfrog integrator (the velocities
+    are half a step behind the positions), run on the device by mb_simulate_verlet (see include/mollyb200.h). dt in ps. The
+    coupling may be None or one AndersenThermostat; simulate raises TypeError for any other."""
+    dt: float
+    coupling: object = None
+    remove_CM_motion: int = 1
+
+    def __post_init__(self):
+        _check_dt(self.dt)
+        _check_remove_cm(self)
+
+
+@dataclass
+class StormerVerlet:
+    """StormerVerlet(dt) — src/simulators.jl:957-1063, run on the device by mb_simulate_stormer_verlet (see
+    include/mollyb200.h). dt in ps. No coupling and no centre-of-mass motion removal; the first step of every call starts
+    from the velocities, later steps from the previous displacement."""
+    dt: float
+
+    def __post_init__(self):
+        _check_dt(self.dt)
+
+
+@dataclass
+class OverdampedLangevin:
+    """OverdampedLangevin(dt, temperature, friction; remove_CM_motion=1) — src/simulators.jl:1400-1490, Brownian dynamics
+    by Euler-Maruyama, run on the device by mb_simulate_overdamped_langevin (see include/mollyb200.h). dt in ps,
+    temperature in K, friction in ps^-1 (> 0: the noise prefactor is sqrt(2 dt / friction)). The velocities only lose
+    their centre-of-mass drift."""
+    dt: float
+    temperature: float
+    friction: float
+    remove_CM_motion: int = 1
+
+    def __post_init__(self):
+        _check_dt(self.dt)
+        _check_temperature(self.temperature)
+        if not (math.isfinite(self.friction) and self.friction > 0):
+            raise ValueError(f"friction must be finite and positive, found {self.friction}")
+        _check_remove_cm(self)
+
+
 def _is_integer(x) -> bool:
     return isinstance(x, (int, np.integer))
 
@@ -1265,6 +1322,9 @@ _SIMULATE_ENTRY = {
     NoseHoover: (capi.MBNoseHooverParams, "mb_simulate_nose_hoover"),
     MTSIntegrator: (capi.MBMTSParams, "mb_simulate_mts"),
     MTSLangevinIntegrator: (capi.MBMTSParams, "mb_simulate_mts"),
+    Verlet: (capi.MBVVParams, "mb_simulate_verlet"),
+    StormerVerlet: (capi.MBStormerParams, "mb_simulate_stormer_verlet"),
+    OverdampedLangevin: (capi.MBLangevinParams, "mb_simulate_overdamped_langevin"),
 }
 
 
@@ -1283,6 +1343,9 @@ def simulate(sys: System, sim, n_steps: Optional[int] = None, init_step: int = 0
     MTSIntegrator, MTSLangevinIntegrator: simulate!(sys, sim, n_steps; run_loggers=true) — src/simulators.jl:1783-1940,
     n_steps outer steps; the same arguments and loggers (once per outer step) as VelocityVerlet. The level of every specific
     term is set on the context (mb_set_specific_levels) before the call.
+    Verlet, StormerVerlet, OverdampedLangevin: simulate!(sys, sim, n_steps; run_loggers=true) — src/simulators.jl:868-955,
+    :970-1063, :1427-1490, the same arguments and loggers as VelocityVerlet. Verlet's velocities are half a step behind the
+    positions; StormerVerlet's first step of every call starts from the velocities.
     SteepestDescentMinimizer: simulate!(sys, sim; run_loggers=false) — src/simulators.jl:183-274, see steepest_descent.
     Loggers are not run during a minimisation (run_loggers must be false)."""
     if isinstance(sim, SteepestDescentMinimizer):
@@ -1301,7 +1364,7 @@ def simulate(sys: System, sim, n_steps: Optional[int] = None, init_step: int = 0
     if run_loggers is None:
         run_loggers = True
     _check_run_loggers(run_loggers)
-    coupling = getattr(sim, "coupling", None)  # (LangevinSplitting has none)
+    coupling = getattr(sim, "coupling", None)  # (LangevinSplitting, StormerVerlet, OverdampedLangevin have none)
     couplings = coupling if isinstance(coupling, (tuple, list)) else ((coupling,) if coupling else ())
     mts = params_t is capi.MBMTSParams
     p = params_t()  # (zero-filled: no Andersen thermostat, no noise)
@@ -1315,6 +1378,12 @@ def simulate(sys: System, sim, n_steps: Optional[int] = None, init_step: int = 0
                 p.andersen_prob = sim.dt / c.coupling_const
             else:
                 raise TypeError(f"unsupported coupling {c!r} (the stock Molly path handles it)")
+    elif isinstance(sim, Verlet):
+        for c in couplings:
+            if not (isinstance(c, AndersenThermostat) and len(couplings) == 1):
+                raise TypeError(f"unsupported coupling {c!r} with Verlet (the stock Molly path handles it)")
+            p.andersen_kT = sys.k * c.temperature
+            p.andersen_prob = sim.dt / c.coupling_const
     elif couplings:
         raise TypeError(f"unsupported coupling {couplings[0]!r} with {type(sim).__name__} (the stock Molly path handles it)")
     if mts:
@@ -1322,9 +1391,9 @@ def simulate(sys: System, sim, n_steps: Optional[int] = None, init_step: int = 0
         p.n_levels = len(sim.ordered_fractions)
         p.fractions[:p.n_levels] = sim.ordered_fractions
         p.langevin = int(isinstance(sim, MTSLangevinIntegrator))
-    if isinstance(sim, (Langevin, NoseHoover, MTSLangevinIntegrator, LangevinSplitting)):
+    if isinstance(sim, (Langevin, NoseHoover, MTSLangevinIntegrator, LangevinSplitting, OverdampedLangevin)):
         p.kT = sys.k * sim.temperature
-    if isinstance(sim, (Langevin, MTSLangevinIntegrator, LangevinSplitting)):
+    if isinstance(sim, (Langevin, MTSLangevinIntegrator, LangevinSplitting, OverdampedLangevin)):
         p.friction = float(sim.friction)
     if isinstance(sim, LangevinSplitting):
         p.n_ops = len(sim.splitting)
@@ -1334,13 +1403,14 @@ def simulate(sys: System, sim, n_steps: Optional[int] = None, init_step: int = 0
     p.dt = float(sim.dt)
     p.n_steps = int(n_steps)
     p.init_step = int(init_step)
-    p.remove_cm_every = int(sim.remove_CM_motion)
+    if not isinstance(sim, StormerVerlet):  # (StormerVerlet never removes it)
+        p.remove_cm_every = int(sim.remove_CM_motion)
     ctx = sys.engine()
     capi.check(sys._L.mb_set_velocity_coupling(ctx, C.byref(vc) if vc is not None else None))  # (Langevin, NoseHoover: cleared)
     if mts:  # (an unchanged level array leaves the context as it is)
         for kind, lv in levels.items():
             capi.check(sys._L.mb_set_specific_levels(ctx, kind, len(lv), lv.ctypes.data))
-    if not isinstance(sim, NoseHoover):  # (NoseHoover draws nothing)
+    if not isinstance(sim, (NoseHoover, StormerVerlet)):  # (these two draw nothing)
         rng = rng or np.random.default_rng()
         p.rng_ctr1 = int(rng.integers(0, 2 ** 63))
         p.rng_key = int(rng.integers(0, 2 ** 63))

@@ -16,6 +16,7 @@
 #include "force.cuh"
 #include "gbsa.cuh"
 #include "langevin.cuh"
+#include "verlet.cuh"
 #include "minimize.cuh"
 #include "mts.cuh"
 #include "nosehoover.cuh"
@@ -318,9 +319,10 @@ static void pme_plan_host(const double box[3], double r_cut, double error_tol, i
 }
 
 // The integrator of one simulate call: VelocityVerlet (vv.cuh), Langevin (langevin.cuh), Nose-Hoover (nosehoover.cuh), the
-// multiple-time-step integrators (mts.cuh) or LangevinSplitting (splitting.cuh). Each mb_simulate_* entry point fills one
-// from its own parameters.
-enum { INTEG_VV = 0, INTEG_LANGEVIN = 1, INTEG_NH = 2, INTEG_MTS = 3, INTEG_MTS_LANGEVIN = 4, INTEG_SPLIT = 5 };
+// multiple-time-step integrators (mts.cuh), LangevinSplitting (splitting.cuh), or Verlet, StormerVerlet and
+// OverdampedLangevin (verlet.cuh). Each mb_simulate_* entry point fills one from its own parameters.
+enum { INTEG_VV = 0, INTEG_LANGEVIN = 1, INTEG_NH = 2, INTEG_MTS = 3, INTEG_MTS_LANGEVIN = 4, INTEG_SPLIT = 5, INTEG_VERLET = 6,
+       INTEG_STORMER = 7, INTEG_OVERDAMPED = 8 };
 static_assert(SPLIT_MAX_OPS == MB_SPLIT_MAX_OPS, "splitting length");
 static bool is_mts(int kind) { return kind == INTEG_MTS || kind == INTEG_MTS_LANGEVIN; }
 struct Integrator {
@@ -329,8 +331,9 @@ struct Integrator {
     int64_t n_steps = 0, init_step = 0;
     int remove_cm_every = 0;
     uint64_t rng_ctr1 = 0, rng_key = 0;
-    double andersen_kT = 0, andersen_prob = 0;  // VelocityVerlet's Andersen thermostat (kT <= 0 or prob <= 0: none)
-    double kT = 0, friction = 0, damping = 0;   // Langevin, MTSLangevinIntegrator and LangevinSplitting: kT, friction;
+    double andersen_kT = 0, andersen_prob = 0;  // VelocityVerlet's and Verlet's Andersen thermostat (kT <= 0 or prob <= 0: none)
+    double kT = 0, friction = 0, damping = 0;   // Langevin, MTSLangevinIntegrator, LangevinSplitting and OverdampedLangevin:
+                                                // kT, friction;
                                                 // Nose-Hoover: kT, damping
     int n_levels = 0;                           // the multiple-time-step integrators' ordered fractions (0 levels: none)
     std::array<int, MTS_MAX_LEVELS> fractions = {};
@@ -1953,6 +1956,7 @@ class Engine : public EngineBase {
         NhCoef nc;        // Nose-Hoover's dt / (2 Q^2) and Nf k T0
         SplitCoef<T> sc;  // LangevinSplitting's dt_A, dt_B, -friction dt_O and kT
         SplitPlan sp;     // LangevinSplitting's passes and evaluations
+        VerletCoef vt;    // StormerVerlet's dt^2; OverdampedLangevin's dt / gamma, sqrt(2 dt / gamma) and kT
     };
     // Langevin's c = exp(-dt friction), sqrt(1 - c^2) and kT (src/simulators.jl:1092-1097), in double. MTSLangevinIntegrator
     // runs its O step at the innermost substep, with f the innermost fraction: c = exp(-dt friction / f) (:1736-1738);
@@ -1984,6 +1988,9 @@ class Engine : public EngineBase {
             c.sc = SplitCoef<T>{k[SPLIT_A] ? (T)(ig.dt / k[SPLIT_A]) : (T)0, k[SPLIT_B] ? (T)(ig.dt / k[SPLIT_B]) : (T)0,
                                 k[SPLIT_O] ? -ig.friction * ig.dt / k[SPLIT_O] : 0.0, ig.kT};
         }
+        // OverdampedLangevin's noise_prefac = sqrt((2 / friction) dt) (src/simulators.jl:1451), in double
+        c.vt = VerletCoef{ig.dt * ig.dt, 0.0, 0.0, 0.0};
+        if (ig.kind == INTEG_OVERDAMPED) c.vt = VerletCoef{0.0, ig.dt / ig.friction, sqrt(2.0 / ig.friction * ig.dt), ig.kT};
         return c;
     }
     // what one step does beyond the plain VelocityVerlet step
@@ -2063,6 +2070,9 @@ class Engine : public EngineBase {
             case INTEG_MTS:
             case INTEG_MTS_LANGEVIN: return enqueue_mts_step(c, o, cap);
             case INTEG_SPLIT: return enqueue_split_step(c, o, cap);
+            case INTEG_VERLET:
+            case INTEG_STORMER:
+            case INTEG_OVERDAMPED: return enqueue_verlet_step(c, o, cap);
             default: return enqueue_vv_step(c, o, cap);
         }
     }
@@ -2124,6 +2134,36 @@ class Engine : public EngineBase {
         MB_TRY(after_drift(cap, o.rebuild_hint));
         MB_TRY(launch_pairs(false, d_f4_.as<T4>()));
         MB_TRY(launch_bonded(false));
+        if (o.log_mask) MB_TRY(enqueue_log(c, o.log_mask));
+        MB_CUDA(cudaGetLastError());
+        return MB_OK;
+    }
+    // One Verlet, StormerVerlet or OverdampedLangevin step (verlet.cuh): the step kernel, [rebuild], forces, [Verlet's
+    // Andersen thermostat], [log records]. The forces are the next step's; the step kernel clears a consumed v_cm itself,
+    // and the thermostat applies the v_cm this step publishes before it resamples.
+    int enqueue_verlet_step(const StepCfg& c, const StepOpts& o, Capture* cap) {
+        const int n = (int)n_;
+        Control* ctl = d_ctl_.as<Control>();
+        CmState<T>* cm = d_cm_.as<CmState<T>>();
+        const int kind = c.ig.kind == INTEG_VERLET ? VERLET_LEAPFROG : c.ig.kind == INTEG_STORMER ? VERLET_STORMER : VERLET_OVERDAMPED;
+        prof_.begin(Prof::VV);
+        int grid;
+        MB_TRY(integ_grid(grid, n, 1, 8, 3));
+        with_const<VERLET_LEAPFROG, VERLET_STORMER, VERLET_OVERDAMPED>(kind, [&](auto K) {
+            verlet_step_kernel<T, K><<<grid, VV_THREADS, 0, stream_>>>(
+                n, c.dt, c.skin_half2, c.vt, o.do_cm, c.inv_mass, cm, d_f4_.as<T4>(), d_xref4_.as<T4>(), d_pos4_.as<T4>(),
+                d_vel4_.as<T4>(), d_orig_.as<int>(), d_mass_.as<T>(), d_partial_.as<double>(), c.flag_ptr, ctl,
+                rebuild_handle(cap), cap && path_ == 1 ? 1 : 0, ext_map());
+        });
+        prof_.end(Prof::VV);
+        launches_++;
+        MB_TRY(after_drift(cap, o.rebuild_hint));
+        MB_TRY(launch_pairs(false, d_f4_.as<T4>()));
+        MB_TRY(launch_bonded(false));
+        if (c.thermostat) {
+            andersen_kernel<T><<<std::max(1, (n + 255) / 256), 256, 0, stream_>>>(0, n, n, c.kT, c.ig.andersen_prob, d_orig_.as<int>(), d_mass_.as<T>(), d_vel4_.as<T4>(), cm, ctl);
+            launches_++;
+        }
         if (o.log_mask) MB_TRY(enqueue_log(c, o.log_mask));
         MB_CUDA(cudaGetLastError());
         return MB_OK;
@@ -2296,7 +2336,7 @@ class Engine : public EngineBase {
     Thermo<T> thermo_in_k1(const StepCfg& c) const {
         Thermo<T> th;
         memset(&th, 0, sizeof(th));
-        if (c.thermostat && !decomposed()) {
+        if (c.thermostat && c.ig.kind == INTEG_VV && !decomposed()) {  // (Verlet runs the standalone kernel: enqueue_verlet_step)
             th.on = 1;
             th.n = (int)n_;
             th.kT = c.kT;
@@ -2614,9 +2654,11 @@ class Engine : public EngineBase {
     // The refusals of a simulate call, made before any work; each names the call's C entry point
     int check_simulate(const void* coords, const void* vels, const Integrator& ig) {
         static const char* const entry[] = {"mb_simulate_vv", "mb_simulate_langevin", "mb_simulate_nose_hoover", "mb_simulate_mts",
-                                            "mb_simulate_mts", "mb_simulate_langevin_splitting"};
+                                            "mb_simulate_mts", "mb_simulate_langevin_splitting", "mb_simulate_verlet",
+                                            "mb_simulate_stormer_verlet", "mb_simulate_overdamped_langevin"};
         static const char* const name[] = {"VelocityVerlet", "Langevin", "Nose-Hoover", "the multiple-time-step integrators",
-                                           "the multiple-time-step integrators", "LangevinSplitting"};
+                                           "the multiple-time-step integrators", "LangevinSplitting", "Verlet", "StormerVerlet",
+                                           "OverdampedLangevin"};
         if (!coords || !vels) return set_error(MB_ERR_INVALID, "null argument");
         if (ig.n_steps < 0 || !(ig.dt > 0)) return set_error(MB_ERR_INVALID, "n_steps < 0 or dt <= 0");
         const std::string who = std::string(entry[ig.kind]) + ": ";
@@ -2644,6 +2686,11 @@ class Engine : public EngineBase {
         if (ig.kind == INTEG_LANGEVIN || ig.kind == INTEG_MTS_LANGEVIN || ig.kind == INTEG_SPLIT) {
             if (!(std::isfinite(ig.kT) && ig.kT >= 0)) return set_error(MB_ERR_INVALID, who + "kT must be finite and >= 0");
             if (!(std::isfinite(ig.friction) && ig.friction >= 0)) return set_error(MB_ERR_INVALID, who + "friction must be finite and >= 0");
+        }
+        if (ig.kind == INTEG_OVERDAMPED) {
+            // (friction = 0 would make the noise prefactor sqrt(2 dt / friction) infinite)
+            if (!(std::isfinite(ig.kT) && ig.kT >= 0)) return set_error(MB_ERR_INVALID, who + "kT must be finite and >= 0");
+            if (!(std::isfinite(ig.friction) && ig.friction > 0)) return set_error(MB_ERR_INVALID, who + "friction must be finite and > 0");
         }
         if (ig.kind == INTEG_NH) {
             // (kT = 0 would make T / T0 infinite)
@@ -3313,6 +3360,32 @@ int mb_simulate_langevin_splitting(mb_ctx* ctx, void* coords, void* vels, const 
     ig.friction = p->friction;
     ig.n_ops = p->n_ops;
     std::copy_n(p->ops, std::clamp(p->n_ops, 0, MB_SPLIT_MAX_OPS), ig.ops.begin());
+    return ctx->e->simulate(coords, vels, ig, log);
+}
+int mb_simulate_verlet(mb_ctx* ctx, void* coords, void* vels, const mb_vv_params_t* p, mb_log_t* log) {
+    MB_CTX_GUARD(ctx);
+    if (!p) return mb::set_error(MB_ERR_INVALID, "null argument");
+    mb::Integrator ig = integrator_call(mb::INTEG_VERLET, p, p->rng_ctr1, p->rng_key);
+    ig.andersen_kT = p->andersen_kT;
+    ig.andersen_prob = p->andersen_prob;
+    return ctx->e->simulate(coords, vels, ig, log);
+}
+int mb_simulate_stormer_verlet(mb_ctx* ctx, void* coords, void* vels, const mb_stormer_params_t* p, mb_log_t* log) {
+    MB_CTX_GUARD(ctx);
+    if (!p) return mb::set_error(MB_ERR_INVALID, "null argument");
+    mb::Integrator ig;  // (no CM removal anywhere, so the prologue skips it too; no draws)
+    ig.kind = mb::INTEG_STORMER;
+    ig.dt = p->dt;
+    ig.n_steps = p->n_steps;
+    ig.init_step = p->init_step;
+    return ctx->e->simulate(coords, vels, ig, log);
+}
+int mb_simulate_overdamped_langevin(mb_ctx* ctx, void* coords, void* vels, const mb_langevin_params_t* p, mb_log_t* log) {
+    MB_CTX_GUARD(ctx);
+    if (!p) return mb::set_error(MB_ERR_INVALID, "null argument");
+    mb::Integrator ig = integrator_call(mb::INTEG_OVERDAMPED, p, p->rng_ctr1, p->rng_key);
+    ig.kT = p->kT;
+    ig.friction = p->friction;
     return ctx->e->simulate(coords, vels, ig, log);
 }
 int mb_minimize_sd(mb_ctx* ctx, void* coords, mb_sd_params_t* p) { MB_CTX_GUARD(ctx); return ctx->e->minimize_sd(coords, p); }
