@@ -527,6 +527,65 @@ int mb_simulate_stormer_verlet(mb_ctx* ctx, void* coords, void* vels, const mb_s
  * and the logging errors of mb_simulate_vv_log. MB_ERR_CAPACITY as in mb_simulate_vv. */
 int mb_simulate_overdamped_langevin(mb_ctx* ctx, void* coords, void* vels, const mb_langevin_params_t* p, mb_log_t* log);
 
+/* DPDInteraction(a, gamma, sigma, r_c, dt, use_neighbors, key) (src/interactions/dpd.jl:57-142), the pairwise interaction
+ * of dissipative particle dynamics. With dr = c_j - c_i, r = |dr|, w = 1 - r / r_c and v_ij = v_i - v_j, the force on i is
+ * -(f_C + f_D + f_R) dr with f_C = a w / r, f_D = gamma w^2 (dr . v_ij) / r^2, f_R = sigma w xi_ij dt^(-1/2) / r (dt is this
+ * struct's, not the integrator's), and the energy is the conservative part (a / 2) r_c w^2; all zero for r >= r_c and for
+ * r == 0. Special pairs get the full force; excluded pairs are skipped when use_neighbors is set (the reference's
+ * use_neighbors = false loop visits every pair). xi_ij is symmetric in (i, j), so momentum is conserved exactly: one
+ * Philox4x32-10 block with counter (min(i, j), max(i, j), step_lo, step_hi), i and j the 1-based atom indices and step the
+ * simulate! step_n, and key (key_lo, key_hi); one N(0, 1) value from its words 0 and 1 by Box-Muller in double (the first
+ * output of the O step's transform). The reference draws through PhiloxRNG.jl's randn: the two agree in distribution only.
+ * It replaces the pairwise interactions of the context and takes part in the path choice through use_neighbors as an
+ * mb_inter_t does: the cell-list path needs use_neighbors and r_list >= r_c (the reference suggests r_list = 1.5 r_c).
+ * Bonded lists (mb_set_specific) are allowed. NULL clears it. Drops the captured step graphs.
+ * MB_ERR_INVALID for r_c <= 0 or not finite, dt <= 0 or not finite, gamma or sigma < 0 or not finite, a not finite. Checked
+ * at the next evaluation or simulate call, before any work: an mb_inter_t interaction, PME, LJDispersionCorrection or
+ * implicit solvent on the same context, a decomposed (multi-GPU) context, r_list < r_c on the cell-list path, and an f32
+ * context of more than 2^24 atoms (the position records carry the atom index as an exact float). */
+typedef struct {
+    double a, gamma, sigma, r_c, dt;
+    uint64_t key;
+    int32_t use_neighbors;
+} mb_dpd_t;
+int mb_set_dpd(mb_ctx* ctx, const mb_dpd_t* p);
+
+/* forces(sys) of a system with a velocity-dependent pairwise term (mb_set_dpd): ADD the forces of all interactions (DPD +
+ * bonded) for coords and vels (n x 3 each, original order) at step step_n into fs_mat and, if non-NULL, the energy (the
+ * conservative DPD part + bonded) into pe. fs_mat may be NULL. On a DPD context mb_forces, mb_forces_energy and
+ * mb_forces_energy_all return MB_ERR_INVALID with a force output (they have no velocities) and with a virial output (DPD has
+ * no virial); mb_energy keeps working. */
+int mb_forces_energy_vel(mb_ctx* ctx, const void* coords, const void* vels, void* fs_mat, void* pe, int64_t step_n);
+
+/* simulate!(sys, DPDVelocityVerlet(dt, lambda; remove_CM_motion), n_steps) (src/simulators.jl:670-842), the Groot-Warren
+ * modified velocity Verlet. Prologue: wrap, CM removal when init_step == 0 and remove_cm_every != 0, neighbours, F0 at step
+ * init_step evaluated with the current velocities, loggers at init_step. Step n, with a = F/m:
+ *   1. v += a(t) dt/2
+ *   2. x += v dt; wrap
+ *   3. v_half = v; v_pred = v_half + (lambda - 1/2) dt a(t)
+ *   4. F(t + dt) = forces(x, v_pred) keyed by step n
+ *   5. v = v_half + a(t + dt) dt/2
+ *   6. CM removal when n % remove_cm_every == 0
+ *   7. neighbours; loggers (mb_log_t, as for mb_simulate_vv_log; NULL: no logging).
+ * One step is VelocityVerlet's launches: the drift kernel (which also stores v_pred), [rebuild or wrap], forces, bonded, the
+ * second kick. Each call's F0 uses v(t), not a v_pred, so a run split into calls differs from one call, as in the
+ * reference. On a context without mb_set_dpd the step is mb_simulate_vv's, bit for bit. Where the engine differs from the
+ * reference:
+ *  - the pairwise draw (mb_set_dpd);
+ *  - the neighbour rebuild is triggered by the exact displacement test after the drift (as for mb_simulate_vv);
+ *  - massless atoms (1/m = 0) get no kick.
+ * MB_ERR_INVALID before any work for dt <= 0, n_steps < 0, lambda not finite, a velocity coupling set on the context
+ * (mb_set_velocity_coupling), a decomposed (multi-GPU) context, the refusals of mb_set_dpd, and the logging errors of
+ * mb_simulate_vv_log. Every other integrator and the minimiser refuse a DPD context. MB_ERR_CAPACITY as in mb_simulate_vv. */
+typedef struct {
+    double dt;
+    int64_t n_steps;
+    int64_t init_step;
+    int32_t remove_cm_every;
+    double lambda;  /* the velocity prediction parameter (reference default 0.65) */
+} mb_dpd_vv_params_t;
+int mb_simulate_dpd_vv(mb_ctx* ctx, void* coords, void* vels, const mb_dpd_vv_params_t* p, mb_log_t* log);
+
 /* simulate!(sys, SteepestDescentMinimizer(step_size, max_steps, tol)) (src/simulators.jl:183-274) on the device: wrap the
  * coordinates, E = potential energy; then for step n = init_step+1 .. init_step+max_steps: F = forces, m = max |F_i|,
  * x <- wrap(x + h F / m), E_trial = potential energy; E_trial < E accepts (h <- 6h/5, E <- E_trial), otherwise x is restored

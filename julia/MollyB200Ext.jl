@@ -16,6 +16,7 @@
 #   Molly.simulate!(sys, sim::Verlet, n_steps; ...) with coupling nothing or one AndersenThermostat           simulators.jl:868
 #   Molly.simulate!(sys, sim::StormerVerlet, n_steps; ...)                                                   simulators.jl:970
 #   Molly.simulate!(sys, sim::OverdampedLangevin, n_steps; ...)                                              simulators.jl:1427
+#   Molly.simulate!(sys, sim::DPDVelocityVerlet, n_steps; ...) with coupling === nothing                     simulators.jl:711
 # (Molly.remove_CM_motion! for CuArray Systems is NOT redefined: the stock extension owns that exact signature)
 # and falls through to the stock methods (invoke) for anything it does not recognise: non-cubic boundaries,
 # constraints, virtual sites, couplings other than one AndersenThermostat, ImmediateThermostat, BerendsenThermostat or
@@ -60,6 +61,24 @@ struct MBVVParams
     andersen_prob::Float64
     rng_ctr1::UInt64
     rng_key::UInt64
+end
+
+# mb_dpd_t (mb_set_dpd) and mb_dpd_vv_params_t (mb_simulate_dpd_vv)
+struct MBDpd
+    a::Float64
+    gamma::Float64
+    sigma::Float64
+    r_c::Float64
+    dt::Float64
+    key::UInt64
+    use_neighbors::Int32
+end
+struct MBDpdVVParams
+    dt::Float64
+    n_steps::Int64
+    init_step::Int64
+    remove_cm_every::Int32
+    lambda::Float64
 end
 
 # mb_langevin_params_t (mb_simulate_langevin)
@@ -222,6 +241,24 @@ mutable struct Context
 end
 const CONTEXTS = IdDict{Any, Context}()
 
+# a pairwise tuple of exactly one DPDInteraction (src/interactions/dpd.jl): the engine runs it through mb_set_dpd, with no
+# mb_inter_t. engine_eligible has no descriptor for it, so every integrator takeover leaves a DPD System to the stock method;
+# only the pairwise seams and the DPDVelocityVerlet method ask dpd_eligible instead.
+dpd_only(inters) = inters isa Tuple && length(inters) == 1 && inters[1] isa DPDInteraction
+# DPD runs in reduced units: parameters with Unitful units are not taken over (nothing)
+function dpd_desc(d::DPDInteraction)
+    all(x -> x isa Real, (d.a, d.γ, d.σ, d.r_c, d.dt)) || return nothing
+    return MBDpd(Float64(d.a), Float64(d.γ), Float64(d.σ), Float64(d.r_c), Float64(d.dt), UInt64(d.key), Int32(d.use_neighbors))
+end
+# set the tuple's DPDInteraction on the context, or clear it (every caller of context_for with the System's tuple)
+function set_dpd!(ctx, inters)
+    if dpd_only(inters)
+        check(ccall((:mb_set_dpd, LIB), Cint, (Ptr{Cvoid}, Ref{MBDpd}), ctx.handle, Ref(dpd_desc(inters[1]))))
+    else
+        check(ccall((:mb_set_dpd, LIB), Cint, (Ptr{Cvoid}, Ptr{MBDpd}), ctx.handle, C_NULL))
+    end
+end
+
 function engine_eligible(sys::System{3, <:CuArray, T}, inters) where T
     T in (Float32, Float64) || return nothing
     (sys.boundary isa CubicBoundary || sys.boundary isa TriclinicBoundary{3, <:Any, <:Any, true}) || return nothing
@@ -232,7 +269,14 @@ function engine_eligible(sys::System{3, <:CuArray, T}, inters) where T
     return collect(MBInter, descs)
 end
 
-function context_for(sys::System{3, <:CuArray, T}, descs::Vector{MBInter}) where T
+# the System-level conditions of engine_eligible (no pairwise interaction to describe) and a unitless lone DPDInteraction:
+# an empty descriptor list for context_for, or nothing
+function dpd_eligible(sys::System{3, <:CuArray}, inters)
+    dpd_only(inters) && !isnothing(dpd_desc(inters[1])) || return nothing
+    return engine_eligible(sys, ())
+end
+
+function context_for(sys::System{3, <:CuArray, T}, descs::Vector{MBInter}, inters=sys.pairwise_inters) where T
     nf = sys.neighbor_finder
     gen = nf isa GPUNeighborFinder ? nf.cache_generation : 0
     ctx = get(CONTEXTS, sys.atoms, nothing)
@@ -266,13 +310,14 @@ function context_for(sys::System{3, <:CuArray, T}, descs::Vector{MBInter}) where
         CONTEXTS[sys.atoms] = ctx
     end
     check(ccall((:mb_set_inters, LIB), Cint, (Ptr{Cvoid}, Cint, Ptr{MBInter}), ctx.handle, length(descs), descs))
+    set_dpd!(ctx, inters)
     return ctx
 end
 
 # ---- forces / energy seam -----------------------------------------------------------------------------
 function Molly.pairwise_forces_loop_gpu!(buffers, sys::System{3, <:CuArray, T}, pairwise_inters::Tuple,
                                          nbs::Nothing, ::Val{needs_vir}, step_n) where {T, needs_vir}
-    descs = engine_eligible(sys, pairwise_inters)
+    descs = dpd_only(pairwise_inters) ? dpd_eligible(sys, pairwise_inters) : engine_eligible(sys, pairwise_inters)
     if isnothing(descs)
         # the STOCK method's own signature (ext/MollyCUDAExt.jl:845: System{D, <:CuArray, T}, untyped pairwise_inters);
         # naming this method's System{3, ...} signature here would recurse into itself
@@ -280,7 +325,20 @@ function Molly.pairwise_forces_loop_gpu!(buffers, sys::System{3, <:CuArray, T}, 
                       Tuple{Any, System{D, <:CuArray, T} where D, Any, Nothing, Val{needs_vir}, Any},
                       buffers, sys, pairwise_inters, nbs, Val(needs_vir), step_n)
     end
-    ctx = context_for(sys, descs)
+    ctx = context_for(sys, descs, pairwise_inters)
+    if dpd_only(pairwise_inters)
+        # the forces depend on the velocities and the step (pairwise_uses_velocity, src/types.jl:50-59). The call adds the
+        # context's bonded forces too, so a System with specific lists takes the stock method instead; no virial.
+        if !isempty(sys.specific_inter_lists) || needs_vir
+            return invoke(Molly.pairwise_forces_loop_gpu!,
+                          Tuple{Any, System{D, <:CuArray, T} where D, Any, Nothing, Val{needs_vir}, Any},
+                          buffers, sys, pairwise_inters, nbs, Val(needs_vir), step_n)
+        end
+        check(ccall((:mb_forces_energy_vel, LIB), Cint,
+                    (Ptr{Cvoid}, CuPtr{Cvoid}, CuPtr{Cvoid}, CuPtr{Cvoid}, CuPtr{Cvoid}, Int64),
+                    ctx.handle, pointer(sys.coords), pointer(sys.velocities), pointer(buffers.fs_mat), CU_NULL, step_n))
+        return buffers
+    end
     vir = needs_vir ? pointer(buffers.virial_nounits) : CU_NULL
     # contract: ADD into buffers.fs_mat (D x N, original order) and buffers.virial_nounits
     check(ccall((:mb_forces, LIB), Cint, (Ptr{Cvoid}, CuPtr{Cvoid}, CuPtr{Cvoid}, CuPtr{Cvoid}, Int64),
@@ -290,13 +348,13 @@ end
 
 function Molly.pairwise_pe_loop_gpu!(pe_vec_nounits, buffers, sys::System{3, <:CuArray, T}, pairwise_inters::Tuple,
                                      nbs::Nothing, step_n) where T
-    descs = engine_eligible(sys, pairwise_inters)
+    descs = dpd_only(pairwise_inters) ? dpd_eligible(sys, pairwise_inters) : engine_eligible(sys, pairwise_inters)
     if isnothing(descs)
         return invoke(Molly.pairwise_pe_loop_gpu!,   # stock: ext/MollyCUDAExt.jl:936
                       Tuple{Any, Any, System{D, <:CuArray, T} where D, Any, Nothing, Any},
                       pe_vec_nounits, buffers, sys, pairwise_inters, nbs, step_n)
     end
-    ctx = context_for(sys, descs)
+    ctx = context_for(sys, descs, pairwise_inters)
     check(ccall((:mb_energy, LIB), Cint, (Ptr{Cvoid}, CuPtr{Cvoid}, CuPtr{Cvoid}, Int64),
                 ctx.handle, pointer(sys.coords), pointer(pe_vec_nounits), step_n))
     return pe_vec_nounits
@@ -669,6 +727,36 @@ function Molly.simulate!(sys::System{3, <:CuArray, T}, sim::Verlet, n_steps::Int
         end
     end
     check(ccall((:mb_simulate_verlet, LIB), Cint, (Ptr{Cvoid}, CuPtr{Cvoid}, CuPtr{Cvoid}, Ref{MBVVParams}, Ptr{MBLog}),
+                ctx.handle, pointer(sys.coords), pointer(sys.velocities), Ref(p), C_NULL))
+    return sys
+end
+
+# ---- simulate!(sys, ::DPDVelocityVerlet, n) (src/simulators.jl:711-842) ---------------------------------------------------
+# Taken over when the coupling is nothing and the System is eligible as for Verlet with a pairwise tuple of exactly one
+# unitless DPDInteraction (dpd_eligible): one mb_simulate_dpd_vv call. Every other integrator leaves a DPD System to its
+# stock method (engine_eligible has no DPD descriptor), whose force loop still goes through the DPD seam above. Anything
+# else runs the stock method.
+function Molly.simulate!(sys::System{3, <:CuArray, T}, sim::DPDVelocityVerlet, n_steps::Integer;
+                         init_step=0, rng=Random.default_rng(), run_loggers=true, kwargs...) where T
+    descs = dpd_eligible(sys, sys.pairwise_inters)
+    if isnothing(descs) || !isnothing(sim.coupling) || !plain_takeover_ok(sys, descs, run_loggers) ||
+            !isempty(sys.general_inters)
+        # stock: simulate!(sys, sim::DPDVelocityVerlet, n_steps_or_time; ...) src/simulators.jl:711
+        return invoke(Molly.simulate!, Tuple{Any, DPDVelocityVerlet, Any}, sys, sim, n_steps;
+                      init_step=init_step, rng=rng, run_loggers=run_loggers, kwargs...)
+    end
+    ctx = context_for(sys, descs)
+    set_specific!(ctx, sys)
+    set_implicit_solvent!(ctx, sys)
+    set_velocity_coupling!(ctx, nothing)
+    p = MBDpdVVParams(_ps(sim.dt), n_steps, init_step, Int32(sim.remove_CM_motion), Float64(sim.λ))
+    if run_loggers != false && !isempty(sys.loggers)
+        return simulate_logged!(sys, ctx, n_steps, init_step, run_loggers) do lg
+            ccall((:mb_simulate_dpd_vv, LIB), Cint, (Ptr{Cvoid}, CuPtr{Cvoid}, CuPtr{Cvoid}, Ref{MBDpdVVParams}, Ref{MBLog}),
+                  ctx.handle, pointer(sys.coords), pointer(sys.velocities), Ref(p), lg)
+        end
+    end
+    check(ccall((:mb_simulate_dpd_vv, LIB), Cint, (Ptr{Cvoid}, CuPtr{Cvoid}, CuPtr{Cvoid}, Ref{MBDpdVVParams}, Ptr{MBLog}),
                 ctx.handle, pointer(sys.coords), pointer(sys.velocities), Ref(p), C_NULL))
     return sys
 end

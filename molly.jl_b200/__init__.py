@@ -10,7 +10,7 @@ from .api import (Atom, CubicBoundary, TriclinicBoundary, System, NoCutoff, Dist
                   ShiftedForceCutoff, LennardJones, Coulomb, CoulombReactionField, CoulombEwald, GPUNeighborFinder,
                   DistanceNeighborFinder, CellListMapNeighborFinder, TreeNeighborFinder, AndersenThermostat,
                   ImmediateThermostat, BerendsenThermostat, VelocityRescaleThermostat,
-                  VelocityVerlet, Langevin, LangevinSplitting, NoseHoover, Verlet, StormerVerlet, OverdampedLangevin, MTSIntegrator, MTSLangevinIntegrator, setup_mts_integrator,
+                  VelocityVerlet, Langevin, LangevinSplitting, NoseHoover, Verlet, StormerVerlet, OverdampedLangevin, DPDInteraction, DPDVelocityVerlet, MTSIntegrator, MTSLangevinIntegrator, setup_mts_integrator,
                   mts_levels, forces, forces_virial, potential_energy, forces_energy, find_neighbors, simulate,
                   kinetic_energy, temperature, remove_CM_motion, random_velocities, wrap_coords, device_count,
                   atoms_from_arrays, atoms_to_array, atom_dtype, MollyB200Error, COULOMB_CONST, BOLTZMANN_K,

@@ -24,6 +24,7 @@ EXPORTED = [
     "mb_simulate_vv_log", "mb_minimize_sd", "mb_set_velocity_coupling", "mb_simulate_langevin",
     "mb_simulate_nose_hoover", "mb_set_specific_levels", "mb_simulate_mts", "mb_set_implicit_solvent",
     "mb_simulate_langevin_splitting", "mb_simulate_verlet", "mb_simulate_stormer_verlet", "mb_simulate_overdamped_langevin",
+    "mb_set_dpd", "mb_forces_energy_vel", "mb_simulate_dpd_vv",
 ]
 MB_GB_MAX_NECK_CLASSES = 32
 # specific interaction kinds of mb_set_specific (include/mollyb200.h)
@@ -68,6 +69,20 @@ class MBVVParams(C.Structure):
     _fields_ = [
         ("dt", C.c_double), ("n_steps", C.c_int64), ("init_step", C.c_int64), ("remove_cm_every", C.c_int32),
         ("andersen_kT", C.c_double), ("andersen_prob", C.c_double), ("rng_ctr1", C.c_uint64), ("rng_key", C.c_uint64),
+    ]
+
+
+class MBDpd(C.Structure):
+    _fields_ = [
+        ("a", C.c_double), ("gamma", C.c_double), ("sigma", C.c_double), ("r_c", C.c_double), ("dt", C.c_double),
+        ("key", C.c_uint64), ("use_neighbors", C.c_int32),
+    ]
+
+
+class MBDpdVVParams(C.Structure):
+    _fields_ = [
+        ("dt", C.c_double), ("n_steps", C.c_int64), ("init_step", C.c_int64), ("remove_cm_every", C.c_int32),
+        ("lambda_", C.c_double),
     ]
 
 
@@ -169,6 +184,9 @@ def load():
     L.mb_simulate_verlet.argtypes = [vp, vp, vp, C.POINTER(MBVVParams), C.POINTER(MBLog)]
     L.mb_simulate_stormer_verlet.argtypes = [vp, vp, vp, C.POINTER(MBStormerParams), C.POINTER(MBLog)]
     L.mb_simulate_overdamped_langevin.argtypes = [vp, vp, vp, C.POINTER(MBLangevinParams), C.POINTER(MBLog)]
+    L.mb_set_dpd.argtypes = [vp, C.POINTER(MBDpd)]
+    L.mb_forces_energy_vel.argtypes = [vp, vp, vp, vp, vp, i64]
+    L.mb_simulate_dpd_vv.argtypes = [vp, vp, vp, C.POINTER(MBDpdVVParams), C.POINTER(MBLog)]
     L.mb_set_specific_levels.argtypes = [vp, C.c_int, i64, vp]
     L.mb_minimize_sd.argtypes = [vp, vp, C.POINTER(MBSDParams)]
     L.mb_set_velocity_coupling.argtypes = [vp, C.POINTER(MBVCoupling)]

@@ -17,6 +17,8 @@ julia/MollyB200Ext.jl, see INTEGRATION.md):
     NoseHoover                                      src/simulators.jl:1491-1614 (mb_simulate_nose_hoover)
     Verlet, StormerVerlet                           src/simulators.jl:858-1063 (mb_simulate_verlet, mb_simulate_stormer_verlet)
     OverdampedLangevin                              src/simulators.jl:1400-1490 (mb_simulate_overdamped_langevin)
+    DPDInteraction, DPDVelocityVerlet               src/interactions/dpd.jl:57-142, src/simulators.jl:670-842 (mb_set_dpd,
+                                                    mb_simulate_dpd_vv, mb_forces_energy_vel)
     MTSIntegrator, MTSLangevinIntegrator            src/simulators.jl:1616-1940 (mb_simulate_mts)
     forces, forces_virial, potential_energy         src/force.jl:678-720, src/energy.jl:202-248
     kinetic_energy, temperature, remove_CM_motion   src/energy.jl:44-175, src/spatial.jl:901-929
@@ -232,6 +234,49 @@ class CoulombEwald:
         alpha = np.sqrt(-np.log(2 * self.error_tol)) / self.dist_cutoff
         return capi.MBInter(capi.MB_EWALD_REAL, capi.MB_CUT_DISTANCE, self.dist_cutoff, 0.0, self.weight_special,
                             self.coulomb_const, 1.0, float(alpha), 0, 1, int(self.approximate_erfc), int(self.use_neighbors))
+
+
+@dataclass
+class DPDInteraction:
+    """DPDInteraction(a, gamma, sigma, r_c, dt, use_neighbors, key) — src/interactions/dpd.jl:57-142, the pairwise
+    interaction of dissipative particle dynamics (conservative, dissipative and random forces), run on the device through
+    mb_set_dpd (see include/mollyb200.h). gamma and sigma are the reference's γ and σ (σ² = 2 γ kT for temperature T); dt
+    is the step the random force is scaled for (dt^(-1/2)). key=None draws one. It must be the System's only pairwise
+    interaction; forces(sys) then uses sys.velocities, and simulate runs it under DPDVelocityVerlet only."""
+    a: float = 25.0
+    gamma: float = 4.5
+    sigma: float = 3.0
+    r_c: float = 1.0
+    dt: float = 0.01
+    use_neighbors: bool = False
+    key: Optional[int] = None
+
+    def __post_init__(self):
+        if not (math.isfinite(self.r_c) and self.r_c > 0):
+            raise ValueError(f"r_c must be finite and positive, found {self.r_c}")
+        if not (math.isfinite(self.dt) and self.dt > 0):
+            raise ValueError(f"dt must be finite and positive, found {self.dt}")
+        for name in ("gamma", "sigma"):
+            v = getattr(self, name)
+            if not (math.isfinite(v) and v >= 0):
+                raise ValueError(f"{name} must be finite and non-negative, found {v}")
+        if not math.isfinite(self.a):
+            raise ValueError(f"a must be finite, found {self.a}")
+        if self.key is None:
+            self.key = int(np.random.default_rng().integers(0, 2 ** 64, dtype=np.uint64))
+        if not (_is_integer(self.key) and 0 <= int(self.key) < 2 ** 64):
+            raise ValueError(f"key must be an integer in [0, 2^64), found {self.key!r}")
+        self.key = int(self.key)
+
+    def dpd_descriptor(self):
+        return capi.MBDpd(float(self.a), float(self.gamma), float(self.sigma), float(self.r_c), float(self.dt), self.key,
+                          int(bool(self.use_neighbors)))
+
+
+def _dpd_of(sys):
+    """The System's DPDInteraction, or None."""
+    d = [it for it in sys.pairwise_inters if isinstance(it, DPDInteraction)]
+    return d[0] if d else None
 
 
 def _pairs_from(obj, n, want_true: bool):
@@ -795,6 +840,24 @@ class OverdampedLangevin:
         _check_remove_cm(self)
 
 
+@dataclass
+class DPDVelocityVerlet:
+    """DPDVelocityVerlet(dt, lam=0.65; coupling=None, remove_CM_motion=1) — src/simulators.jl:670-842, the Groot-Warren
+    modified velocity Verlet, run on the device by mb_simulate_dpd_vv (see include/mollyb200.h). lam is the reference's λ:
+    the forces of step t + dt are evaluated with v_pred = v(t + dt/2) + (λ - 1/2) dt a(t). No coupling is supported
+    (simulate raises TypeError for one)."""
+    dt: float
+    lam: float = 0.65
+    coupling: object = None
+    remove_CM_motion: int = 1
+
+    def __post_init__(self):
+        _check_dt(self.dt)
+        if not math.isfinite(self.lam):
+            raise ValueError(f"lam must be finite, found {self.lam}")
+        _check_remove_cm(self)
+
+
 def _is_integer(x) -> bool:
     return isinstance(x, (int, np.integer))
 
@@ -1106,9 +1169,13 @@ class System:
         else:
             side = (C.c_double * 3)(*self.boundary.side_lengths)
             capi.check(L.mb_set_box(ctx, side))
-        descs = [it.descriptor() for it in self.pairwise_inters]
+        dpd = [it for it in self.pairwise_inters if isinstance(it, DPDInteraction)]
+        if len(dpd) > 1:
+            raise ValueError("at most one DPDInteraction per System")
+        descs = [it.descriptor() for it in self.pairwise_inters if not isinstance(it, DPDInteraction)]
         arr = (capi.MBInter * max(1, len(descs)))(*descs)
         capi.check(L.mb_set_inters(ctx, len(descs), arr))
+        capi.check(L.mb_set_dpd(ctx, C.byref(dpd[0].dpd_descriptor()) if dpd else None))
         nf = self.neighbor_finder
         if nf is not None:
             if nf.excluded_pairs is not None:
@@ -1215,10 +1282,13 @@ def _evaluate(call, *outputs):
 
 
 def forces(sys: System, neighbors=None, step_n: int = 0) -> np.ndarray:
-    """forces(sys[, neighbors, step_n]) — src/force.jl:678-687. Returns (n,3) in kJ mol^-1 nm^-1."""
+    """forces(sys[, neighbors, step_n]) — src/force.jl:678-687. Returns (n,3) in kJ mol^-1 nm^-1. With a DPDInteraction the
+    forces are those of sys.velocities and of the draws of step step_n (mb_forces_energy_vel)."""
     ctx = sys.engine()
     fs = np.zeros((sys.n, 3), sys.dtype)
-    if sys.specific_inter_lists or sys.general_inters:  # forces(sys) sums pairwise + specific + general interactions
+    if _dpd_of(sys) is not None:
+        _evaluate(lambda: sys._L.mb_forces_energy_vel(ctx, _ptr(sys.coords), _ptr(sys.velocities), fs.ctypes.data, None, step_n), fs)
+    elif sys.specific_inter_lists or sys.general_inters:  # forces(sys) sums pairwise + specific + general interactions
         _evaluate(lambda: sys._L.mb_forces_energy_all(ctx, _ptr(sys.coords), fs.ctypes.data, None, step_n), fs)
     else:
         _evaluate(lambda: sys._L.mb_forces(ctx, _ptr(sys.coords), fs.ctypes.data, None, step_n), fs)
@@ -1253,7 +1323,10 @@ def forces_energy(sys: System, step_n: int = 0):
     ctx = sys.engine()
     fs = np.zeros((sys.n, 3), sys.dtype)
     pe = np.zeros(1, sys.dtype)
-    if sys.specific_inter_lists or sys.general_inters:
+    if _dpd_of(sys) is not None:
+        _evaluate(lambda: sys._L.mb_forces_energy_vel(ctx, _ptr(sys.coords), _ptr(sys.velocities), fs.ctypes.data, pe.ctypes.data,
+                                                      step_n), fs, pe)
+    elif sys.specific_inter_lists or sys.general_inters:
         _evaluate(lambda: sys._L.mb_forces_energy_all(ctx, _ptr(sys.coords), fs.ctypes.data, pe.ctypes.data, step_n), fs, pe)
     else:
         _evaluate(lambda: sys._L.mb_forces_energy(ctx, _ptr(sys.coords), fs.ctypes.data, pe.ctypes.data, None, step_n), fs, pe)
@@ -1325,6 +1398,7 @@ _SIMULATE_ENTRY = {
     Verlet: (capi.MBVVParams, "mb_simulate_verlet"),
     StormerVerlet: (capi.MBStormerParams, "mb_simulate_stormer_verlet"),
     OverdampedLangevin: (capi.MBLangevinParams, "mb_simulate_overdamped_langevin"),
+    DPDVelocityVerlet: (capi.MBDpdVVParams, "mb_simulate_dpd_vv"),
 }
 
 
@@ -1346,6 +1420,8 @@ def simulate(sys: System, sim, n_steps: Optional[int] = None, init_step: int = 0
     Verlet, StormerVerlet, OverdampedLangevin: simulate!(sys, sim, n_steps; run_loggers=true) — src/simulators.jl:868-955,
     :970-1063, :1427-1490, the same arguments and loggers as VelocityVerlet. Verlet's velocities are half a step behind the
     positions; StormerVerlet's first step of every call starts from the velocities.
+    DPDVelocityVerlet: simulate!(sys, sim, n_steps; run_loggers=true) — src/simulators.jl:711-842, the same arguments and
+    loggers as VelocityVerlet; each call's first force evaluation uses the current velocities.
     SteepestDescentMinimizer: simulate!(sys, sim; run_loggers=false) — src/simulators.jl:183-274, see steepest_descent.
     Loggers are not run during a minimisation (run_loggers must be false)."""
     if isinstance(sim, SteepestDescentMinimizer):
@@ -1400,6 +1476,8 @@ def simulate(sys: System, sim, n_steps: Optional[int] = None, init_step: int = 0
         p.ops = sim.splitting.encode()
     if isinstance(sim, NoseHoover):
         p.damping = float(sim.damping)
+    if isinstance(sim, DPDVelocityVerlet):
+        p.lambda_ = float(sim.lam)
     p.dt = float(sim.dt)
     p.n_steps = int(n_steps)
     p.init_step = int(init_step)
@@ -1410,7 +1488,7 @@ def simulate(sys: System, sim, n_steps: Optional[int] = None, init_step: int = 0
     if mts:  # (an unchanged level array leaves the context as it is)
         for kind, lv in levels.items():
             capi.check(sys._L.mb_set_specific_levels(ctx, kind, len(lv), lv.ctypes.data))
-    if not isinstance(sim, (NoseHoover, StormerVerlet)):  # (these two draw nothing)
+    if not isinstance(sim, (NoseHoover, StormerVerlet, DPDVelocityVerlet)):  # (these draw nothing of their own)
         rng = rng or np.random.default_rng()
         p.rng_ctr1 = int(rng.integers(0, 2 ** 63))
         p.rng_key = int(rng.integers(0, 2 ** 63))

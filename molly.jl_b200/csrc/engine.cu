@@ -320,9 +320,10 @@ static void pme_plan_host(const double box[3], double r_cut, double error_tol, i
 
 // The integrator of one simulate call: VelocityVerlet (vv.cuh), Langevin (langevin.cuh), Nose-Hoover (nosehoover.cuh), the
 // multiple-time-step integrators (mts.cuh), LangevinSplitting (splitting.cuh), or Verlet, StormerVerlet and
-// OverdampedLangevin (verlet.cuh). Each mb_simulate_* entry point fills one from its own parameters.
+// OverdampedLangevin (verlet.cuh), or DPDVelocityVerlet (vv.cuh's step with the DPD drift, dpd.cuh). Each mb_simulate_* entry
+// point fills one from its own parameters.
 enum { INTEG_VV = 0, INTEG_LANGEVIN = 1, INTEG_NH = 2, INTEG_MTS = 3, INTEG_MTS_LANGEVIN = 4, INTEG_SPLIT = 5, INTEG_VERLET = 6,
-       INTEG_STORMER = 7, INTEG_OVERDAMPED = 8 };
+       INTEG_STORMER = 7, INTEG_OVERDAMPED = 8, INTEG_DPD_VV = 9 };
 static_assert(SPLIT_MAX_OPS == MB_SPLIT_MAX_OPS, "splitting length");
 static bool is_mts(int kind) { return kind == INTEG_MTS || kind == INTEG_MTS_LANGEVIN; }
 struct Integrator {
@@ -339,11 +340,12 @@ struct Integrator {
     std::array<int, MTS_MAX_LEVELS> fractions = {};
     int n_ops = 0;                              // LangevinSplitting's splitting: the letters 'A', 'B', 'O' (0: none)
     std::array<char, SPLIT_MAX_OPS> ops = {};
+    double lambda = 0;                          // DPDVelocityVerlet's velocity prediction parameter
     // What the step graphs bake in (GraphKey): every field but n_steps, init_step and the RNG keys, which are uploaded
     // into Control on every call
     auto graph_fields() const {
         return std::tie(kind, dt, remove_cm_every, andersen_kT, andersen_prob, kT, friction, damping, n_levels, fractions, n_ops,
-                        ops);
+                        ops, lambda);
     }
 };
 
@@ -415,7 +417,8 @@ class EngineBase {
     virtual int set_exceptions(int64_t ne, const int32_t* ei, const int32_t* ej, int64_t ns, const int32_t* si,
                                const int32_t* sj) = 0;
     virtual int set_neighbor_policy(double r_list, int rebuild_every) = 0;
-    virtual int forces_energy(const void* coords, void* fs, void* pe, void* vir, int64_t step_n, bool with_specific) = 0;
+    virtual int forces_energy(const void* coords, void* fs, void* pe, void* vir, int64_t step_n, bool with_specific,
+                              const void* vels) = 0;
     virtual int simulate(void* coords, void* vels, const Integrator& ig, mb_log_t* log) = 0;
     virtual int remove_cm(void* vels) = 0;
     virtual int kinetic_energy(const void* vels, double* out) = 0;
@@ -435,6 +438,7 @@ class EngineBase {
     virtual int random_velocities(void* vels, double kT, uint64_t ctr1, uint64_t key) = 0;
     virtual int kinetic_tensor(const void* vels, double* out9) = 0;
     virtual int minimize_sd(void* coords, mb_sd_params_t* p) = 0;
+    virtual int set_dpd(const mb_dpd_t* p) = 0;
     mb_vcoupling_t vcoupling = {MB_VC_NONE, 0, 0.0, 0.0};  // mb_set_velocity_coupling (validated there)
 };
 
@@ -642,9 +646,10 @@ class Engine : public EngineBase {
         if (!(box_[0] > 0)) return set_error(MB_ERR_STATE, "box not set");
         if (n_ > 2000000000LL) return set_error(MB_ERR_INVALID, "too many atoms");
         memset(&P_, 0, sizeof(P_));
+        MB_TRY(check_dpd());
         const double inf = std::numeric_limits<double>::infinity();
-        bool all_nl = !inters_.empty();
-        double max_rc = 0;
+        bool all_nl = dpd_on_ ? dpd_.use_neighbors != 0 : !inters_.empty();  // (a DPD context has no mb_inter_t: check_dpd)
+        double max_rc = dpd_on_ ? dpd_.r_c : 0;
         bool any_nocut_nl = false;
         for (auto& in : inters_) {
             if (!in.use_neighbors) all_nl = false;
@@ -733,7 +738,7 @@ class Engine : public EngineBase {
             if (h_sigma_[i] != h_sigma_[0] || h_eps_[i] != h_eps_[0]) uniform = false;
         }
         if (!P_.has_lj || h_sigma_[0] == (T)0 || h_eps_[0] == (T)0) uniform = uniform && !P_.has_lj;
-        P_.uniform_lj = (uniform && P_.coul_kind == COUL_NONE) ? 1 : 0;
+        P_.uniform_lj = ((uniform || dpd_on_) && P_.coul_kind == COUL_NONE) ? 1 : 0;  // (DPD stages positions only)
         if (P_.uniform_lj) {
             P_.uni_sig2 = P_.has_lj ? h_sigma_[0] * h_sigma_[0] : (T)0;
             P_.uni_eps = P_.has_lj ? h_eps_[0] : (T)0;
@@ -750,9 +755,15 @@ class Engine : public EngineBase {
         MB_CUDA(d_charge_in_.ensure(np * sizeof(T)));
         MB_CUDA(d_ljp_in_.ensure(np * sizeof(T2)));
         MB_CUDA(cudaMemcpyAsync(d_mass_in_.p, h_mass_.data(), n_ * sizeof(T), cudaMemcpyHostToDevice, stream_));
-        MB_CUDA(cudaMemcpyAsync(d_charge_in_.p, h_charge_.data(), n_ * sizeof(T), cudaMemcpyHostToDevice, stream_));
+        // a DPD context's position records carry the original index (exact up to 2^24 in f32: check_dpd) in place of the charge
+        std::vector<T> index_w;
+        if (dpd_on_) {
+            index_w.resize(n_);
+            for (int64_t i = 0; i < n_; i++) index_w[i] = (T)i;
+        }
+        MB_CUDA(cudaMemcpyAsync(d_charge_in_.p, dpd_on_ ? index_w.data() : h_charge_.data(), n_ * sizeof(T), cudaMemcpyHostToDevice, stream_));
         MB_CUDA(cudaMemcpyAsync(d_ljp_in_.p, ljp.data(), n_ * sizeof(T2), cudaMemcpyHostToDevice, stream_));
-        MB_CUDA(cudaStreamSynchronize(stream_));  // ljp is a local
+        MB_CUDA(cudaStreamSynchronize(stream_));  // ljp and index_w are locals
         // slot-order state
         MB_CUDA(d_pos4_.ensure(np * sizeof(T4)));
         MB_CUDA(d_vel4_.ensure(np * sizeof(T4)));
@@ -774,6 +785,13 @@ class Engine : public EngineBase {
         MB_CUDA(d_stage_b_.ensure(3 * np * sizeof(T)));
         MB_CUDA(d_stage_c_.ensure(3 * np * sizeof(T)));
         MB_CUDA(d_scalars_.ensure(10 * sizeof(T)));  // [pe, vir(9)] of forces_energy
+        if (dpd_on_) {
+            MB_CUDA(d_vpred4_.ensure(np * sizeof(T4)));
+            MB_CUDA(cudaMemsetAsync(d_vpred4_.p, 0, np * sizeof(T4), stream_));
+            const DpdArgs<T> da = dpd_args();  // (the buffers it points at are allocated above)
+            MB_CUDA(d_dpd_args_.ensure(sizeof(da)));
+            MB_CUDA(cudaMemcpy(d_dpd_args_.p, &da, sizeof(da), cudaMemcpyHostToDevice));
+        }
         // exclusion CSR
         auto up = [&](DevBuf& b, const std::vector<int>& v) -> cudaError_t {
             if (v.empty()) return cudaSuccess;
@@ -907,7 +925,7 @@ class Engine : public EngineBase {
         const size_t stage = force_stage();
         const size_t sm_total = smem_optin_ + 1024;  // 228 KB per SM, 1 KB reserved per resident CTA
         const size_t static_bytes = 1024;
-        ctas_per_sm = (sizeof(T) == 8) ? 1 : FORCE_CTAS_F32;
+        ctas_per_sm = (sizeof(T) == 8 || dpd_on_) ? 1 : FORCE_CTAS_F32;  // (the DPD variants are compiled for one CTA per SM)
         while (ctas_per_sm > 1 && (sm_total / ctas_per_sm - 1024 - static_bytes) / stage < 1) ctas_per_sm--;
         const size_t budget = (ctas_per_sm > 1) ? sm_total / ctas_per_sm - 1024 - static_bytes : smem_optin_ - static_bytes;
         nbuf = (int)std::min<size_t>(FORCE_MAX_STAGES, std::max<size_t>(1, budget / stage));
@@ -1221,6 +1239,54 @@ class Engine : public EngineBase {
         disp_rc_ = r_cut;
         disp_ready_ = false;
         return MB_OK;
+    }
+    // ---- DPDInteraction (dpd.cuh): replaces the pairwise interactions; prepare() digests it and picks the path -------------
+    int set_dpd(const mb_dpd_t* p) override {
+        const std::string who = "mb_set_dpd: ";
+        if (p) {
+            if (!(std::isfinite(p->r_c) && p->r_c > 0)) return set_error(MB_ERR_INVALID, who + "r_c must be finite and > 0");
+            if (!(std::isfinite(p->dt) && p->dt > 0)) return set_error(MB_ERR_INVALID, who + "dt must be finite and > 0");
+            if (!(std::isfinite(p->gamma) && p->gamma >= 0)) return set_error(MB_ERR_INVALID, who + "gamma must be finite and >= 0");
+            if (!(std::isfinite(p->sigma) && p->sigma >= 0)) return set_error(MB_ERR_INVALID, who + "sigma must be finite and >= 0");
+            if (!std::isfinite(p->a)) return set_error(MB_ERR_INVALID, who + "a must be finite");
+            dpd_ = *p;
+        }
+        if (dpd_on_ || p) dirty_ = true;  // (prepare drops the graphs: they bake the DPD constants in)
+        dpd_on_ = p != nullptr;
+        return MB_OK;
+    }
+    // What a DPD context cannot be combined with; checked before every evaluation and simulate call
+    int check_dpd() const {
+        if (!dpd_on_) return MB_OK;
+        const std::string who = "DPDInteraction (mb_set_dpd): ";
+        if (!inters_.empty()) return set_error(MB_ERR_INVALID, who + "cannot be combined with other pairwise interactions (mb_set_inters)");
+        if (pme_on_ || disp_rc_ > 0 || gb_on_)
+            return set_error(MB_ERR_INVALID, who + "cannot be combined with PME, LJDispersionCorrection or implicit solvent");
+        if (decomposed()) return set_error(MB_ERR_INVALID, who + "not available in decomposed (multi-GPU) runs");
+        if (sizeof(T) == 4 && n_ > (1 << 24))
+            return set_error(MB_ERR_INVALID, who + "an f32 context holds at most 2^24 atoms (the position records carry the atom index as a float)");
+        return MB_OK;
+    }
+    // The brick kernel's DPD variant takes the address of its DpdArgs (uploaded by prepare) in place of the LJ parameters it
+    // does not stage; dpd_args_of reads it back. Only launch_dpd_pairs passes it.
+    const T2* dpd_args_as_lj2e() const { return reinterpret_cast<const T2*>(d_dpd_args_.p); }
+    DpdArgs<T> dpd_args() const {
+        DpdArgs<T> a;
+        memset(&a, 0, sizeof(a));
+        if (!dpd_on_) return a;
+        a.a = (T)dpd_.a;
+        a.gamma = (T)dpd_.gamma;
+        a.sigma = (T)dpd_.sigma;
+        a.rc = (T)dpd_.r_c;
+        a.inv_sqrt_dt = (T)(1.0 / std::sqrt(dpd_.dt));
+        a.e_pre = (T)(dpd_.a / 2) * (T)dpd_.r_c;
+        a.key_lo = (uint32_t)dpd_.key;
+        a.key_hi = (uint32_t)(dpd_.key >> 32);
+        a.nl = dpd_.use_neighbors ? 1 : 0;
+        a.dissipative = (dpd_.gamma != 0 || dpd_.sigma != 0) ? 1 : 0;
+        a.vpred = d_vpred4_.as<T4>();
+        a.step = &d_ctl_.as<Control>()->step;
+        return a;
     }
     // factor_6 / factor_12 of the constructor (:170-226): means over all i <= j pairs, N (N + 1) / 2 terms, Lorentz sigma
     // and geometric epsilon without the zero shortcut; accumulated in double, grouped by distinct (sigma, eps)
@@ -1765,6 +1831,9 @@ class Engine : public EngineBase {
         }
         out.pe_partial = d_pe_partial_.as<double>();
         out.vir_partial = out.pe_partial + vir_at;
+        if (dpd_on_) {
+            MB_TRY(launch_dpd_pairs(energy, f4, out, grid, smem, nbuf, b0, nbr));
+        } else {
         MB_TRY((with_const<COUL_NONE, COUL_PLAIN, COUL_CRF, COUL_EWALD>(P_.coul_kind, [&](auto COUL) {
             return with_const<CUTM_TWO_POINT, CUTM_SHIFTED, CUTM_PLAIN>(cutm_, [&](auto CUTM) {
                 return with_const<true, false>(energy, [&](auto EN) -> int {
@@ -1772,7 +1841,7 @@ class Engine : public EngineBase {
                         prof_.begin(Prof::FORCE);
                         allpairs_force_kernel<T, COUL, CUTM, EN><<<grid, AP_THREADS, 0, stream_>>>(
                             (int)n_, P_, (T)box_[0], (T)box_[1], (T)box_[2], tric_, d_pos4_.as<T4>(), d_lj2_.as<T2>(), ex_ptr_dev(),
-                            ex_idx_dev(), sp_ptr_dev(), sp_idx_dev(), f4, out.pe_partial, out.vir_partial);
+                            ex_idx_dev(), sp_ptr_dev(), sp_idx_dev(), f4, out.pe_partial, out.vir_partial, DpdArgs<T>{});
                         prof_.end(Prof::FORCE);
                         return MB_OK;
                     }
@@ -1791,11 +1860,34 @@ class Engine : public EngineBase {
                 });
             });
         })));
+        }
         launches_++;
         n_force_evals_++;
         MB_CUDA(cudaGetLastError());
         if (parts) *parts = Partials{out.pe_partial, out.vir_partial, grid};
         return MB_OK;
+    }
+
+    // The DPDInteraction variants of the two pair kernels (the launch shape of launch_pairs)
+    int launch_dpd_pairs(bool energy, T4* f4, const ForceOut<T>& out, int grid, size_t smem, int nbuf, int b0, int nbr) {
+        const DpdArgs<T> da = dpd_args();
+        return with_const<true, false>(energy, [&](auto EN) -> int {
+            prof_.begin(Prof::FORCE);
+            if (path_ == 0) {
+                allpairs_force_kernel<T, COUL_NONE, CUTM_PLAIN, EN, true><<<grid, AP_THREADS, 0, stream_>>>(
+                    (int)n_, P_, (T)box_[0], (T)box_[1], (T)box_[2], tric_, d_pos4_.as<T4>(), d_lj2_.as<T2>(), ex_ptr_dev(),
+                    ex_idx_dev(), sp_ptr_dev(), sp_idx_dev(), f4, out.pe_partial, out.vir_partial, da);
+            } else {
+                // (the kernel reads its DpdArgs through the LJ-parameter pointer: dpd_args_of, uploaded by prepare)
+                auto kern = brick_force_kernel<T, COUL_NONE, true, CUTM_PLAIN, EN, true>;
+                MB_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+                kern<<<grid, FORCE_THREADS, smem, stream_>>>(g_, P_, d_hdrs_.as<BrickHdr>(), d_runs_.as<Run>(), d_task_tab_.as<int2>(),
+                                                             d_pos4e_.as<T4>(), dpd_args_as_lj2e(), d_list_.as<unsigned short>(),
+                                                             d_slist_.as<unsigned short>(), out, b0, nbr, nbuf, d_sched_.as<unsigned int>());
+            }
+            prof_.end(Prof::FORCE);
+            return MB_OK;
+        });
     }
 
     // A caller's array in host or device memory, as the kernels see it (CallerBuf): for a host array the staging buffer
@@ -1880,10 +1972,16 @@ class Engine : public EngineBase {
     }
 
     // ------------------------------------------------------------------------------------------
-    int forces_energy(const void* coords, void* fs, void* pe, void* vir, int64_t step_n, bool with_specific) override {
-        (void)step_n;
+    // vels: the velocities a velocity-dependent pair term (DPD) is evaluated with (mb_forces_energy_vel); null elsewhere
+    int forces_energy(const void* coords, void* fs, void* pe, void* vir, int64_t step_n, bool with_specific,
+                      const void* vels) override {
         MB_TRY(prepare());
+        MB_TRY(check_dpd());
         if (!coords) return set_error(MB_ERR_INVALID, "coords is null");
+        if (dpd_on_ && fs && !vels)
+            return set_error(MB_ERR_INVALID, "the DPDInteraction forces depend on the velocities: use mb_forces_energy_vel");
+        if (dpd_on_ && vir) return set_error(MB_ERR_INVALID, "a DPDInteraction has no virial: the virial output must be null");
+        if (!dpd_on_ && vels) return set_error(MB_ERR_INVALID, "mb_forces_energy_vel: no velocity-dependent interaction is set (mb_set_dpd)");
         CallerBuf xb;
         MB_TRY(caller_xyz(coords, d_stage_a_, true, xb));
         const bool energy = (pe != nullptr) || (vir != nullptr);
@@ -1892,6 +1990,16 @@ class Engine : public EngineBase {
         } else {
             if (decomposed()) have_list_ = false;  // forces()/potential_energy() evaluate the whole box on every rank
             MB_TRY(sync_state_from(xb.as<T>(), nullptr));
+        }
+        if (dpd_on_) {  // the draws of step step_n (the Control step counter, rewritten by every simulate call) and v_pred = vels
+            const long long st = step_n;
+            MB_CUDA(cudaMemcpyAsync(&d_ctl_.as<Control>()->step, &st, sizeof(st), cudaMemcpyHostToDevice, stream_));
+            if (vels) {
+                CallerBuf vb;
+                MB_TRY(caller_xyz(vels, d_stage_c_, true, vb));
+                dpd_vpred_from_kernel<T><<<(int)((n_ + 255) / 256), 256, 0, stream_>>>((int)n_, vb.as<T>(), d_vpred4_.as<T4>());
+                launches_++;
+            }
         }
         Partials parts;
         MB_TRY(launch_pairs(energy, d_f4_.as<T4>(), false, &parts));
@@ -1957,6 +2065,7 @@ class Engine : public EngineBase {
         SplitCoef<T> sc;  // LangevinSplitting's dt_A, dt_B, -friction dt_O and kT
         SplitPlan sp;     // LangevinSplitting's passes and evaluations
         VerletCoef vt;    // StormerVerlet's dt^2; OverdampedLangevin's dt / gamma, sqrt(2 dt / gamma) and kT
+        T lam_dt;         // DPDVelocityVerlet's (lambda - 1/2) dt
     };
     // Langevin's c = exp(-dt friction), sqrt(1 - c^2) and kT (src/simulators.jl:1092-1097), in double. MTSLangevinIntegrator
     // runs its O step at the innermost substep, with f the innermost fraction: c = exp(-dt friction / f) (:1736-1738);
@@ -1991,6 +2100,7 @@ class Engine : public EngineBase {
         // OverdampedLangevin's noise_prefac = sqrt((2 / friction) dt) (src/simulators.jl:1451), in double
         c.vt = VerletCoef{ig.dt * ig.dt, 0.0, 0.0, 0.0};
         if (ig.kind == INTEG_OVERDAMPED) c.vt = VerletCoef{0.0, ig.dt / ig.friction, sqrt(2.0 / ig.friction * ig.dt), ig.kT};
+        c.lam_dt = (T)((ig.lambda - 0.5) * ig.dt);
         return c;
     }
     // what one step does beyond the plain VelocityVerlet step
@@ -2085,12 +2195,15 @@ class Engine : public EngineBase {
         prof_.begin(Prof::VV);
         int grid;
         const Thermo<T> th = thermo_in_k1(c);
-        const int thk = th.on ? TH_ANDERSEN : (c.vc.kind != VC_NONE ? TH_SCALE : TH_NONE);
+        // (DPDVelocityVerlet on a context without DPD is the VelocityVerlet step)
+        const bool dpd = c.ig.kind == INTEG_DPD_VV && dpd_on_;
+        const int thk = dpd ? TH_DPD : (th.on ? TH_ANDERSEN : (c.vc.kind != VC_NONE ? TH_SCALE : TH_NONE));
+        const DpdDrift<T> dd = {dpd ? d_vpred4_.as<T4>() : nullptr, c.lam_dt};
         MB_TRY(integ_grid(grid, n, 2, 5, 0));  // two atoms per thread, one wave (48 registers: 5 CTAs per SM)
-        with_const<TH_NONE, TH_ANDERSEN, TH_SCALE>(thk, [&](auto TH) {
+        with_const<TH_NONE, TH_ANDERSEN, TH_SCALE, TH_DPD>(thk, [&](auto TH) {
             vv_kick_drift_kernel<T, TH><<<grid, VV_THREADS, 0, stream_>>>(
                 0, n, c.dt, c.dt_half, c.skin_half2, cm, d_f4_.as<T4>(), d_xref4_.as<T4>(), d_pos4_.as<T4>(), d_vel4_.as<T4>(),
-                c.flag_ptr, ctl, rebuild_handle(cap), cap && path_ == 1 ? 1 : 0, PeerPush<T>{}, ext_map(), th);
+                c.flag_ptr, ctl, rebuild_handle(cap), cap && path_ == 1 ? 1 : 0, PeerPush<T>{}, ext_map(), th, dd);
         });
         prof_.end(Prof::VV);
         launches_++;
@@ -2562,7 +2675,7 @@ class Engine : public EngineBase {
         MB_TRY(integ_grid(grid, own_n_, 2, 5, 0));
         vv_kick_drift_kernel<T, TH_NONE><<<grid, VV_THREADS, 0, stream_>>>(own_s0_, own_n_, c.dt, c.dt_half, c.skin_half2, cm, d_f4_.as<T4>(),
                                                                           d_xref4_.as<T4>(), d_pos4_.as<T4>(), d_vel4_.as<T4>(), c.flag_ptr,
-                                                                          ctl, 0, 0, push, ext_map(), thermo_in_k1(c));
+                                                                          ctl, 0, 0, push, ext_map(), thermo_in_k1(c), DpdDrift<T>{});
         prof_.end(Prof::VV);
         launches_++;
         if (o.clear_cm_after_k1) {
@@ -2655,12 +2768,13 @@ class Engine : public EngineBase {
     int check_simulate(const void* coords, const void* vels, const Integrator& ig) {
         static const char* const entry[] = {"mb_simulate_vv", "mb_simulate_langevin", "mb_simulate_nose_hoover", "mb_simulate_mts",
                                             "mb_simulate_mts", "mb_simulate_langevin_splitting", "mb_simulate_verlet",
-                                            "mb_simulate_stormer_verlet", "mb_simulate_overdamped_langevin"};
+                                            "mb_simulate_stormer_verlet", "mb_simulate_overdamped_langevin", "mb_simulate_dpd_vv"};
         static const char* const name[] = {"VelocityVerlet", "Langevin", "Nose-Hoover", "the multiple-time-step integrators",
                                            "the multiple-time-step integrators", "LangevinSplitting", "Verlet", "StormerVerlet",
-                                           "OverdampedLangevin"};
+                                           "OverdampedLangevin", "DPDVelocityVerlet"};
         if (!coords || !vels) return set_error(MB_ERR_INVALID, "null argument");
         if (ig.n_steps < 0 || !(ig.dt > 0)) return set_error(MB_ERR_INVALID, "n_steps < 0 or dt <= 0");
+        MB_TRY(check_dpd());
         const std::string who = std::string(entry[ig.kind]) + ": ";
         if (is_mts(ig.kind)) {
             if (ig.n_levels < 1 || ig.n_levels > MB_MTS_MAX_LEVELS)
@@ -2692,6 +2806,9 @@ class Engine : public EngineBase {
             if (!(std::isfinite(ig.kT) && ig.kT >= 0)) return set_error(MB_ERR_INVALID, who + "kT must be finite and >= 0");
             if (!(std::isfinite(ig.friction) && ig.friction > 0)) return set_error(MB_ERR_INVALID, who + "friction must be finite and > 0");
         }
+        if (ig.kind == INTEG_DPD_VV && !std::isfinite(ig.lambda)) return set_error(MB_ERR_INVALID, who + "lambda must be finite");
+        if (dpd_on_ && ig.kind != INTEG_DPD_VV)
+            return set_error(MB_ERR_INVALID, who + "a DPDInteraction is set (mb_set_dpd): only mb_simulate_dpd_vv runs it");
         if (ig.kind == INTEG_NH) {
             // (kT = 0 would make T / T0 infinite)
             if (!(std::isfinite(ig.kT) && ig.kT > 0)) return set_error(MB_ERR_INVALID, who + "kT must be finite and > 0");
@@ -2779,6 +2896,10 @@ class Engine : public EngineBase {
                                                                         PeerSignal{}, VCouple{});
             launches_++;
             cm_pending = true;
+        }
+        if (c.ig.kind == INTEG_DPD_VV && dpd_on_) {  // F0 with the current velocities: v_pred = v after the pending v_cm
+            dpd_vpred_init_kernel<T><<<nb, 256, 0, stream_>>>((int)n_, d_vel4_.as<T4>(), d_orig_.as<int>(), cm, d_vpred4_.as<T4>());
+            launches_++;
         }
         if (dec) {
             MB_TRY(simulate_decomposed(c, cm_pending));
@@ -2898,6 +3019,7 @@ class Engine : public EngineBase {
     int minimize_sd(void* coords, mb_sd_params_t* p) override {
         MB_TRY(prepare());
         if (!coords || !p) return set_error(MB_ERR_INVALID, "null argument");
+        if (dpd_on_) return set_error(MB_ERR_INVALID, "mb_minimize_sd: a DPDInteraction is set (mb_set_dpd): only mb_simulate_dpd_vv runs it");
         if (p->max_steps < 0 || !(p->step_size > 0) || !(p->tol >= 0))
             return set_error(MB_ERR_INVALID, "mb_minimize_sd: max_steps < 0, step_size <= 0 or tol < 0");
         if (p->trace && p->trace_capacity < p->max_steps + 1)
@@ -3155,6 +3277,10 @@ class Engine : public EngineBase {
     DevBuf d_f4_mts_;  // forces of the inner multiple-time-step levels (slot order; fixed address: the step graphs bake it in)
     // PME (pme.cuh)
     bool pme_on_ = false, pme_ready_ = false;
+    bool dpd_on_ = false;  // mb_set_dpd: dpd_ replaces the pairwise interactions
+    mb_dpd_t dpd_ = {};
+    DevBuf d_vpred4_;      // DPD: predicted velocities, original order (dpd.cuh)
+    DevBuf d_dpd_args_;    // DPD: the brick kernel's DpdArgs (dpd_args_of)
     double pme_rc_ = 0, pme_tol_ = 0, pme_epsr_ = 1, pme_alpha_ = 0, pme_self_e_ = 0, pme_ke_ = 138.93545764;
     PmeGeom pme_g_ = {{0, 0, 0}, {0, 0, 0}};
     int pme_plan_ = -1;
@@ -3276,21 +3402,27 @@ int mb_set_neighbor_policy(mb_ctx* ctx, double r_list, int rebuild_every) {
 int mb_forces(mb_ctx* ctx, const void* coords, void* fs_mat, void* virial, int64_t step_n) {
     MB_CTX_GUARD(ctx);
     if (!fs_mat) return mb::set_error(MB_ERR_INVALID, "fs_mat is null");
-    return ctx->e->forces_energy(coords, fs_mat, nullptr, virial, step_n, false);
+    return ctx->e->forces_energy(coords, fs_mat, nullptr, virial, step_n, false, nullptr);
 }
 int mb_energy(mb_ctx* ctx, const void* coords, void* pe, int64_t step_n) {
     MB_CTX_GUARD(ctx);
     if (!pe) return mb::set_error(MB_ERR_INVALID, "pe is null");
-    return ctx->e->forces_energy(coords, nullptr, pe, nullptr, step_n, false);
+    return ctx->e->forces_energy(coords, nullptr, pe, nullptr, step_n, false, nullptr);
 }
 int mb_forces_energy(mb_ctx* ctx, const void* coords, void* fs_mat, void* pe, void* virial, int64_t step_n) {
     MB_CTX_GUARD(ctx);
-    return ctx->e->forces_energy(coords, fs_mat, pe, virial, step_n, false);
+    return ctx->e->forces_energy(coords, fs_mat, pe, virial, step_n, false, nullptr);
 }
 int mb_forces_energy_all(mb_ctx* ctx, const void* coords, void* fs_mat, void* pe, int64_t step_n) {
     MB_CTX_GUARD(ctx);
-    return ctx->e->forces_energy(coords, fs_mat, pe, nullptr, step_n, true);
+    return ctx->e->forces_energy(coords, fs_mat, pe, nullptr, step_n, true, nullptr);
 }
+int mb_forces_energy_vel(mb_ctx* ctx, const void* coords, const void* vels, void* fs_mat, void* pe, int64_t step_n) {
+    MB_CTX_GUARD(ctx);
+    if (!vels) return mb::set_error(MB_ERR_INVALID, "mb_forces_energy_vel: vels is null");
+    return ctx->e->forces_energy(coords, fs_mat, pe, nullptr, step_n, true, vels);
+}
+int mb_set_dpd(mb_ctx* ctx, const mb_dpd_t* p) { MB_CTX_GUARD(ctx); return ctx->e->set_dpd(p); }
 int mb_set_specific(mb_ctx* ctx, int kind, int64_t n_terms, const int32_t* atom_idx, const double* params) {
     MB_CTX_GUARD(ctx);
     return ctx->e->set_specific(kind, n_terms, atom_idx, params);
@@ -3386,6 +3518,13 @@ int mb_simulate_overdamped_langevin(mb_ctx* ctx, void* coords, void* vels, const
     mb::Integrator ig = integrator_call(mb::INTEG_OVERDAMPED, p, p->rng_ctr1, p->rng_key);
     ig.kT = p->kT;
     ig.friction = p->friction;
+    return ctx->e->simulate(coords, vels, ig, log);
+}
+int mb_simulate_dpd_vv(mb_ctx* ctx, void* coords, void* vels, const mb_dpd_vv_params_t* p, mb_log_t* log) {
+    MB_CTX_GUARD(ctx);
+    if (!p) return mb::set_error(MB_ERR_INVALID, "null argument");
+    mb::Integrator ig = integrator_call(mb::INTEG_DPD_VV, p, 0, 0);  // (no draws of its own: the DPD draws are keyed by mb_dpd_t)
+    ig.lambda = p->lambda;
     return ctx->e->simulate(coords, vels, ig, log);
 }
 int mb_minimize_sd(mb_ctx* ctx, void* coords, mb_sd_params_t* p) { MB_CTX_GUARD(ctx); return ctx->e->minimize_sd(coords, p); }

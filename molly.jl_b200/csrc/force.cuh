@@ -14,6 +14,7 @@
 // pairwise_force_kernel_nonl! (ext/MollyCUDAExt.jl:2305-2371).
 #pragma once
 #include "cells.cuh"
+#include "dpd.cuh"
 #include "pair.cuh"
 #include "peer.cuh"
 
@@ -62,13 +63,21 @@ __host__ __device__ inline size_t force_stage_bytes(int halo_cap, int task_cap, 
 //     neighbour rows (software-pipelined: the next quad's first index words are requested while the current one is
 //     evaluated, across stage boundaries), reduce with shuffles and store. A warp releases a stage (mbarrier empty[s])
 //     once it holds no quad in it; there is no CTA-wide barrier in the steady state.
-template <typename T, int COUL, bool UNIFORM, int CUTM, bool ENERGY>
-__global__ void __launch_bounds__(FORCE_THREADS, (sizeof(T) == 8) ? 1 : FORCE_CTAS_F32)
+//   DPD: the DPDInteraction variant (dpd.cuh; instantiated with COUL_NONE, UNIFORM, CUTM_PLAIN): the staged w is the
+//     original index, v_j is gathered from the predicted velocities and the pair's draw is keyed by the device step counter.
+//     Special-list entries get the full force. No virial: the ENERGY variant sums the conservative energy only. One CTA per
+//     SM: the draw's double-precision Box-Muller needs more than 64 registers.
+template <typename T, int COUL, bool UNIFORM, int CUTM, bool ENERGY, bool DPD = false>
+__global__ void __launch_bounds__(FORCE_THREADS, (sizeof(T) == 8 || DPD) ? 1 : FORCE_CTAS_F32)
     brick_force_kernel(Geom<T> g, PairParams<T> P, const BrickHdr* __restrict__ hdrs, const Run* __restrict__ runs,
                        const int2* __restrict__ task_tab, const typename VT<T>::T4* __restrict__ pos4e,
                        const typename VT<T>::T2* __restrict__ lj2e, const unsigned short* __restrict__ list,
                        const unsigned short* __restrict__ slist, ForceOut<T> out, int brick0, int nbr, int nbuf,
                        unsigned int* __restrict__ sched) {
+    // DPD stages positions only, so the LJ-parameter pointer carries the address of its constants (DpdArgs in device
+    // memory, dpd_args_of): the parameter list, and with it the code of every other variant, stays as it is
+    static_assert(!DPD || (COUL == COUL_NONE && UNIFORM && CUTM == CUTM_PLAIN),
+                  "the DPD variant stages positions only: its LJ-parameter pointer carries the DpdArgs (dpd_args_of)");
     using T4 = typename VT<T>::T4;
     using T2 = typename VT<T>::T2;
     extern __shared__ __align__(128) unsigned char smem_raw[];
@@ -195,8 +204,14 @@ __global__ void __launch_bounds__(FORCE_THREADS, (sizeof(T) == 8) ? 1 : FORCE_CT
         T4 pi = make4<T>(0, 0, 0, 0);
         T lj_s_i = (T)0, lj_e_i = (T)0, kq_i = (T)0;
         T fx = (T)0, fy = (T)0, fz = (T)0;
+        // DPD: the step the draws are keyed by, and the quad's atom: original index and predicted velocity
+        long long dstep = 0;
+        int oi = 0;
+        T4 vi;
+        if constexpr (DPD) dstep = *dpd_args_of<T>(lj2e).step;
         auto eval = [&](int j, auto special_tag) {
             constexpr bool SPECIAL = decltype(special_tag)::value;
+            (void)SPECIAL;  // (the DPD variant gives special pairs the full force)
             const T4 pj = lds_pos(s_pos_u32 + (uint32_t)j * (uint32_t)sizeof(T4), (T)0);
             T lj_s_j = (T)0, lj_e_j = (T)0;
             if (!UNIFORM) {
@@ -207,21 +222,42 @@ __global__ void __launch_bounds__(FORCE_THREADS, (sizeof(T) == 8) ? 1 : FORCE_CT
             const T dx = pi.x - pj.x, dy = pi.y - pj.y, dz = pi.z - pj.z;
             const T r2 = dx * dx + dy * dy + dz * dz;
             T fr, e;
-            pair_eval<T, COUL, UNIFORM, CUTM, ENERGY, SPECIAL>(P, r2, lj_s_i, lj_e_i, lj_s_j, lj_e_j, kq_i, pj.w, fr, e);
+            if constexpr (DPD) dpd_eval<T>(dpd_args_of<T>(lj2e), dstep, oi, vi, r2, dx, dy, dz, pj.w, fr, e);
+            else pair_eval<T, COUL, UNIFORM, CUTM, ENERGY, SPECIAL>(P, r2, lj_s_i, lj_e_i, lj_s_j, lj_e_j, kq_i, pj.w, fr, e);
             const T gx = fr * dx, gy = fr * dy, gz = fr * dz;
             fx += gx;
             fy += gy;
             fz += gz;
             if (ENERGY) {
                 e_acc += e;
-                vir[0] += dx * gx; vir[1] += dy * gy; vir[2] += dz * gz;
-                vir[3] += dx * gy; vir[4] += dx * gz; vir[5] += dy * gz;
+                if constexpr (!DPD) {
+                    vir[0] += dx * gx; vir[1] += dy * gy; vir[2] += dz * gz;
+                    vir[3] += dx * gy; vir[4] += dx * gz; vir[5] += dy * gz;
+                }
             }
         };
         // four neighbours at once, stage by stage, so the four shared-memory loads and the four reciprocal
         // chains are independent and in flight together
         auto eval4 = [&](uint2 wd) {
             // entries are byte offsets of float4 records (halo index << LIST_SHIFT)
+            if constexpr (DPD) {
+                // one neighbour at a time: four draws (Philox and a Box-Muller in double each) in flight do not fit the registers
+#pragma unroll 1
+                for (int u = 0; u < 4; u++) {
+                    const uint32_t w32 = (u < 2) ? wd.x : wd.y;
+                    const uint32_t j = (u & 1) ? (w32 >> 16) : (w32 & 0xffffu);
+                    const T4 pj = lds_pos(s_pos_u32 + j * (uint32_t)(sizeof(T4) >> LIST_SHIFT), (T)0);
+                    const T dx = pi.x - pj.x, dy = pi.y - pj.y, dz = pi.z - pj.z;
+                    T fr, e;
+                    dpd_eval<T>(dpd_args_of<T>(lj2e), dstep, oi, vi, dx * dx + dy * dy + dz * dz, dx, dy, dz, pj.w, fr, e);
+                    const T gx = fr * dx, gy = fr * dy, gz = fr * dz;
+                    fx += gx;
+                    fy += gy;
+                    fz += gz;
+                    if (ENERGY) e_acc += e;
+                }
+                return;
+            }
             const int j[4] = {(int)(wd.x & 0xffffu), (int)(wd.x >> 16), (int)(wd.y & 0xffffu), (int)(wd.y >> 16)};
             T4 pj[4];
             T2 lj[4];
@@ -335,6 +371,10 @@ __global__ void __launch_bounds__(FORCE_THREADS, (sizeof(T) == 8) ? 1 : FORCE_CT
                 lj_e_i = t.y;
             }
             kq_i = P.ke * pi.w;
+            if constexpr (DPD) {
+                oi = (int)pi.w;
+                vi = dpd_args_of<T>(lj2e).vpred[oi];
+            }
             fx = (T)0; fy = (T)0; fz = (T)0;
             // main list: groups of 32 entries; each of the 8 lanes owns 4 entries (one 8-byte word) per group
             const int n_groups = (cur_n_main + 31) >> 5;
@@ -459,13 +499,15 @@ __device__ __forceinline__ T mic_1d(T ci, T cj, T L) {
 
 constexpr int AP_THREADS = 128;
 
-template <typename T, int COUL, int CUTM, bool ENERGY>
+// DPD: the DPDInteraction variant (dpd.cuh; instantiated with COUL_NONE, CUTM_PLAIN): the position records' w is the atom's
+// index, v_j is gathered from dpd.vpred; exclusions apply when the interaction uses the neighbour list (dpd.nl). No virial.
+template <typename T, int COUL, int CUTM, bool ENERGY, bool DPD = false>
 __global__ void __launch_bounds__(AP_THREADS)
     allpairs_force_kernel(int n, PairParams<T> P, T Lx, T Ly, T Lz, Tric<T> tric, const typename VT<T>::T4* __restrict__ posq,
                           const typename VT<T>::T2* __restrict__ lj2, const int* __restrict__ ex_ptr,
                           const int* __restrict__ ex_idx, const int* __restrict__ sp_ptr,
                           const int* __restrict__ sp_idx, typename VT<T>::T4* __restrict__ f4,
-                          double* __restrict__ pe_partial, double* __restrict__ vir_partial) {
+                          double* __restrict__ pe_partial, double* __restrict__ vir_partial, DpdArgs<T> dpd) {
     using T4 = typename VT<T>::T4;
     using T2 = typename VT<T>::T2;
     __shared__ T4 s_pos[AP_THREADS];
@@ -481,6 +523,8 @@ __global__ void __launch_bounds__(AP_THREADS)
     if (active && sp_ptr) { sp_a = sp_ptr[i]; sp_n = sp_ptr[i + 1] - sp_a; }
     T fx = 0, fy = 0, fz = 0, e_acc = 0;
     T vir[6] = {0, 0, 0, 0, 0, 0};
+    const long long dstep = DPD ? *dpd.step : 0;
+    const T4 vi = (DPD && active) ? dpd.vpred[i] : make4<T>(0, 0, 0, 0);
     for (int j0 = 0; j0 < n; j0 += AP_THREADS) {
         int jj = j0 + tid;
         __syncthreads();
@@ -508,13 +552,20 @@ __global__ void __launch_bounds__(AP_THREADS)
             }
             T r2 = dx * dx + dy * dy + dz * dz;
             T fr, e;
-            pair_eval_rt<T, COUL, CUTM, ENERGY>(P, r2, li.x, li.y, lj.x, lj.y, kq_i, pj.w, excluded, special, fr, e);
+            if constexpr (DPD) {
+                if (excluded && dpd.nl) { fr = (T)0; e = (T)0; }
+                else dpd_eval<T>(dpd, dstep, i, vi, r2, dx, dy, dz, pj.w, fr, e);
+            } else {
+                pair_eval_rt<T, COUL, CUTM, ENERGY>(P, r2, li.x, li.y, lj.x, lj.y, kq_i, pj.w, excluded, special, fr, e);
+            }
             T gx = fr * dx, gy = fr * dy, gz = fr * dz;
             fx += gx; fy += gy; fz += gz;
             if (ENERGY) {
                 e_acc += e;
-                vir[0] += dx * gx; vir[1] += dy * gy; vir[2] += dz * gz;
-                vir[3] += dx * gy; vir[4] += dx * gz; vir[5] += dy * gz;
+                if constexpr (!DPD) {  // (DPD has no virial)
+                    vir[0] += dx * gx; vir[1] += dy * gy; vir[2] += dz * gz;
+                    vir[3] += dx * gy; vir[4] += dx * gz; vir[5] += dy * gz;
+                }
             }
         }
     }

@@ -9,6 +9,7 @@
 // is applied at every rebuild and on export, which is equivalent under the minimum-image convention.
 #pragma once
 #include "cells.cuh"
+#include "dpd.cuh"
 #include "peer.cuh"
 #include "vrescale.cuh"
 
@@ -186,15 +187,16 @@ __device__ __forceinline__ void step_advance(Control* __restrict__ ctl, cudaGrap
 // ---- K1: first half kick + drift + displacement check; the last CTA to finish does the step bookkeeping (step_advance).
 // THERMO: the variants that also apply the previous step's thermostat are separate instantiations so that the plain kernel
 // keeps its register count (one atom per thread, latency-bound: occupancy matters): TH_ANDERSEN resamples (Philox +
-// Box-Muller inlined), TH_SCALE applies the pending velocity-rescaling factor after the pending v_cm.
-enum { TH_NONE = 0, TH_ANDERSEN = 1, TH_SCALE = 2 };
+// Box-Muller inlined), TH_SCALE applies the pending velocity-rescaling factor after the pending v_cm. TH_DPD is the
+// DPDVelocityVerlet drift: K1 unchanged plus the predicted velocity of dd (dpd.cuh) stored by the original index in p.w.
+enum { TH_NONE = 0, TH_ANDERSEN = 1, TH_SCALE = 2, TH_DPD = 3 };
 template <typename T, int THERMO>
 __global__ void vv_kick_drift_kernel(int s0, int n, T dt, T dt_half, T skin_half2, const CmState<T>* __restrict__ cm,
                                      const typename VT<T>::T4* __restrict__ f4,
                                      const typename VT<T>::T4* __restrict__ xref4, typename VT<T>::T4* __restrict__ pos4,
                                      typename VT<T>::T4* __restrict__ vel4, int* __restrict__ flag, Control* __restrict__ ctl,
                                      cudaGraphConditionalHandle handle, int use_handle, PeerPush<T> push, ExtMap<T> ext,
-                                     Thermo<T> th) {
+                                     Thermo<T> th, DpdDrift<T> dd) {
     bool cmv = cm->valid != 0;
     // thermostat of the step that just ended, folded in here (the standalone kernel would be one more launch per step):
     // same order of operations on v - subtract the pending v_cm, resample, then this step's first kick
@@ -265,6 +267,10 @@ __global__ void vv_kick_drift_kernel(int s0, int n, T dt, T dt_half, T skin_half
             const T a = v[u].w * dt_half;  // (1/m) dt/2
             v[u].x += f[u].x * a; v[u].y += f[u].y * a; v[u].z += f[u].z * a;
             p[u].x += v[u].x * dt; p[u].y += v[u].y * dt; p[u].z += v[u].z * dt;
+            if (THERMO == TH_DPD) {
+                const T b = v[u].w * dd.lam_dt;  // (1/m) (lambda - 1/2) dt
+                dd.vpred[(int)p[u].w] = make4<T>(v[u].x + f[u].x * b, v[u].y + f[u].y * b, v[u].z + f[u].z * b, (T)0);
+            }
             vel4[s] = v[u];
             pos4[s] = p[u];
             if (ext.pos4e) {
