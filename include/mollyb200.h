@@ -187,14 +187,18 @@ int mb_forces_energy_all(mb_ctx* ctx, const void* coords, void* fs_mat, void* pe
 int mb_set_lj_dispersion_correction(mb_ctx* ctx, double dist_cutoff);
 
 /* Particle-mesh Ewald, SURVEY.md §8(f)-3. GPU parity: tests/test_zz_gpu_pme.py (OpenMM forces_all_pme_exact at the
- * reference's 1e-7 kJ/mol/nm / 1e-5 kJ/mol in f64); the per-item arithmetic is also checked on the host
- * (tests/test_pme_host.py), the plan by mb_pme_plan's test. Replaces the `PME`
+ * reference's 1e-7 kJ/mol/nm / 1e-5 kJ/mol in f64) and tests/test_gpu_pme_matrix.py (oracle/pme.py in f64 and f32 over
+ * meshes, error_tol, charges, eps_r, coordinate and exclusion-pair edges, both force paths and the live-context setters);
+ * the per-item arithmetic is also checked on the host (tests/test_pme_host.py), the oracle against a direct Ewald sum
+ * (tests/test_pme_direct_ewald.py), the plan by mb_pme_plan's test. Replaces the `PME`
  * general interaction (src/interactions/ewald.jl:363-958; constructor PME(dist_cutoff, atoms, boundary; error_tol,
  * order=5, eps_r)) and the `EwaldExclusion` specific interaction list (:979-1055) that src/setup.jl:1903-1912 builds
  * from find_excluded_pairs(eligible, special): pairs = excluded OR special, 1-based. Use together with an
  * MB_EWALD_REAL pairwise interaction of the same r_cut / error_tol (ewald_alpha = sqrt(-ln(2 error_tol)) / r_cut).
  * Once set, mb_forces_energy_all and mb_simulate_vv add the reciprocal-space + exclusion forces (and energies incl.
- * the self and neutralising-background terms) after the pair kernel. order = 0 switches it off; only order 5 exists. */
+ * the self and neutralising-background terms) after the pair kernel. order = 0 switches it off; only order 5 exists.
+ * The self and background energy follow later mb_set_atoms calls. If mb_set_atoms lowers the atom count below a pair
+ * index, every evaluation and simulate call fails with MB_ERR_STATE, before any launch, until this is called again. */
 int mb_set_pme(mb_ctx* ctx, double r_cut, double error_tol, int order, double eps_r, int64_t n_pairs,
                const int32_t* pair_i, const int32_t* pair_j);
 /* The host-side PME plan (no GPU needed; what the PME constructor computes, ewald.jl:373, :484-487, :311-361): Ewald

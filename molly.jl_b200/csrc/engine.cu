@@ -491,6 +491,7 @@ class Engine : public EngineBase {
         }
         n_ = n;
         dirty_ = true;
+        pme_ready_ = disp_ready_ = false;  // the PME self energy and the dispersion factors come from the atoms
         return MB_OK;
     }
     int set_atoms_soa(int64_t n, const void* mass, const void* charge, const void* sigma, const void* eps) override {
@@ -504,6 +505,7 @@ class Engine : public EngineBase {
         h_eps_raw_ = h_eps_;
         n_ = n;
         dirty_ = true;
+        pme_ready_ = disp_ready_ = false;
         return MB_OK;
     }
     int set_box(const double side[3]) override {
@@ -645,6 +647,11 @@ class Engine : public EngineBase {
         if (n_ <= 0) return set_error(MB_ERR_STATE, "atoms not set");
         if (!(box_[0] > 0)) return set_error(MB_ERR_STATE, "box not set");
         if (n_ > 2000000000LL) return set_error(MB_ERR_INVALID, "too many atoms");
+        // mb_set_pme checked its pairs against the atom count of that time; mb_set_atoms may have lowered it since. This
+        // runs before any kernel of the evaluation writes into the forces.
+        if (pme_on_)
+            for (int a : pme_pairs_)
+                if (a >= n_) return set_error(MB_ERR_STATE, "PME: an exclusion pair indexes past the atom count set by mb_set_atoms; call mb_set_pme again");
         memset(&P_, 0, sizeof(P_));
         MB_TRY(check_dpd());
         const double inf = std::numeric_limits<double>::infinity();

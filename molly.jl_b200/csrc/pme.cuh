@@ -7,11 +7,14 @@
 // (ix * K1 + iy) * K2 + iz, transformed in place by cuFFT (C2C / Z2Z, unnormalised both ways like fft! / bfft!).
 // Checker: oracle/pme.py, pinned against OpenMM's forces_all_pme_exact (tests/test_oracle.py).
 //
-// STATUS: first implementation, written after the GPU budget of round 1 was spent. Every kernel is a thin loop over
-// a __host__ __device__ per-item function, and those functions ARE validated: tests/test_pme_host.py compiles them
-// for the host, runs spread -> numpy FFT -> convolution -> numpy inverse FFT -> interpolation -> exclusion and compares
-// with oracle/pme.py / the OpenMM goldens. What has not run yet is the launch plumbing, the atomics and cuFFT; the GPU
-// test (tests/test_zz_gpu_pme.py) is marked xfail until it has. Nothing calls into this file unless mb_set_pme was.
+// Validation. Every kernel is a thin loop over a __host__ __device__ per-item function. tests/test_pme_host.py compiles
+// those functions for the host and checks the chain spread -> FFT -> convolution -> inverse FFT -> interpolation ->
+// exclusion against oracle/pme.py and the OpenMM goldens. On the device, tests/test_zz_gpu_pme.py matches OpenMM for 6mrr
+// (f64) and the three waters (f64, f32). tests/test_gpu_pme_matrix.py compares PME-only systems with oracle/pme.py in
+// f64 (1e-9) and f32: cubic, anisotropic and K = 6 meshes with odd and even K, error_tol 1e-3 to 1e-5, net charge,
+// uncharged atoms, eps_r != 1, coordinates outside the box, edge exclusion pairs, both force paths, 6mrr, a finite-
+// difference check, and mb_set_box / mb_set_atoms on a live context. tests/test_pme_direct_ewald.py pins oracle/pme.py
+// against a direct Ewald sum on the same shapes. Nothing calls into this file unless mb_set_pme was.
 #pragma once
 #include "common.cuh"
 

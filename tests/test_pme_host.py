@@ -1,8 +1,8 @@
 """The PME device functions, run on the HOST (SURVEY.md §8(f)-3). csrc/pme.cuh writes every kernel as a thin loop over a
 __host__ __device__ per-item function; tests/host/pme_host.cu compiles those functions for the CPU (nvcc, host code
 only) and this test drives spread -> FFT (numpy) -> convolution -> inverse FFT -> interpolation -> exclusion with them and
-compares with the numpy oracle and, end to end, with OpenMM's forces_all_pme_exact for 6mrr. What this does NOT cover is
-the CUDA launch plumbing, the atomics and cuFFT (tests/test_zz_gpu_pme.py, xfail until it has run on a GPU)."""
+compares with the numpy oracle and, end to end, with OpenMM's forces_all_pme_exact for 6mrr. The CUDA launch plumbing,
+the atomics and cuFFT are covered on the GPU by tests/test_zz_gpu_pme.py and tests/test_gpu_pme_matrix.py."""
 import ctypes as C
 import os
 import shutil
