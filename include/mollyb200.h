@@ -590,6 +590,49 @@ typedef struct {
 } mb_dpd_vv_params_t;
 int mb_simulate_dpd_vv(mb_ctx* ctx, void* coords, void* vels, const mb_dpd_vv_params_t* p, mb_log_t* log);
 
+/* Several simulate calls on one GPU with their steps in flight at once (temperature replica exchange runs one per
+ * thermodynamic state). Member i is the call mb_simulate_<kind>(ctx, coords, vels, params, log) with `params` pointing at
+ * that entry's parameter struct:
+ *   MB_INTEG_VV                  mb_simulate_vv_log               mb_vv_params_t
+ *   MB_INTEG_LANGEVIN            mb_simulate_langevin             mb_langevin_params_t
+ *   MB_INTEG_NOSE_HOOVER         mb_simulate_nose_hoover          mb_nosehoover_params_t
+ *   MB_INTEG_MTS                 mb_simulate_mts                  mb_mts_params_t
+ *   MB_INTEG_LANGEVIN_SPLITTING  mb_simulate_langevin_splitting   mb_splitting_params_t
+ *   MB_INTEG_VERLET              mb_simulate_verlet               mb_vv_params_t
+ *   MB_INTEG_STORMER_VERLET      mb_simulate_stormer_verlet       mb_stormer_params_t
+ *   MB_INTEG_OVERDAMPED_LANGEVIN mb_simulate_overdamped_langevin  mb_langevin_params_t
+ *   MB_INTEG_DPD_VV              mb_simulate_dpd_vv               mb_dpd_vv_params_t
+ * Every member's prologue runs first (refusals, ingest, F0, the loggers at init_step, graph capture); then the steps,
+ * round-robin, one per member per round, each enqueued on its own context's stream (a member with fewer steps drops out
+ * early); then every member's epilogue (export, copy-back, the overflow check). Each member computes what its single call
+ * computes; the step kernels are the same, and no kernel reads state another context writes.
+ * Returns MB_OK when every member succeeded, otherwise the first failing member's status; `status` holds each member's
+ * outcome. A failed member leaves its buffers as its single call would have (after MB_ERR_CAPACITY: invalid; retry it
+ * with its single call). MB_ERR_INVALID before any work for n <= 0, a null member array, context or params, an unknown
+ * kind, one context in two members, members on different devices, and a decomposed (multi-GPU) context; a refused group
+ * (n > 0, members non-null) sets every member's status to MB_ERR_INVALID. */
+enum {
+    MB_INTEG_VV = 0,
+    MB_INTEG_LANGEVIN = 1,
+    MB_INTEG_NOSE_HOOVER = 2,
+    MB_INTEG_MTS = 3,
+    MB_INTEG_LANGEVIN_SPLITTING = 4,
+    MB_INTEG_VERLET = 5,
+    MB_INTEG_STORMER_VERLET = 6,
+    MB_INTEG_OVERDAMPED_LANGEVIN = 7,
+    MB_INTEG_DPD_VV = 8
+};
+typedef struct {
+    mb_ctx* ctx;
+    void* coords;
+    void* vels;
+    int32_t kind;        /* MB_INTEG_* */
+    const void* params;  /* that kind's parameter struct */
+    mb_log_t* log;       /* NULL: no logging */
+    int32_t status;      /* out: this member's MB_* status */
+} mb_group_member_t;
+int mb_simulate_group(int32_t n, mb_group_member_t* members);
+
 /* simulate!(sys, SteepestDescentMinimizer(step_size, max_steps, tol)) (src/simulators.jl:183-274) on the device: wrap the
  * coordinates, E = potential energy; then for step n = init_step+1 .. init_step+max_steps: F = forces, m = max |F_i|,
  * x <- wrap(x + h F / m), E_trial = potential energy; E_trial < E accepts (h <- 6h/5, E <- E_trial), otherwise x is restored

@@ -18,4 +18,5 @@ from .api import (Atom, CubicBoundary, TriclinicBoundary, System, NoCutoff, Dist
                   InteractionList4Atoms, PotentialEnergyLogger, KineticEnergyLogger, TotalEnergyLogger, TemperatureLogger,
                   CoordinatesLogger, VelocitiesLogger, values, record_steps, SteepestDescentMinimizer, steepest_descent,
                   sd_log_lines, ImplicitSolventOBC, ImplicitSolventGBN2, InteractionList1Atoms, MorseBonds, FENEBonds,
-                  CosineAngles, UreyBradleys, HarmonicTorsions, RBTorsions, add_position_restraints)
+                  CosineAngles, UreyBradleys, HarmonicTorsions, RBTorsions, add_position_restraints, ThermoState,
+                  ReplicaSystem, ReplicaExchangeMD, ReplicaExchangeLogger, simulate_remd)

@@ -24,7 +24,7 @@ EXPORTED = [
     "mb_simulate_vv_log", "mb_minimize_sd", "mb_set_velocity_coupling", "mb_simulate_langevin",
     "mb_simulate_nose_hoover", "mb_set_specific_levels", "mb_simulate_mts", "mb_set_implicit_solvent",
     "mb_simulate_langevin_splitting", "mb_simulate_verlet", "mb_simulate_stormer_verlet", "mb_simulate_overdamped_langevin",
-    "mb_set_dpd", "mb_forces_energy_vel", "mb_simulate_dpd_vv",
+    "mb_set_dpd", "mb_forces_energy_vel", "mb_simulate_dpd_vv", "mb_simulate_group",
 ]
 MB_GB_MAX_NECK_CLASSES = 32
 # specific interaction kinds of mb_set_specific (include/mollyb200.h)
@@ -32,6 +32,9 @@ MB_GB_MAX_NECK_CLASSES = 32
  MB_SPECIFIC_MORSE_BOND, MB_SPECIFIC_FENE_BOND, MB_SPECIFIC_COSINE_ANGLE, MB_SPECIFIC_UREY_BRADLEY, MB_SPECIFIC_HARMONIC_TORSION,
  MB_SPECIFIC_RB_TORSION, MB_SPECIFIC_N_KINDS) = range(11)
 MB_MTS_MAX_LEVELS = 8
+# integrator kinds of mb_simulate_group, one per mb_simulate_* entry (include/mollyb200.h)
+(MB_INTEG_VV, MB_INTEG_LANGEVIN, MB_INTEG_NOSE_HOOVER, MB_INTEG_MTS, MB_INTEG_LANGEVIN_SPLITTING, MB_INTEG_VERLET,
+ MB_INTEG_STORMER_VERLET, MB_INTEG_OVERDAMPED_LANGEVIN, MB_INTEG_DPD_VV) = range(9)
 MB_SPLIT_MAX_OPS = 32
 
 
@@ -147,6 +150,11 @@ class MollyB200Error(RuntimeError):
         self.code = code
 
 
+class MBGroupMember(C.Structure):
+    _fields_ = [("ctx", C.c_void_p), ("coords", C.c_void_p), ("vels", C.c_void_p), ("kind", C.c_int32),
+                ("params", C.c_void_p), ("log", C.c_void_p), ("status", C.c_int32)]
+
+
 _lib = None
 
 
@@ -187,6 +195,7 @@ def load():
     L.mb_set_dpd.argtypes = [vp, C.POINTER(MBDpd)]
     L.mb_forces_energy_vel.argtypes = [vp, vp, vp, vp, vp, i64]
     L.mb_simulate_dpd_vv.argtypes = [vp, vp, vp, C.POINTER(MBDpdVVParams), C.POINTER(MBLog)]
+    L.mb_simulate_group.argtypes = [i32, C.POINTER(MBGroupMember)]
     L.mb_set_specific_levels.argtypes = [vp, C.c_int, i64, vp]
     L.mb_minimize_sd.argtypes = [vp, vp, C.POINTER(MBSDParams)]
     L.mb_set_velocity_coupling.argtypes = [vp, C.POINTER(MBVCoupling)]

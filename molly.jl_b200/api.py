@@ -1387,23 +1387,120 @@ def steepest_descent(sys: System, sim: SteepestDescentMinimizer, init_step: int 
     return sys, trace
 
 
-# simulator type -> its parameter struct and C entry point (each takes an optional log plan; NULL: no logging)
+# simulator type -> its parameter struct, C entry point and mb_simulate_group kind (each entry takes an optional log plan;
+# NULL: no logging)
 _SIMULATE_ENTRY = {
-    VelocityVerlet: (capi.MBVVParams, "mb_simulate_vv_log"),
-    Langevin: (capi.MBLangevinParams, "mb_simulate_langevin"),
-    LangevinSplitting: (capi.MBSplittingParams, "mb_simulate_langevin_splitting"),
-    NoseHoover: (capi.MBNoseHooverParams, "mb_simulate_nose_hoover"),
-    MTSIntegrator: (capi.MBMTSParams, "mb_simulate_mts"),
-    MTSLangevinIntegrator: (capi.MBMTSParams, "mb_simulate_mts"),
-    Verlet: (capi.MBVVParams, "mb_simulate_verlet"),
-    StormerVerlet: (capi.MBStormerParams, "mb_simulate_stormer_verlet"),
-    OverdampedLangevin: (capi.MBLangevinParams, "mb_simulate_overdamped_langevin"),
-    DPDVelocityVerlet: (capi.MBDpdVVParams, "mb_simulate_dpd_vv"),
+    VelocityVerlet: (capi.MBVVParams, "mb_simulate_vv_log", capi.MB_INTEG_VV),
+    Langevin: (capi.MBLangevinParams, "mb_simulate_langevin", capi.MB_INTEG_LANGEVIN),
+    LangevinSplitting: (capi.MBSplittingParams, "mb_simulate_langevin_splitting", capi.MB_INTEG_LANGEVIN_SPLITTING),
+    NoseHoover: (capi.MBNoseHooverParams, "mb_simulate_nose_hoover", capi.MB_INTEG_NOSE_HOOVER),
+    MTSIntegrator: (capi.MBMTSParams, "mb_simulate_mts", capi.MB_INTEG_MTS),
+    MTSLangevinIntegrator: (capi.MBMTSParams, "mb_simulate_mts", capi.MB_INTEG_MTS),
+    Verlet: (capi.MBVVParams, "mb_simulate_verlet", capi.MB_INTEG_VERLET),
+    StormerVerlet: (capi.MBStormerParams, "mb_simulate_stormer_verlet", capi.MB_INTEG_STORMER_VERLET),
+    OverdampedLangevin: (capi.MBLangevinParams, "mb_simulate_overdamped_langevin", capi.MB_INTEG_OVERDAMPED_LANGEVIN),
+    DPDVelocityVerlet: (capi.MBDpdVVParams, "mb_simulate_dpd_vv", capi.MB_INTEG_DPD_VV),
 }
 
 
-def simulate(sys: System, sim, n_steps: Optional[int] = None, init_step: int = 0, rng=None, max_retries: int = 2,
-             run_loggers=None):
+class _Call:
+    """One simulate call of `sim` on `sys`: the entry point, its parameter struct, the velocity coupling and MTS levels to
+    set on the context first, and the log plan (None: no loggers) for the loggers and arrays of `log_sys` (default sys)."""
+
+    def __init__(self, sys, sim, n_steps: int, init_step: int, rng, run_loggers, log_sys=None):
+        entry = next((e for t, e in _SIMULATE_ENTRY.items() if isinstance(sim, t)), None)
+        if entry is None:
+            raise TypeError(f"unsupported simulator {type(sim).__name__}")
+        params_t, self.entry, self.kind = entry
+        coupling = getattr(sim, "coupling", None)  # (LangevinSplitting, StormerVerlet, OverdampedLangevin have none)
+        couplings = coupling if isinstance(coupling, (tuple, list)) else ((coupling,) if coupling else ())
+        mts = params_t is capi.MBMTSParams
+        p = params_t()  # (zero-filled: no Andersen thermostat, no noise)
+        vc = None
+        if isinstance(sim, VelocityVerlet):
+            for c in couplings:
+                if isinstance(c, _SCALING_THERMOSTATS) and len(couplings) == 1:  # (one thermostat per run)
+                    vc = c.descriptor(sys.k)
+                elif isinstance(c, AndersenThermostat):
+                    p.andersen_kT = sys.k * c.temperature
+                    p.andersen_prob = sim.dt / c.coupling_const
+                else:
+                    raise TypeError(f"unsupported coupling {c!r} (the stock Molly path handles it)")
+        elif isinstance(sim, Verlet):
+            for c in couplings:
+                if not (isinstance(c, AndersenThermostat) and len(couplings) == 1):
+                    raise TypeError(f"unsupported coupling {c!r} with Verlet (the stock Molly path handles it)")
+                p.andersen_kT = sys.k * c.temperature
+                p.andersen_prob = sim.dt / c.coupling_const
+        elif couplings:
+            raise TypeError(f"unsupported coupling {couplings[0]!r} with {type(sim).__name__} (the stock Molly path handles it)")
+        self.levels = {}
+        if mts:
+            self.levels = mts_levels(sys, sim)
+            p.n_levels = len(sim.ordered_fractions)
+            p.fractions[:p.n_levels] = sim.ordered_fractions
+            p.langevin = int(isinstance(sim, MTSLangevinIntegrator))
+        if isinstance(sim, (Langevin, NoseHoover, MTSLangevinIntegrator, LangevinSplitting, OverdampedLangevin)):
+            p.kT = sys.k * sim.temperature
+        if isinstance(sim, (Langevin, MTSLangevinIntegrator, LangevinSplitting, OverdampedLangevin)):
+            p.friction = float(sim.friction)
+        if isinstance(sim, LangevinSplitting):
+            p.n_ops = len(sim.splitting)
+            p.ops = sim.splitting.encode()
+        if isinstance(sim, NoseHoover):
+            p.damping = float(sim.damping)
+        if isinstance(sim, DPDVelocityVerlet):
+            p.lambda_ = float(sim.lam)
+        p.dt = float(sim.dt)
+        p.n_steps = int(n_steps)
+        p.init_step = int(init_step)
+        if not isinstance(sim, StormerVerlet):  # (StormerVerlet never removes it)
+            p.remove_cm_every = int(sim.remove_CM_motion)
+        if not isinstance(sim, (NoseHoover, StormerVerlet, DPDVelocityVerlet)):  # (these draw nothing of their own)
+            rng = rng or np.random.default_rng()
+            p.rng_ctr1 = int(rng.integers(0, 2 ** 63))
+            p.rng_key = int(rng.integers(0, 2 ** 63))
+        self.p, self.vc = p, vc
+        log_sys = log_sys or sys
+        self.plan = (_LogPlan(log_sys, int(n_steps), int(init_step), run_loggers)
+                     if log_sys.loggers and run_loggers is not False else None)
+
+    def configure(self, sys):
+        """Set the call's velocity coupling (cleared when it has none) and MTS levels on sys's context."""
+        ctx = sys.engine()
+        capi.check(sys._L.mb_set_velocity_coupling(ctx, C.byref(self.vc) if self.vc is not None else None))
+        for kind, lv in self.levels.items():  # (an unchanged level array leaves the context as it is)
+            capi.check(sys._L.mb_set_specific_levels(ctx, kind, len(lv), lv.ctypes.data))
+
+    def log_arg(self):
+        return C.byref(self.plan.desc) if self.plan is not None else None
+
+    def run(self, sys, max_retries: int, rc=None, backup=None):
+        """Run the call on sys.coords / sys.velocities. rc: the status an attempt made elsewhere (mb_simulate_group) already
+        returned, and backup the host state from before it. After MB_ERR_CAPACITY a host state is restored and the call
+        repeated with doubled capacities; the records go to the loggers only after success."""
+        if rc is None:
+            host = not hasattr(sys.coords, "data_ptr")
+            backup = (sys.coords.copy(), sys.velocities.copy()) if host else None
+        scale = 1.0
+        for attempt in range(max_retries + 1):  # (a retry overwrites the records of the failed attempt)
+            if rc is None:
+                rc = getattr(sys._L, self.entry)(sys.engine(), _ptr(sys.coords), _ptr(sys.velocities), C.byref(self.p),
+                                                 self.log_arg())
+            if rc == capi.MB_ERR_CAPACITY and backup is not None and attempt < max_retries:
+                sys.coords[...], sys.velocities[...] = backup
+                scale *= 2.0
+                capi.check(sys._L.mb_set_capacity_scale(sys.engine(), scale))
+                rc = None
+                continue
+            capi.check(rc)
+            break
+        if self.plan is not None:
+            self.plan.push()
+
+
+def simulate(sys, sim, n_steps: Optional[int] = None, init_step: Optional[int] = None, rng=None, max_retries: int = 2,
+             run_loggers=None, assign_velocities: bool = False):
     """simulate!(sys, sim, ...) dispatched on the simulator's type.
 
     VelocityVerlet: simulate!(sys, sim, n_steps; run_loggers=true) — src/simulators.jl:547-668. Mutates sys.coords /
@@ -1423,7 +1520,21 @@ def simulate(sys: System, sim, n_steps: Optional[int] = None, init_step: int = 0
     DPDVelocityVerlet: simulate!(sys, sim, n_steps; run_loggers=true) — src/simulators.jl:711-842, the same arguments and
     loggers as VelocityVerlet; each call's first force evaluation uses the current velocities.
     SteepestDescentMinimizer: simulate!(sys, sim; run_loggers=false) — src/simulators.jl:183-274, see steepest_descent.
-    Loggers are not run during a minimisation (run_loggers must be false)."""
+    Loggers are not run during a minimisation (run_loggers must be false).
+    ReplicaExchangeMD on a ReplicaSystem: see simulate_remd (init_step defaults to sys.current_step there, and to 0 for
+    a System)."""
+    if isinstance(sim, ReplicaExchangeMD):
+        if not isinstance(sys, ReplicaSystem):
+            raise TypeError("simulate(sys, ::ReplicaExchangeMD, n_steps) needs a ReplicaSystem")
+        if n_steps is None:
+            raise TypeError("simulate(sys, ::ReplicaExchangeMD, n_steps) needs n_steps")
+        return simulate_remd(sys, sim, n_steps, init_step=init_step, assign_velocities=assign_velocities,
+                             run_loggers=True if run_loggers is None else run_loggers, rng=rng, max_retries=max_retries)
+    if isinstance(sys, ReplicaSystem):
+        raise TypeError(f"a ReplicaSystem runs with ReplicaExchangeMD, not {type(sim).__name__}")
+    if assign_velocities:
+        raise TypeError("assign_velocities is an argument of simulate(::ReplicaSystem, ::ReplicaExchangeMD, ...) only")
+    init_step = 0 if init_step is None else init_step
     if isinstance(sim, SteepestDescentMinimizer):
         if n_steps is not None:
             raise TypeError("simulate(sys, ::SteepestDescentMinimizer) takes no n_steps (the minimiser's max_steps bounds it)")
@@ -1431,84 +1542,255 @@ def simulate(sys: System, sim, n_steps: Optional[int] = None, init_step: int = 0
             raise NotImplementedError("loggers are not run during a minimisation on the device (run_loggers must be false)")
         steepest_descent(sys, sim, init_step=init_step, max_retries=max_retries)
         return sys
-    entry = next((e for t, e in _SIMULATE_ENTRY.items() if isinstance(sim, t)), None)
-    if entry is None:
+    if not any(isinstance(sim, t) for t in _SIMULATE_ENTRY):
         raise TypeError(f"unsupported simulator {type(sim).__name__}")
-    params_t, entry = entry
     if n_steps is None:
         raise TypeError(f"simulate(sys, ::{type(sim).__name__}, n_steps) needs n_steps")
     if run_loggers is None:
         run_loggers = True
     _check_run_loggers(run_loggers)
-    coupling = getattr(sim, "coupling", None)  # (LangevinSplitting, StormerVerlet, OverdampedLangevin have none)
-    couplings = coupling if isinstance(coupling, (tuple, list)) else ((coupling,) if coupling else ())
-    mts = params_t is capi.MBMTSParams
-    p = params_t()  # (zero-filled: no Andersen thermostat, no noise)
-    vc = None
-    if isinstance(sim, VelocityVerlet):
-        for c in couplings:
-            if isinstance(c, _SCALING_THERMOSTATS) and len(couplings) == 1:  # (one thermostat per run)
-                vc = c.descriptor(sys.k)
-            elif isinstance(c, AndersenThermostat):
-                p.andersen_kT = sys.k * c.temperature
-                p.andersen_prob = sim.dt / c.coupling_const
-            else:
-                raise TypeError(f"unsupported coupling {c!r} (the stock Molly path handles it)")
-    elif isinstance(sim, Verlet):
-        for c in couplings:
-            if not (isinstance(c, AndersenThermostat) and len(couplings) == 1):
-                raise TypeError(f"unsupported coupling {c!r} with Verlet (the stock Molly path handles it)")
-            p.andersen_kT = sys.k * c.temperature
-            p.andersen_prob = sim.dt / c.coupling_const
-    elif couplings:
-        raise TypeError(f"unsupported coupling {couplings[0]!r} with {type(sim).__name__} (the stock Molly path handles it)")
-    if mts:
-        levels = mts_levels(sys, sim)
-        p.n_levels = len(sim.ordered_fractions)
-        p.fractions[:p.n_levels] = sim.ordered_fractions
-        p.langevin = int(isinstance(sim, MTSLangevinIntegrator))
-    if isinstance(sim, (Langevin, NoseHoover, MTSLangevinIntegrator, LangevinSplitting, OverdampedLangevin)):
-        p.kT = sys.k * sim.temperature
-    if isinstance(sim, (Langevin, MTSLangevinIntegrator, LangevinSplitting, OverdampedLangevin)):
-        p.friction = float(sim.friction)
-    if isinstance(sim, LangevinSplitting):
-        p.n_ops = len(sim.splitting)
-        p.ops = sim.splitting.encode()
-    if isinstance(sim, NoseHoover):
-        p.damping = float(sim.damping)
-    if isinstance(sim, DPDVelocityVerlet):
-        p.lambda_ = float(sim.lam)
-    p.dt = float(sim.dt)
-    p.n_steps = int(n_steps)
-    p.init_step = int(init_step)
-    if not isinstance(sim, StormerVerlet):  # (StormerVerlet never removes it)
-        p.remove_cm_every = int(sim.remove_CM_motion)
-    ctx = sys.engine()
-    capi.check(sys._L.mb_set_velocity_coupling(ctx, C.byref(vc) if vc is not None else None))  # (Langevin, NoseHoover: cleared)
-    if mts:  # (an unchanged level array leaves the context as it is)
-        for kind, lv in levels.items():
-            capi.check(sys._L.mb_set_specific_levels(ctx, kind, len(lv), lv.ctypes.data))
-    if not isinstance(sim, (NoseHoover, StormerVerlet, DPDVelocityVerlet)):  # (these draw nothing of their own)
-        rng = rng or np.random.default_rng()
-        p.rng_ctr1 = int(rng.integers(0, 2 ** 63))
-        p.rng_key = int(rng.integers(0, 2 ** 63))
-    host = not hasattr(sys.coords, "data_ptr")
-    backup = (sys.coords.copy(), sys.velocities.copy()) if host else None
-    plan = _LogPlan(sys, int(n_steps), int(init_step), run_loggers) if sys.loggers and run_loggers is not False else None
-    scale = 1.0
-    for attempt in range(max_retries + 1):  # (a retry overwrites the records of the failed attempt)
-        rc = getattr(sys._L, entry)(ctx, _ptr(sys.coords), _ptr(sys.velocities), C.byref(p),
-                                    C.byref(plan.desc) if plan is not None else None)
-        if rc == capi.MB_ERR_CAPACITY and backup is not None and attempt < max_retries:
-            sys.coords[...], sys.velocities[...] = backup
-            scale *= 2.0
-            capi.check(sys._L.mb_set_capacity_scale(ctx, scale))
-            continue
-        capi.check(rc)
-        break
-    if plan is not None:
-        plan.push()
+    call = _Call(sys, sim, int(n_steps), int(init_step), rng, run_loggers)
+    call.configure(sys)  # (Langevin, NoseHoover: the coupling is cleared)
+    call.run(sys, max_retries)
     return sys
+
+
+# ------------------------------------------------------------------------------------------------
+# temperature replica exchange (src/types.jl:1183-1427, src/simulators.jl:1942-2206, src/loggers.jl:1170-1218)
+# ------------------------------------------------------------------------------------------------
+class ThermoState:
+    """ThermoState(system, integrator; temperature) — src/types.jl:1211-1280: one thermodynamic state, beta = 1 / (k T)
+    with k = system.k. Without `temperature` it is the thermostat coupling's temperature, or else the integrator's.
+    Pressure (a barostat's state) is not provided."""
+
+    def __init__(self, system, integrator, temperature=None, pressure=None, name=None):
+        if pressure is not None:
+            raise TypeError("ThermoState pressure (constant-pressure replica exchange) is not provided; the stock Molly "
+                            "path handles it")
+        coupling = getattr(integrator, "coupling", None)
+        for c in coupling if isinstance(coupling, (tuple, list)) else ((coupling,) if coupling else ()):
+            if temperature is None and hasattr(c, "temperature"):
+                temperature = c.temperature
+        if temperature is None:
+            temperature = getattr(integrator, "temperature", None)
+        if temperature is None:
+            raise ValueError("no temperature provided or inferred from the integrator: give one explicitly, use a "
+                             "thermostat, or use an integrator with a temperature")
+        self.system, self.integrator, self.name = system, integrator, name
+        self.temperature = float(temperature)
+        self.beta = 1.0 / (system.k * self.temperature)
+
+
+class ReplicaExchangeLogger:
+    """ReplicaExchangeLogger(n_replicas) — src/loggers.jl:1170-1218: the accepted exchanges (the pair of physical
+    replica indices, 0-based, the step and Delta of each) and the number of attempts."""
+
+    def __init__(self, n_replicas: int):
+        self.n_replicas = int(n_replicas)
+        self.n_attempts = self.n_exchanges = self.end_step = 0
+        self.indices, self.steps, self.deltas = [], [], []
+
+
+class ReplicaExchangeMD:
+    """ReplicaExchangeMD(dt, exchange_time) — src/simulators.jl:1953-1963."""
+
+    def __init__(self, dt, exchange_time):
+        if not exchange_time > dt:
+            raise ValueError(f"exchange time ({exchange_time}) must be greater than the time step ({dt})")
+        self.dt, self.exchange_time = float(dt), float(exchange_time)
+
+
+class ReplicaSystem:
+    """ReplicaSystem(thermo_states, replica_coords; replica_velocities, replica_loggers, exchange_logger, initial_step) —
+    src/types.jl:1343-1427, for states that share one System (temperature replica exchange). Holds the coordinates and
+    velocities of every physical replica (numpy, or torch CUDA tensors), state_indices (physical replica -> state, 0-based,
+    starting at the identity), current_step and the exchange logger. replica_loggers[i] is a dict of loggers like
+    System.loggers. Each state runs on a private engine context of its own, so its captured step graphs survive every
+    exchange."""
+
+    def __init__(self, thermo_states, replica_coords, replica_velocities=None, replica_boundaries=None,
+                 replica_neighbor_finders=None, replica_loggers=None, exchange_logger=None, initial_step: int = 0):
+        self.thermo_states = list(thermo_states)
+        n = self.n_replicas = len(self.thermo_states)
+        if n < 1:
+            raise ValueError("a ReplicaSystem needs at least one ThermoState")
+        if int(initial_step) < 0:
+            raise ValueError("initial_step must be non-negative")
+        base = self.thermo_states[0].system
+        if any(ts.system is not base for ts in self.thermo_states):
+            raise TypeError("ThermoStates on different Systems (Hamiltonian replica exchange) are not provided: every "
+                            "state must share one System; the stock Molly path handles it")
+        if replica_boundaries is not None or replica_neighbor_finders is not None:
+            raise TypeError("per-replica boundaries or neighbour finders are not provided; the stock Molly path handles them")
+        for ts in self.thermo_states:
+            if not any(isinstance(ts.integrator, t) for t in _SIMULATE_ENTRY):
+                raise TypeError(f"unsupported integrator {type(ts.integrator).__name__} for replica exchange; the stock Molly "
+                                "path handles it")
+        for name, arg in (("replica_coords", replica_coords), ("replica_velocities", replica_velocities),
+                          ("replica_loggers", replica_loggers)):
+            if arg is not None and len(arg) != n:
+                raise ValueError(f"{len(arg)} {name} for {n} ThermoStates")
+        self.system = base
+        self.k, self.n, self.dtype = base.k, base.n, base.dtype
+        self.replica_coords = [base._as_state(x) for x in replica_coords]
+        if replica_velocities is None:
+            replica_velocities = [x.clone().zero_() if hasattr(x, "data_ptr") else np.zeros_like(x) for x in self.replica_coords]
+        self.replica_velocities = [base._as_state(v) for v in replica_velocities]
+        self.replica_loggers = [dict(lg or {}) for lg in (replica_loggers or [None] * n)]
+        for lgs in self.replica_loggers:
+            for name, lg in lgs.items():
+                if type(lg) not in _LOGGER_TYPES:
+                    raise TypeError(f"logger {name!r}: {type(lg).__name__} is not supported")
+        self.exchange_logger = exchange_logger if exchange_logger is not None else ReplicaExchangeLogger(n)
+        self.state_indices = list(range(n))
+        self.betas = [ts.beta for ts in self.thermo_states]
+        self.current_step = int(initial_step)
+        self.initial_log_pending = True
+        self._state_sys = [None] * n
+
+    def state_system(self, s: int) -> System:
+        """The private System of state s: the shared System's Hamiltonian on a context of its own, no loggers."""
+        if self._state_sys[s] is None:
+            import copy
+            st = copy.copy(self.system)
+            st._ctx, st.loggers = None, {}
+            self._state_sys[s] = st
+        return self._state_sys[s]
+
+    def close(self):
+        for st in self._state_sys:
+            if st is not None:
+                st.close()
+
+
+class _ReplicaView:
+    """What _LogPlan reads of a System, for one physical replica's arrays and loggers."""
+
+    def __init__(self, repsys, i):
+        self.loggers, self.coords = repsys.replica_loggers[i], repsys.replica_coords[i]
+        self.n, self.dtype, self.k = repsys.n, repsys.dtype, repsys.k
+
+
+class _EngineRunner:
+    """Runs a cycle's calls (one per state that holds a replica) as one mb_simulate_group call, and evaluates U on a
+    state's context. The seam tests substitute to drive simulate_remd with other integrators."""
+
+    def run(self, repsys, calls, max_retries):
+        """calls: [(state, _Call)], the state's System holding its replica's arrays. Members that hit MB_ERR_CAPACITY
+        are retried one at a time through the single call."""
+        L = capi.load()
+        members = (capi.MBGroupMember * len(calls))()
+        backups = []
+        for m, (s, call) in zip(members, calls):
+            st = repsys.state_system(s)
+            call.configure(st)
+            m.ctx, m.coords, m.vels, m.kind = st.engine(), _ptr(st.coords), _ptr(st.velocities), call.kind
+            m.params = C.addressof(call.p)
+            m.log = C.addressof(call.plan.desc) if call.plan is not None else None
+            host = not hasattr(st.coords, "data_ptr")
+            backups.append((st.coords.copy(), st.velocities.copy()) if host else None)
+        rc = L.mb_simulate_group(len(calls), members)
+        if rc == capi.MB_ERR_INVALID and all(m.status == capi.MB_ERR_INVALID for m in members):
+            capi.check(rc)  # (refused before any work)
+        for m, (s, call), backup in zip(members, calls, backups):
+            call.run(repsys.state_system(s), max_retries, rc=m.status, backup=backup)
+
+    def energy(self, repsys, s, coords):
+        st = repsys.state_system(s)
+        st.coords = coords
+        return potential_energy(st)
+
+
+def _scale_velocities(v, factor, dtype):
+    """v *= factor in place, the factor (computed in f64) cast to the state dtype first."""
+    if hasattr(v, "data_ptr"):
+        v.mul_(float(np.asarray(factor, dtype)))
+    else:
+        v *= np.asarray(factor, dtype)
+
+
+def simulate_remd(repsys: ReplicaSystem, sim: ReplicaExchangeMD, n_steps: int, init_step: Optional[int] = None,
+                  assign_velocities: bool = False, run_loggers=True, rng=None, max_retries: int = 2, runner=None):
+    """simulate!(repsys, ::ReplicaExchangeMD, n_steps; init_step=repsys.current_step, assign_velocities, run_loggers, rng) —
+    src/simulators.jl:1965-2206 for temperature replica exchange.
+
+    n_cycles = (n_steps dt) // exchange_time and cycle_length = n_steps // n_cycles; the remaining n_steps % n_cycles
+    steps run after the last cycle, with no exchange after them. In cycle c (1-based) physical replica i runs cycle_length
+    steps of the integrator of state state_indices[i] from step init_step + (c - 1) cycle_length, on that state's context;
+    the states' calls run together (mb_simulate_group). Loggers run with run_loggers = True while
+    repsys.initial_log_pending is set and with "skipstart" after that. Then exchanges are attempted between adjacent
+    physical replicas (i, i + 1), i = 1, 3, ... (0-based) in odd cycles and i = 0, 2, ... in even ones:
+    Delta = (beta_n - beta_m)(U(x_i) - U(x_j)), m and n the states of i and j and U the potential energy of the replica's
+    final coordinates, accepted when Delta <= 0 or rng.random() < exp(-Delta). On acceptance the states swap and the
+    velocities scale, v_i *= sqrt(beta_m / beta_n), v_j *= sqrt(beta_n / beta_m) (the factor computed in f64 and cast to
+    the system dtype); the exchange logger records (i, j), the step init_step + c cycle_length and Delta.
+
+    The draws from `rng`, in order: with assign_velocities, random_velocities of each replica at its state's temperature,
+    in physical order; then per cycle (and for the remainder) the integrator keys of each replica in physical order (the
+    two rng.integers draws simulate makes, for integrators that draw), and that cycle's exchange uniforms, one per
+    attempt with Delta > 0, in pair order."""
+    if not isinstance(repsys, ReplicaSystem):
+        raise TypeError("simulate_remd needs a ReplicaSystem")
+    _check_run_loggers(run_loggers)
+    rng = rng or np.random.default_rng()
+    runner = runner or _EngineRunner()
+    init_step = repsys.current_step if init_step is None else int(init_step)
+    n_steps = int(n_steps)
+    R = repsys.n_replicas
+    repsys.current_step = init_step
+    n_cycles = int((n_steps * sim.dt) // sim.exchange_time)
+    cycle_length = n_steps // n_cycles if n_cycles > 0 else 0
+    remaining = n_steps % n_cycles if n_cycles > 0 else n_steps
+    if assign_velocities:
+        for i in range(R):
+            s = repsys.state_indices[i]
+            v = random_velocities(repsys.state_system(s), repsys.thermo_states[s].temperature, rng)
+            if hasattr(repsys.replica_velocities[i], "data_ptr"):
+                import torch
+                repsys.replica_velocities[i].copy_(torch.from_numpy(v))
+            else:
+                repsys.replica_velocities[i][...] = v
+
+    def run_cycle(length, start):
+        rl = False if run_loggers is False else (True if repsys.initial_log_pending else "skipstart")
+        calls = []
+        for i in range(R):
+            s = repsys.state_indices[i]
+            st = repsys.state_system(s)
+            st.coords, st.velocities = repsys.replica_coords[i], repsys.replica_velocities[i]
+            calls.append((s, _Call(st, repsys.thermo_states[s].integrator, length, start, rng, rl, _ReplicaView(repsys, i))))
+        runner.run(repsys, calls, max_retries)
+        repsys.initial_log_pending = False
+
+    n_attempts = 0
+    xl = repsys.exchange_logger
+    for cycle in range(1, n_cycles + 1):
+        run_cycle(cycle_length, init_step + (cycle - 1) * cycle_length)
+        for i in range(cycle % 2, R - 1, 2):
+            j = i + 1
+            n_attempts += 1
+            m, n = repsys.state_indices[i], repsys.state_indices[j]
+            bm, bn = repsys.betas[m], repsys.betas[n]
+            ui = runner.energy(repsys, m, repsys.replica_coords[i])
+            uj = runner.energy(repsys, n, repsys.replica_coords[j])
+            delta = (bn - bm) * (float(ui) - float(uj))
+            if delta <= 0 or rng.random() < math.exp(-delta):
+                repsys.state_indices[i], repsys.state_indices[j] = n, m
+                if bm != bn:
+                    _scale_velocities(repsys.replica_velocities[i], math.sqrt(bm / bn), repsys.dtype)
+                    _scale_velocities(repsys.replica_velocities[j], math.sqrt(bn / bm), repsys.dtype)
+                if run_loggers is not False and xl is not None:
+                    xl.indices.append((i, j))
+                    xl.steps.append(init_step + cycle * cycle_length)
+                    xl.deltas.append(delta)
+                    xl.n_exchanges += 1
+    if remaining > 0:
+        run_cycle(remaining, init_step + n_cycles * cycle_length)
+    if run_loggers is not False and xl is not None:
+        xl.end_step = init_step + n_steps
+        xl.n_attempts += n_attempts
+    repsys.current_step = init_step + n_steps
+    return repsys
 
 
 def kinetic_energy(sys: System) -> float:

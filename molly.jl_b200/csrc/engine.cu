@@ -420,6 +420,12 @@ class EngineBase {
     virtual int forces_energy(const void* coords, void* fs, void* pe, void* vir, int64_t step_n, bool with_specific,
                               const void* vels) = 0;
     virtual int simulate(void* coords, void* vels, const Integrator& ig, mb_log_t* log) = 0;
+    // simulate's phases, for mb_simulate_group (single-GPU contexts only): sim_begin, then sim_step(k) for k = 1 ..
+    // ig.n_steps, then sim_end
+    virtual int sim_begin(void* coords, void* vels, const Integrator& ig, mb_log_t* log) = 0;
+    virtual int sim_step(int64_t k) = 0;
+    virtual int sim_end() = 0;
+    virtual bool is_decomposed() const = 0;
     virtual int remove_cm(void* vels) = 0;
     virtual int kinetic_energy(const void* vels, double* out) = 0;
     virtual int rebuild(const void* coords) = 0;
@@ -2838,22 +2844,49 @@ class Engine : public EngineBase {
         return MB_OK;
     }
 
-    // Every mb_simulate_* entry point: one prologue and epilogue; in between, the single-GPU step graphs or stream loop, or
-    // the decomposed steps (simulate_decomposed)
+    // One simulate call in flight on this context, from sim_begin to sim_end (a context runs one call at a time)
+    struct SimRun {
+        Integrator ig;
+        StepCfg c;
+        mb_log_t* log = nullptr;
+        LogRun lr;
+        CallerBuf xb, vb;
+        bool dec = false, cm_pending = false;  // cm_pending: host mirror of cm->valid
+    } run_;
+
+    // Every mb_simulate_* entry point: the prologue (sim_begin), the steps (sim_step; a decomposed run steps in
+    // simulate_decomposed) and the epilogue (sim_end). mb_simulate_group runs the same phases with several contexts'
+    // steps interleaved.
     int simulate(void* coords, void* vels, const Integrator& call, mb_log_t* log) override {
+        MB_TRY(sim_begin(coords, vels, call, log));
+        if (run_.dec) {
+            MB_TRY(simulate_decomposed(run_.c, run_.cm_pending));
+        } else {
+            for (int64_t k = 1; k <= run_.ig.n_steps; k++) MB_TRY(sim_step(k));
+        }
+        return sim_end();
+    }
+    bool is_decomposed() const override { return decomposed(); }
+    // everything up to the first step: refusals, ingest, the call's Control tail, F0, the loggers at init_step and the
+    // step graphs this call launches
+    int sim_begin(void* coords, void* vels, const Integrator& call, mb_log_t* log) override {
         MB_TRY(prepare());
         MB_TRY(check_simulate(coords, vels, call));
-        const bool dec = decomposed() && path_ == 1;  // a decomposed run: each rank integrates its slab (simulate_decomposed)
+        run_ = SimRun{};
+        run_.dec = decomposed() && path_ == 1;  // a decomposed run: each rank integrates its slab (simulate_decomposed)
+        run_.log = log;
         // one level without noise is the VelocityVerlet step: it runs as one (after the refusals, which name mb_simulate_mts)
-        Integrator ig = call;
+        Integrator& ig = run_.ig;
+        ig = call;
         if (ig.kind == INTEG_MTS && ig.n_levels == 1) {
             ig.kind = INTEG_VV;
             ig.n_levels = 0;
             ig.fractions.fill(0);
         }
-        LogRun lr;
+        const bool dec = run_.dec;
+        LogRun& lr = run_.lr;
         MB_TRY(log_begin(log, ig, lr));
-        CallerBuf xb, vb;
+        CallerBuf &xb = run_.xb, &vb = run_.vb;
         MB_TRY(caller_xyz(coords, d_stage_a_, true, xb));
         MB_TRY(caller_xyz(vels, d_stage_c_, true, vb));
         const int nb = (int)((n_ + 255) / 256);
@@ -2862,7 +2895,8 @@ class Engine : public EngineBase {
         clear_cm_kernel<T><<<1, 1, 0, stream_>>>(cm);
         launches_++;
         if (ig.kind == INTEG_NH) MB_CUDA(cudaMemsetAsync(d_nh_.p, 0, sizeof(NhState), stream_));  // zeta = 0 at the start of every call
-        StepCfg c = step_cfg(ig);
+        StepCfg& c = run_.c;
+        c = step_cfg(ig);
         if (c.ig.n_levels > 1) MB_CUDA(d_f4_mts_.ensure(((size_t)n_ + 16) * sizeof(T4)));
         if (path_ == 0) {
             init_slots(xb.as<T>());
@@ -2893,7 +2927,6 @@ class Engine : public EngineBase {
                                     cudaMemcpyHostToDevice, stream_));
             MB_CUDA(cudaStreamSynchronize(stream_));  // t is a local
         }
-        bool cm_pending = false;  // host mirror of cm->valid
         if (ig.init_step == 0 && ig.remove_cm_every != 0) {
             // remove_CM_motion! before the first force evaluation (simulators.jl:563): zero-length kick
             int grid;
@@ -2902,81 +2935,86 @@ class Engine : public EngineBase {
                                                                         d_vel4_.as<T4>(), d_partial_.as<double>(), ctl, cm, nullptr,
                                                                         PeerSignal{}, VCouple{});
             launches_++;
-            cm_pending = true;
+            run_.cm_pending = true;
         }
         if (c.ig.kind == INTEG_DPD_VV && dpd_on_) {  // F0 with the current velocities: v_pred = v after the pending v_cm
             dpd_vpred_init_kernel<T><<<nb, 256, 0, stream_>>>((int)n_, d_vel4_.as<T4>(), d_orig_.as<int>(), cm, d_vpred4_.as<T4>());
             launches_++;
         }
-        if (dec) {
-            MB_TRY(simulate_decomposed(c, cm_pending));
-        } else {
-            MB_TRY(launch_pairs(false, d_f4_.as<T4>()));
-            MB_TRY(launch_bonded(false, nullptr, is_mts(c.ig.kind) ? 0 : -1));  // (multiple time steps: F_0 of level 0)
-            if (log && log->log_initial) {  // apply_loggers! at init_step (run_loggers == true), after F0
-                const int m = log_mask_at(log, ig.init_step);
-                if (m) {
-                    MB_TRY(enqueue_log(c, m));
-                    MB_TRY(log_step(lr, m));
-                }
+        if (dec) return MB_OK;  // (simulate_decomposed evaluates F0 itself)
+        MB_TRY(launch_pairs(false, d_f4_.as<T4>()));
+        MB_TRY(launch_bonded(false, nullptr, is_mts(c.ig.kind) ? 0 : -1));  // (multiple time steps: F_0 of level 0)
+        if (log && log->log_initial) {  // apply_loggers! at init_step (run_loggers == true), after F0
+            const int m = log_mask_at(log, ig.init_step);
+            if (m) {
+                MB_TRY(enqueue_log(c, m));
+                MB_TRY(log_step(lr, m));
             }
+        }
 
-            // CUDA-graph path: static per-step sequence (remove_CM_motion in {0,1})
-            bool use_graph = graphs_usable() && c.do_cm >= 0 && ig.n_steps >= 4;
-            if (use_graph) {
-                // one executable per log mask this call uses (the plain step and the log steps)
-                bool need[8] = {false, false, false, false, false, false, false, false};
-                for (int64_t k = 1; k <= ig.n_steps; k++) need[log_mask_at(log, ig.init_step + k)] = true;
-                GraphKey key{ig, vcoupling, 0};
-                for (int m = 0; m < 8 && use_graph; m++) {
-                    if (!need[m]) continue;
-                    key.log_mask = m;
-                    if (!graphs_[m].exec || !(key == graphs_[m].key)) {
-                        if (build_step_graph(c, key) != MB_OK) {
-                            graph_failed_ = true;  // stay on the stream path for this context
-                            use_graph = false;
-                        }
+        // CUDA-graph path: static per-step sequence (remove_CM_motion in {0,1})
+        bool use_graph = graphs_usable() && c.do_cm >= 0 && ig.n_steps >= 4;
+        if (use_graph) {
+            // one executable per log mask this call uses (the plain step and the log steps)
+            bool need[8] = {false, false, false, false, false, false, false, false};
+            for (int64_t k = 1; k <= ig.n_steps; k++) need[log_mask_at(log, ig.init_step + k)] = true;
+            GraphKey key{ig, vcoupling, 0};
+            for (int m = 0; m < 8 && use_graph; m++) {
+                if (!need[m]) continue;
+                key.log_mask = m;
+                if (!graphs_[m].exec || !(key == graphs_[m].key)) {
+                    if (build_step_graph(c, key) != MB_OK) {
+                        graph_failed_ = true;  // stay on the stream path for this context
+                        use_graph = false;
                     }
                 }
             }
-            graph_used_ = use_graph;
-            if (use_graph) {
-                for (int64_t k = 1; k <= ig.n_steps; k++) {
-                    const int m = log_mask_at(log, ig.init_step + k);
-                    MB_CUDA(cudaGraphLaunch(graphs_[m].exec, stream_));
-                    launches_ += graphs_[m].launches;  // rebuild-body kernels are not counted
-                    n_force_evals_ += graphs_[m].evals;
-                    MB_TRY(log_step(lr, m));
-                }
-                n_steps_ += ig.n_steps;
-            } else {
-                for (int64_t k = 1; k <= ig.n_steps; k++) {
-                    const int64_t step_n = ig.init_step + k;
-                    const int do_cm = (ig.remove_cm_every != 0 && step_n % ig.remove_cm_every == 0) ? 1 : 0;
-                    StepOpts o;
-                    o.do_cm = do_cm;
-                    o.clear_cm_after_k1 = cm_pending && !do_cm;  // K1 consumed v_cm; nothing overwrites it this step
-                    o.rebuild_hint = rebuild_every_ > 0 && k > 1 && (step_n - 1) % rebuild_every_ == 0;
-                    o.log_mask = log_mask_at(log, step_n);
-                    MB_TRY(enqueue_step(c, o));
-                    MB_TRY(log_step(lr, o.log_mask));
-                    cm_pending = do_cm != 0;
-                    n_steps_++;
-                }
-            }
-            if (thermo_in_k1(c).on && ig.n_steps > 0) {
-                // the thermostat of the last step (the earlier ones ran inside the next step's drift kernel)
-                andersen_kernel<T><<<nb, 256, 0, stream_>>>(0, (int)n_, (int)n_, c.kT, c.ig.andersen_prob, d_orig_.as<int>(), d_mass_.as<T>(), d_vel4_.as<T4>(), cm, ctl);
-                launches_++;
-            }
+        }
+        graph_used_ = use_graph;
+        return MB_OK;
+    }
+    // step k (1 .. n_steps) of the call sim_begin started: one graph launch, or the step enqueued on the stream
+    int sim_step(int64_t k) override {
+        const Integrator& ig = run_.ig;
+        const int64_t step_n = ig.init_step + k;
+        if (graph_used_) {
+            const int m = log_mask_at(run_.log, step_n);
+            MB_CUDA(cudaGraphLaunch(graphs_[m].exec, stream_));
+            launches_ += graphs_[m].launches;  // rebuild-body kernels are not counted
+            n_force_evals_ += graphs_[m].evals;
+            MB_TRY(log_step(run_.lr, m));
+        } else {
+            const int do_cm = (ig.remove_cm_every != 0 && step_n % ig.remove_cm_every == 0) ? 1 : 0;
+            StepOpts o;
+            o.do_cm = do_cm;
+            o.clear_cm_after_k1 = run_.cm_pending && !do_cm;  // K1 consumed v_cm; nothing overwrites it this step
+            o.rebuild_hint = rebuild_every_ > 0 && k > 1 && (step_n - 1) % rebuild_every_ == 0;
+            o.log_mask = log_mask_at(run_.log, step_n);
+            MB_TRY(enqueue_step(run_.c, o));
+            MB_TRY(log_step(run_.lr, o.log_mask));
+            run_.cm_pending = do_cm != 0;
+        }
+        n_steps_++;
+        return MB_OK;
+    }
+    // after the last step: the last step's thermostat, export, copy-back, the loggers' records and the overflow check
+    int sim_end() override {
+        const StepCfg& c = run_.c;
+        const int nb = (int)((n_ + 255) / 256);
+        CmState<T>* cm = d_cm_.as<CmState<T>>();
+        if (!run_.dec && thermo_in_k1(c).on && c.ig.n_steps > 0) {
+            // the thermostat of the last step (the earlier ones ran inside the next step's drift kernel)
+            andersen_kernel<T><<<nb, 256, 0, stream_>>>(0, (int)n_, (int)n_, c.kT, c.ig.andersen_prob, d_orig_.as<int>(), d_mass_.as<T>(), d_vel4_.as<T4>(), cm, d_ctl_.as<Control>());
+            launches_++;
         }
         // export
+        const CallerBuf &xb = run_.xb, &vb = run_.vb;
         export_kernel<T><<<nb, 256, 0, stream_>>>((int)n_, geom(), d_pos4_.as<T4>(), d_vel4_.as<T4>(), d_orig_.as<int>(), cm, xb.as<T>(),
                                                   vb.as<T>());
         launches_++;
         MB_TRY(copy_back_xyz(xb));
         MB_TRY(copy_back_xyz(vb));
-        MB_TRY(log_end(lr));
+        MB_TRY(log_end(run_.lr));
         MB_CUDA(cudaGetLastError());
         if (path_ == 1) MB_TRY(check_overflow_sync());
         else MB_CUDA(cudaStreamSynchronize(stream_));
@@ -3333,7 +3371,7 @@ struct mb_ctx {
     if (!(ctx) || !(ctx)->e) return mb::set_error(MB_ERR_INVALID, "null context"); \
     if (cudaSetDevice((ctx)->device) != cudaSuccess) return mb::set_error(MB_ERR_CUDA, "cudaSetDevice failed")
 
-// the fields every mb_simulate_* parameter struct has, and the draws' keys; each entry point adds its method's fields
+// the fields every mb_simulate_* parameter struct has, and the draws' keys; each kind adds its method's fields
 template <typename P>
 static mb::Integrator integrator_call(int kind, const P* p, uint64_t rng_ctr1, uint64_t rng_key) {
     mb::Integrator ig;
@@ -3345,6 +3383,78 @@ static mb::Integrator integrator_call(int kind, const P* p, uint64_t rng_ctr1, u
     ig.rng_ctr1 = rng_ctr1;
     ig.rng_key = rng_key;
     return ig;
+}
+// The integrator record of an MB_INTEG_* kind from that kind's mb_simulate_* parameter struct (non-null)
+static int integrator_from(int32_t kind, const void* params, mb::Integrator& ig) {
+    switch (kind) {
+        case MB_INTEG_VV:
+        case MB_INTEG_VERLET: {
+            const auto* p = static_cast<const mb_vv_params_t*>(params);
+            ig = integrator_call(kind == MB_INTEG_VV ? mb::INTEG_VV : mb::INTEG_VERLET, p, p->rng_ctr1, p->rng_key);
+            ig.andersen_kT = p->andersen_kT;
+            ig.andersen_prob = p->andersen_prob;
+            return MB_OK;
+        }
+        case MB_INTEG_LANGEVIN:
+        case MB_INTEG_OVERDAMPED_LANGEVIN: {
+            const auto* p = static_cast<const mb_langevin_params_t*>(params);
+            ig = integrator_call(kind == MB_INTEG_LANGEVIN ? mb::INTEG_LANGEVIN : mb::INTEG_OVERDAMPED, p, p->rng_ctr1, p->rng_key);
+            ig.kT = p->kT;
+            ig.friction = p->friction;
+            return MB_OK;
+        }
+        case MB_INTEG_NOSE_HOOVER: {
+            const auto* p = static_cast<const mb_nosehoover_params_t*>(params);
+            ig = integrator_call(mb::INTEG_NH, p, 0, 0);
+            ig.kT = p->kT;
+            ig.damping = p->damping;
+            return MB_OK;
+        }
+        case MB_INTEG_MTS: {
+            const auto* p = static_cast<const mb_mts_params_t*>(params);
+            ig = integrator_call(p->langevin ? mb::INTEG_MTS_LANGEVIN : mb::INTEG_MTS, p, p->rng_ctr1, p->rng_key);
+            ig.n_levels = p->n_levels;
+            std::copy_n(p->fractions, std::clamp(p->n_levels, 0, MB_MTS_MAX_LEVELS), ig.fractions.begin());
+            if (p->langevin) {  // (MTSIntegrator has neither)
+                ig.kT = p->kT;
+                ig.friction = p->friction;
+            }
+            return MB_OK;
+        }
+        case MB_INTEG_LANGEVIN_SPLITTING: {
+            const auto* p = static_cast<const mb_splitting_params_t*>(params);
+            ig = integrator_call(mb::INTEG_SPLIT, p, p->rng_ctr1, p->rng_key);
+            ig.kT = p->kT;
+            ig.friction = p->friction;
+            ig.n_ops = p->n_ops;
+            std::copy_n(p->ops, std::clamp(p->n_ops, 0, MB_SPLIT_MAX_OPS), ig.ops.begin());
+            return MB_OK;
+        }
+        case MB_INTEG_STORMER_VERLET: {
+            const auto* p = static_cast<const mb_stormer_params_t*>(params);
+            ig = mb::Integrator{};  // (no CM removal anywhere, so the prologue skips it too; no draws)
+            ig.kind = mb::INTEG_STORMER;
+            ig.dt = p->dt;
+            ig.n_steps = p->n_steps;
+            ig.init_step = p->init_step;
+            return MB_OK;
+        }
+        case MB_INTEG_DPD_VV: {
+            const auto* p = static_cast<const mb_dpd_vv_params_t*>(params);
+            ig = integrator_call(mb::INTEG_DPD_VV, p, 0, 0);  // (no draws of its own: the DPD draws are keyed by mb_dpd_t)
+            ig.lambda = p->lambda;
+            return MB_OK;
+        }
+        default: return MB_ERR_INVALID;
+    }
+}
+// one mb_simulate_* call: its parameters as an integrator record, then the context's simulate
+static int simulate_entry(mb_ctx* ctx, void* coords, void* vels, int32_t kind, const void* p, mb_log_t* log) {
+    MB_CTX_GUARD(ctx);
+    if (!p) return mb::set_error(MB_ERR_INVALID, "null argument");
+    mb::Integrator ig;
+    integrator_from(kind, p, ig);
+    return ctx->e->simulate(coords, vels, ig, log);
 }
 
 extern "C" {
@@ -3456,83 +3566,71 @@ int mb_random_velocities(mb_ctx* ctx, void* vels, double kT, uint64_t rng_ctr1, 
 int mb_kinetic_energy_tensor(mb_ctx* ctx, const void* vels, double* ke_tensor9_host) { MB_CTX_GUARD(ctx); return ctx->e->kinetic_tensor(vels, ke_tensor9_host); }
 int mb_simulate_vv(mb_ctx* ctx, void* coords, void* vels, const mb_vv_params_t* p) { return mb_simulate_vv_log(ctx, coords, vels, p, nullptr); }
 int mb_simulate_vv_log(mb_ctx* ctx, void* coords, void* vels, const mb_vv_params_t* p, mb_log_t* log) {
-    MB_CTX_GUARD(ctx);
-    if (!p) return mb::set_error(MB_ERR_INVALID, "null argument");
-    mb::Integrator ig = integrator_call(mb::INTEG_VV, p, p->rng_ctr1, p->rng_key);
-    ig.andersen_kT = p->andersen_kT;
-    ig.andersen_prob = p->andersen_prob;
-    return ctx->e->simulate(coords, vels, ig, log);
+    return simulate_entry(ctx, coords, vels, MB_INTEG_VV, p, log);
 }
 int mb_simulate_langevin(mb_ctx* ctx, void* coords, void* vels, const mb_langevin_params_t* p, mb_log_t* log) {
-    MB_CTX_GUARD(ctx);
-    if (!p) return mb::set_error(MB_ERR_INVALID, "null argument");
-    mb::Integrator ig = integrator_call(mb::INTEG_LANGEVIN, p, p->rng_ctr1, p->rng_key);
-    ig.kT = p->kT;
-    ig.friction = p->friction;
-    return ctx->e->simulate(coords, vels, ig, log);
+    return simulate_entry(ctx, coords, vels, MB_INTEG_LANGEVIN, p, log);
 }
 int mb_simulate_nose_hoover(mb_ctx* ctx, void* coords, void* vels, const mb_nosehoover_params_t* p, mb_log_t* log) {
-    MB_CTX_GUARD(ctx);
-    if (!p) return mb::set_error(MB_ERR_INVALID, "null argument");
-    mb::Integrator ig = integrator_call(mb::INTEG_NH, p, 0, 0);
-    ig.kT = p->kT;
-    ig.damping = p->damping;
-    return ctx->e->simulate(coords, vels, ig, log);
+    return simulate_entry(ctx, coords, vels, MB_INTEG_NOSE_HOOVER, p, log);
 }
 int mb_simulate_mts(mb_ctx* ctx, void* coords, void* vels, const mb_mts_params_t* p, mb_log_t* log) {
-    MB_CTX_GUARD(ctx);
-    if (!p) return mb::set_error(MB_ERR_INVALID, "null argument");
-    mb::Integrator ig = integrator_call(p->langevin ? mb::INTEG_MTS_LANGEVIN : mb::INTEG_MTS, p, p->rng_ctr1, p->rng_key);
-    ig.n_levels = p->n_levels;
-    std::copy_n(p->fractions, std::clamp(p->n_levels, 0, MB_MTS_MAX_LEVELS), ig.fractions.begin());
-    if (p->langevin) {  // (MTSIntegrator has neither)
-        ig.kT = p->kT;
-        ig.friction = p->friction;
-    }
-    return ctx->e->simulate(coords, vels, ig, log);
+    return simulate_entry(ctx, coords, vels, MB_INTEG_MTS, p, log);
 }
 int mb_simulate_langevin_splitting(mb_ctx* ctx, void* coords, void* vels, const mb_splitting_params_t* p, mb_log_t* log) {
-    MB_CTX_GUARD(ctx);
-    if (!p) return mb::set_error(MB_ERR_INVALID, "null argument");
-    mb::Integrator ig = integrator_call(mb::INTEG_SPLIT, p, p->rng_ctr1, p->rng_key);
-    ig.kT = p->kT;
-    ig.friction = p->friction;
-    ig.n_ops = p->n_ops;
-    std::copy_n(p->ops, std::clamp(p->n_ops, 0, MB_SPLIT_MAX_OPS), ig.ops.begin());
-    return ctx->e->simulate(coords, vels, ig, log);
+    return simulate_entry(ctx, coords, vels, MB_INTEG_LANGEVIN_SPLITTING, p, log);
 }
 int mb_simulate_verlet(mb_ctx* ctx, void* coords, void* vels, const mb_vv_params_t* p, mb_log_t* log) {
-    MB_CTX_GUARD(ctx);
-    if (!p) return mb::set_error(MB_ERR_INVALID, "null argument");
-    mb::Integrator ig = integrator_call(mb::INTEG_VERLET, p, p->rng_ctr1, p->rng_key);
-    ig.andersen_kT = p->andersen_kT;
-    ig.andersen_prob = p->andersen_prob;
-    return ctx->e->simulate(coords, vels, ig, log);
+    return simulate_entry(ctx, coords, vels, MB_INTEG_VERLET, p, log);
 }
 int mb_simulate_stormer_verlet(mb_ctx* ctx, void* coords, void* vels, const mb_stormer_params_t* p, mb_log_t* log) {
-    MB_CTX_GUARD(ctx);
-    if (!p) return mb::set_error(MB_ERR_INVALID, "null argument");
-    mb::Integrator ig;  // (no CM removal anywhere, so the prologue skips it too; no draws)
-    ig.kind = mb::INTEG_STORMER;
-    ig.dt = p->dt;
-    ig.n_steps = p->n_steps;
-    ig.init_step = p->init_step;
-    return ctx->e->simulate(coords, vels, ig, log);
+    return simulate_entry(ctx, coords, vels, MB_INTEG_STORMER_VERLET, p, log);
 }
 int mb_simulate_overdamped_langevin(mb_ctx* ctx, void* coords, void* vels, const mb_langevin_params_t* p, mb_log_t* log) {
-    MB_CTX_GUARD(ctx);
-    if (!p) return mb::set_error(MB_ERR_INVALID, "null argument");
-    mb::Integrator ig = integrator_call(mb::INTEG_OVERDAMPED, p, p->rng_ctr1, p->rng_key);
-    ig.kT = p->kT;
-    ig.friction = p->friction;
-    return ctx->e->simulate(coords, vels, ig, log);
+    return simulate_entry(ctx, coords, vels, MB_INTEG_OVERDAMPED_LANGEVIN, p, log);
 }
 int mb_simulate_dpd_vv(mb_ctx* ctx, void* coords, void* vels, const mb_dpd_vv_params_t* p, mb_log_t* log) {
-    MB_CTX_GUARD(ctx);
-    if (!p) return mb::set_error(MB_ERR_INVALID, "null argument");
-    mb::Integrator ig = integrator_call(mb::INTEG_DPD_VV, p, 0, 0);  // (no draws of its own: the DPD draws are keyed by mb_dpd_t)
-    ig.lambda = p->lambda;
-    return ctx->e->simulate(coords, vels, ig, log);
+    return simulate_entry(ctx, coords, vels, MB_INTEG_DPD_VV, p, log);
+}
+int mb_simulate_group(int32_t n, mb_group_member_t* members) {
+    if (n <= 0 || !members) return mb::set_error(MB_ERR_INVALID, "mb_simulate_group: n must be > 0 and members non-null");
+    for (int32_t i = 0; i < n; i++) members[i].status = MB_ERR_INVALID;  // (a refused group runs no member)
+    // every refusal before any work: a member the group cannot run leaves every member's buffers untouched
+    std::vector<mb::Integrator> ig(n);
+    for (int32_t i = 0; i < n; i++) {
+        const mb_group_member_t& m = members[i];
+        const std::string who = "mb_simulate_group: member " + std::to_string(i) + ": ";
+        if (!m.ctx || !m.ctx->e) return mb::set_error(MB_ERR_INVALID, who + "null context");
+        if (!m.params) return mb::set_error(MB_ERR_INVALID, who + "null params");
+        if (integrator_from(m.kind, m.params, ig[i]) != MB_OK) return mb::set_error(MB_ERR_INVALID, who + "unknown integrator kind");
+        if (m.ctx->device != members[0].ctx->device) return mb::set_error(MB_ERR_INVALID, who + "on another device than member 0");
+        if (m.ctx->e->is_decomposed()) return mb::set_error(MB_ERR_INVALID, who + "a decomposed (multi-GPU) context");
+        for (int32_t j = 0; j < i; j++)
+            if (members[j].ctx == m.ctx) return mb::set_error(MB_ERR_INVALID, who + "the same context as member " + std::to_string(j));
+    }
+    if (cudaSetDevice(members[0].ctx->device) != cudaSuccess) return mb::set_error(MB_ERR_CUDA, "cudaSetDevice failed");
+    // The phases of mb_simulate_* for every member; the steps round-robin, one per member per round, each on its own
+    // context's stream, so that the members' kernels may run at the same time. A member that fails drops out where the
+    // single call would have returned.
+    std::vector<std::string> err(n);
+    auto outcome = [&](int32_t i, int rc) {
+        members[i].status = rc;
+        if (rc != MB_OK) err[i] = mb::g_last_error;
+    };
+    int64_t rounds = 0;
+    for (int32_t i = 0; i < n; i++) {
+        outcome(i, members[i].ctx->e->sim_begin(members[i].coords, members[i].vels, ig[i], members[i].log));
+        rounds = std::max(rounds, ig[i].n_steps);
+    }
+    for (int64_t k = 1; k <= rounds; k++)
+        for (int32_t i = 0; i < n; i++)
+            if (members[i].status == MB_OK && k <= ig[i].n_steps) outcome(i, members[i].ctx->e->sim_step(k));
+    for (int32_t i = 0; i < n; i++)
+        if (members[i].status == MB_OK) outcome(i, members[i].ctx->e->sim_end());
+    for (int32_t i = 0; i < n; i++)
+        if (members[i].status != MB_OK)
+            return mb::set_error(members[i].status, "mb_simulate_group: member " + std::to_string(i) + ": " + err[i]);
+    return MB_OK;
 }
 int mb_minimize_sd(mb_ctx* ctx, void* coords, mb_sd_params_t* p) { MB_CTX_GUARD(ctx); return ctx->e->minimize_sd(coords, p); }
 int mb_set_velocity_coupling(mb_ctx* ctx, const mb_vcoupling_t* c) {
