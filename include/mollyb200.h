@@ -163,8 +163,12 @@ int mb_forces_energy(mb_ctx* ctx, const void* coords, void* fs_mat, void* pe, vo
  *  - RBTorsion: the force is -grad E of the reference's own energy, (f1 (1 + cos th) + f2 (1 - cos 2th) + f3 (1 + cos 3th)
  *    + f4) / 2. rb_torsion.jl:30 uses dE/dth = (f1 sin th - 2 f2 sin 2th + 3 f3 sin 3th) / 2, which is minus that
  *    derivative, so its forces push up the energy; the magnitudes agree, the directions are reversed.
- *  - A torsion with three collinear atoms (a cross product of exactly zero) gets no force, for all three torsion kinds;
- *    the reference divides by zero there. */
+ *  - The bend angle of HarmonicAngle, CosineAngle and UreyBradley is theta = atan2(|ba x bc|, ba . bc). It is the
+ *    reference's angle (acos of the clamped cosine, bond_angle) computed with the same few-rounding-unit error at every
+ *    angle; acos loses most of its digits near 0 and pi, where linear groups (theta0 = pi) sit.
+ *  - Collinear angles and torsions (a cross product of exactly zero) keep their energy and get no force. For angles this is
+ *    the reference's behaviour (theta is exactly 0 or pi there). For all three torsion kinds the reference divides by zero
+ *    in the force. */
 enum { MB_SPECIFIC_HARMONIC_BOND = 0, MB_SPECIFIC_HARMONIC_ANGLE = 1, MB_SPECIFIC_PERIODIC_TORSION = 2,
        MB_SPECIFIC_POSITION_RESTRAINT = 3, MB_SPECIFIC_MORSE_BOND = 4, MB_SPECIFIC_FENE_BOND = 5, MB_SPECIFIC_COSINE_ANGLE = 6,
        MB_SPECIFIC_UREY_BRADLEY = 7, MB_SPECIFIC_HARMONIC_TORSION = 8, MB_SPECIFIC_RB_TORSION = 9, MB_SPECIFIC_N_KINDS = 10 };

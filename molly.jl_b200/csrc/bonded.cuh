@@ -123,11 +123,9 @@ __device__ __forceinline__ double angle_term(int t, int n, const int* __restrict
         Vec3<T> bc = mic(pos4[j], pos4[kk]);
         Vec3<T> nrm = cross(ba, bc);
         const T n2 = dot(nrm, nrm);
+        const T th = atan2(fsqrt(n2), dot(ba, bc));  // the angle of bond_angle, without acos's loss near 0 and pi
         if (n2 > (T)0) {
             const T nba = fsqrt(dot(ba, ba)), nbc = fsqrt(dot(bc, bc));
-            T cs = dot(ba, bc) / (nba * nbc);
-            cs = fmin(fmax(cs, (T)-1), (T)1);
-            const T th = acos(cs);
             Vec3<T> pa = cross(ba, nrm), pc = cross(-bc, nrm);
             pa = ((T)1 / fsqrt(dot(pa, pa))) * pa;
             pc = ((T)1 / fsqrt(dot(pc, pc))) * pc;
@@ -136,8 +134,8 @@ __device__ __forceinline__ double angle_term(int t, int n, const int* __restrict
             add_force<T>(f4, i, fa);
             add_force<T>(f4, kk, fc);
             add_force<T>(f4, j, -(fa + fc));
-            if (ENERGY) e = 0.5 * (double)k * (double)(th - th0) * (double)(th - th0);
         }
+        if (ENERGY) e = 0.5 * (double)k * (double)(th - th0) * (double)(th - th0);  // collinear too (harmonic_angle.jl:64-67)
     }
     return e;
 }
@@ -171,8 +169,8 @@ __device__ __forceinline__ double torsion_term(int t, int n, const int* __restri
             add_force<T>(f4, j, v - fi);
             add_force<T>(f4, k, -v - fl);
             add_force<T>(f4, l, fl);
-            if (ENERGY) e = (double)kk * (1.0 + cos((double)ang));
         }
+        if (ENERGY) e = (double)kk * (1.0 + cos((double)ang));  // collinear too (periodic_torsion.jl:131-141)
     }
     return e;
 }
@@ -250,8 +248,10 @@ __device__ __forceinline__ double fene_term(int t, int n, const int* __restrict_
     return e;
 }
 
-// bend geometry of atoms i-j-k (j in the middle): ba = x_i - x_j, bc = x_k - x_j, theta by acos (bond_angle,
-// src/spatial.jl:845-853); pa, pc the unit in-plane directions that open the angle, set only when not collinear
+// bend geometry of atoms i-j-k (j in the middle): ba = x_i - x_j, bc = x_k - x_j, theta = atan2(|ba x bc|, ba . bc), the
+// angle of bond_angle (src/spatial.jl:845-853) to a few rounding units at every angle, where acos of the cosine loses
+// digits near 0 and pi; exactly collinear atoms give exactly 0 or pi. pa, pc the unit in-plane directions that open the
+// angle, set only when not collinear
 template <typename T>
 struct Bend {
     Vec3<T> ba, bc, pa, pc;
@@ -266,9 +266,10 @@ __device__ __forceinline__ Bend<T> bend(const Mic<T, B>& mic, const typename VT<
     g.bc = mic(xj, xk);
     g.nba = fsqrt(dot(g.ba, g.ba));
     g.nbc = fsqrt(dot(g.bc, g.bc));
-    g.th = acos(fmin(fmax(dot(g.ba, g.bc) / (g.nba * g.nbc), (T)-1), (T)1));
     Vec3<T> nrm = cross(g.ba, g.bc);
-    g.bent = dot(nrm, nrm) > (T)0;
+    const T n2 = dot(nrm, nrm);
+    g.th = atan2(fsqrt(n2), dot(g.ba, g.bc));
+    g.bent = n2 > (T)0;
     if (g.bent) {
         g.pa = cross(g.ba, nrm);
         g.pc = cross(-g.bc, nrm);

@@ -5,8 +5,9 @@ the layout of mb_set_specific (include/mollyb200.h) and returns forces (n, 3) an
 
 Formulas: src/interactions/harmonic_position_restraint.jl:18-32, morse_bond.jl:24-38, fene_bond.jl:31-64,
 cosine_angle.jl:19-42, urey_bradley.jl:32-61, harmonic_torsion.jl:27-44, rb_torsion.jl:19-43; bond_angle and
-torsion_vectors (src/spatial.jl:845-894). RBTorsion's force is -grad E by default; reference_sign=True restates
-rb_torsion.jl:30 as written, whose dE/dtheta has the opposite sign."""
+torsion_vectors (src/spatial.jl:845-894), with the bend angle and the degenerate geometry of oracle/bonded.py.
+RBTorsion's force is -grad E by default; reference_sign=True restates rb_torsion.jl:30 as written, whose dE/dtheta has
+the opposite sign."""
 import numpy as np
 
 from oracle import bonded as bd
@@ -67,8 +68,7 @@ def _bend(x, box, idx):
     ba = _mic(x[idx[:, 0]] - x[idx[:, 1]], box)
     bc = _mic(x[idx[:, 2]] - x[idx[:, 1]], box)
     nba, nbc = np.linalg.norm(ba, axis=1), np.linalg.norm(bc, axis=1)
-    th = np.arccos(np.clip(np.sum(ba * bc, 1) / (nba * nbc), -1.0, 1.0))
-    n = np.cross(ba, bc)
+    th, n = bd.bend_angle(ba, bc)
     bent = np.sum(n * n, 1) > 0
     pa, pc = np.cross(ba, n), np.cross(-bc, n)
     with np.errstate(divide="ignore", invalid="ignore"):
@@ -118,9 +118,7 @@ def _torsion(x, box, idx):
 
 def _torsion_add(f, idx, geo, dedth):
     ab, bc, cd, m, n, nbc, _ = geo
-    fi = (dedth * nbc / np.sum(m * m, 1))[:, None] * m
-    fl = (-dedth * nbc / np.sum(n * n, 1))[:, None] * n
-    v = ((-np.sum(ab * bc, 1)) / nbc ** 2)[:, None] * fi - ((-np.sum(cd * bc, 1)) / nbc ** 2)[:, None] * fl
+    fi, fl, v = bd.torsion_arms(ab, bc, cd, m, n, nbc, dedth)
     for col, ff in zip(range(4), (fi, v - fi, -v - fl, fl)):
         np.add.at(f, idx[:, col], ff)
 
